@@ -2,7 +2,7 @@
 """bench.py — headline benchmark: local_laplacian (8 levels, alpha=1, beta=1) on synthetic uint16
 frames, Mpixels/s (1 Mpx = 1e6 output pixels W*H, channels not counted).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--dump-outputs DIR]
 
 Default workload = the north-star configuration of BASELINE.json: ONE 16384x16384x3 uint16 frame, levels=8,
 alpha=1/7 (the harness passes alpha/(levels-1), apps/local_laplacian/process.cpp:31), beta=1.  At N=1 the whole
@@ -14,6 +14,8 @@ input rows from its neighbours and gathers one coarse pyramid level (halide_b200
 One JSON line on stdout (rank 0).  `value` is device-resident throughput (inputs in HBM), timed with CUDA events on
 the launch stream over exactly K steps, max over ranks; `e2e` is the same metric through the C ABI with HOST
 (pinned) buffers, H2D + D2H inside the timed region, one caller thread (the same form at every N).
+`--dump-outputs DIR` writes the output frame of the last timed step to DIR (see dump_outputs); the inputs are seeded, so
+two builds run with the same arguments can be compared output for output.
 `--impl reference` times the CPU oracle (a port of the reference's algorithm — libHalide needs LLVM and cannot be
 built in this image) on the box's host cores for the same config, on a bounded sample of the frame.
 """
@@ -55,7 +57,7 @@ def make_config(workload, world):
     return {"workload": workload, "levels": LEVELS, "alpha": 1, "beta": 1, "frame": [W, H, 3],
             "frame_per_gpu": [W, H // world, 3],
             "parallelism": "single GPU" if world == 1 else f"one frame row-sharded x{world} (strong scaling): input-row halo exchange + one gathered pyramid level",
-            "l2": "frame pairs larger than the 126 MB L2 (rotating sets when one pair is not)",
+            "l2": "frame pairs larger than the 50 MB L2 (rotating sets when one pair is not)",
             "input": "uniform random uint16, worst case for the remap-table gathers"}
 
 
@@ -124,7 +126,7 @@ def measured_peak():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3, not a measured figure)"
 
 
 def recorded_traffic(workload, kernel):
@@ -187,6 +189,25 @@ def cpu_oracle_rate(W, H, budget_s=12.0, max_steps=8):
             "ms": best * 1e3, "published_reference": PUBLISHED_HALIDE_CPU}
 
 
+def dump_outputs(out_dir, out, name, max_bytes):
+    """Writes a (3, H, W) uint16 output frame of the device as float32 `DIR/<name>.npy`: the whole frame when it fits in
+    max_bytes, otherwise a fixed seeded sample of its elements (`<name>_sample.npy`) with their flat indices into the frame
+    (`<name>_sample_index.npy`, float64, exact below 2^53)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    flat = out.view(torch.int16).reshape(-1)
+    n = flat.numel()
+    if n * 4 <= max_bytes:
+        vals = (flat.to(torch.int32) & 0xFFFF).to(torch.float32).cpu().numpy().reshape(tuple(out.shape))
+        np.save(os.path.join(out_dir, f"{name}.npy"), vals)
+        return
+    idx = np.unique(np.random.default_rng(0).integers(0, n, max_bytes // 12, dtype=np.int64))
+    vals = (flat[torch.from_numpy(idx).to(flat.device)].to(torch.int32) & 0xFFFF).to(torch.float32).cpu().numpy()
+    np.save(os.path.join(out_dir, f"{name}_sample.npy"), vals)
+    np.save(os.path.join(out_dir, f"{name}_sample_index.npy"), idx.astype(np.float64))
+
+
 def run_reference(args, rank, world):
     """--impl reference: the reference's CPU algorithm (oracle port) on the host cores."""
     if rank != 0:
@@ -239,7 +260,7 @@ def run_ours(args, rank, world, local_rank):
     band_h = H // world          # strong scaling: the same frame, N bands
     dev = torch.device("cuda", local_rank)
     nbytes = 3 * band_h * W * 2
-    # rotate frame pairs so that the working set exceeds the 126 MB L2 (one pair is enough for big frames)
+    # rotate frame pairs so that the working set exceeds the 50 MB L2 (one pair is enough for big frames)
     NSETS = max(1, min(4, -(-300_000_000 // (2 * nbytes))))
     gen = torch.Generator(device=dev)
     gen.manual_seed(1234 + rank)
@@ -292,6 +313,10 @@ def run_ours(args, rank, world, local_rank):
     barrier()
     sampler.stop()
     launches = halide_b200.capi.halide_b200_kernel_launch_count() - n0
+    if args.dump_outputs:   # the last timed step's result, before the context passes below reuse the output buffers
+        # 48 MB for the whole run (each rank writes its own band), under the 64 MB a dump may take
+        dump_outputs(args.dump_outputs, outs[(args.steps - 1) % NSETS], "output" if world == 1 else f"output_rank{rank}",
+                     (48 << 20) // world)
     ms_total = e0.elapsed_time(e1)
     if dist is not None:
         tt = torch.tensor([ms_total], device=dev)
@@ -453,7 +478,7 @@ def run_ours(args, rank, world, local_rank):
             "config": cfg, "e2e": e2e,
             "gpu_launches": int(launches), "roofline": roofline, "cpu_baseline": cpu, "clocks": sampler.summary(),
             "kernels": kernels, "comm": comm, "host_enqueue_ms_per_step": host_enqueue_ms,
-            "l2_detail": f"rotating {NSETS} device-resident frame pair(s) per GPU ({NSETS * 2 * nbytes / 1e6:.0f} MB) > 126 MB L2",
+            "l2_detail": f"rotating {NSETS} device-resident frame pair(s) per GPU ({NSETS * 2 * nbytes / 1e6:.0f} MB) > 50 MB L2",
             "extra": {"smooth_frame_Mpixels_per_s": smooth_value,
                       "note": "same call on a low-frequency synthetic frame (coherent LUT / plane gathers); context only"}}
     print(json.dumps(line), flush=True)
@@ -468,7 +493,13 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default=DEFAULT_WORKLOAD, choices=sorted(WORKLOADS))
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's output frame to DIR as float32 output.npy, or, when the frame is larger than "
+                         "48 MB, a fixed seeded sample output_sample.npy with its flat indices output_sample_index.npy "
+                         "(output_rank<r>* per rank when row-sharded; 48 MB in all)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3)
     rank, world, local_rank = env_int("RANK", 0), env_int("WORLD_SIZE", 1), env_int("LOCAL_RANK", 0)
     if args.impl == "reference":

@@ -1,6 +1,6 @@
-"""halide_b200 — B200-native drop-in for Halide's canonical apps/ pipelines.
+"""halide_b200 — H100-native drop-in for Halide's canonical apps/ pipelines.
 
-The product is ``libhalide_b200.so``: hand-written sm_100a CUDA kernels behind the exact C ABI a
+The product is ``libhalide_b200.so``: hand-written sm_90a CUDA kernels behind the exact C ABI a
 Halide AOT filter exports (``int local_laplacian(halide_buffer_t*, int, float, float,
 halide_buffer_t*)`` ...; see ``include/*.h``).  This Python package is only the thin ctypes
 binding the tests and ``bench.py`` use to call that C ABI; it contains no compute and no

@@ -1,4 +1,4 @@
-// bilateral_grid.cu — bilateral_grid(input, r_sigma, output) for sm_100a (s_sigma = 8).
+// bilateral_grid.cu — bilateral_grid(input, r_sigma, output) for sm_90a (s_sigma = 8).
 //
 // Reference algorithm: apps/bilateral_grid/bilateral_grid_generator.cpp:17-67
 //   histogram(x,y,zi,c) += mux(c,{val,1}) over the 8x8 pixels of cell (x,y) (offset -4), zi = int(val/r_sigma + 0.5)
@@ -110,7 +110,7 @@ __global__ void __launch_bounds__(256) bg_blur_xy_kernel(BGParams p, int rows_pe
     if (y_begin >= y_end) return;
     // x-blur of one grid row at this thread's (cell, value): five loads, combined in the generator's order.  The loads of
     // two rows are issued together (ten in flight per thread): with one row per iteration the kernel sat on its own load
-    // latency (long-scoreboard 60 % of the stall samples, DRAM 19 %: profiles/r02_blur_bilateral_ncu_b.md).
+    // latency.
     struct Taps {
         float t[5];
     };
@@ -149,9 +149,8 @@ __global__ void __launch_bounds__(256) bg_blur_xy_kernel(BGParams p, int rows_pe
 // load.  Lane l of a warp owns the 4 pixels of cell (l & 15) at offset 4 * (l >> 4): the 16 lanes of a half-warp — the
 // unit an 8-byte shared load is served in — then read 16 DIFFERENT cells, and with a plane stride of 48 entries
 // (= 0 mod 16 bank pairs) the bank of a fetch depends on the cell only, never on the data-dependent plane zi: no
-// conflicts whatever the image.  (First version: corners gathered straight from L1, 92 % of the L1 data pipe.  Second:
-// shared memory, but lanes 2c and 2c+1 shared cell c, so on a noisy image — different zi — every fetch was a two-way
-// conflict: 58 % of the wavefronts, L1 data pipe 96 % busy, profiles/r02_other_pipelines_ncu.md.)
+// conflicts whatever the image.  (Lanes 2c and 2c+1 sharing cell c would make every fetch a two-way conflict on a noisy
+// image, where the two lanes' planes zi differ.)
 constexpr int kSliceW = 128, kSliceCells = 17, kSlicePitch = 24;
 
 __global__ void __launch_bounds__(256) bg_slice_kernel(BGParams p) {
@@ -223,8 +222,8 @@ const halide_filter_argument_t kArgs[3] = {
     {"r_sigma", halide_argument_kind_input_scalar, 0, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, &sv_rsigma, nullptr},
     {"bilateral_grid", halide_argument_kind_output_buffer, 2, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
-const halide_filter_metadata_t kMeta = {1, 3, kArgs, "x86-64-linux-cuda-cuda_capability_100-b200_native", "bilateral_grid"};
-const halide_filter_metadata_t kMetaAuto = {1, 3, kArgs, "x86-64-linux-cuda-cuda_capability_100-b200_native",
+const halide_filter_metadata_t kMeta = {1, 3, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "bilateral_grid"};
+const halide_filter_metadata_t kMetaAuto = {1, 3, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native",
                                             "bilateral_grid_auto_schedule"};
 
 inline int fdiv(int a, int b) {  // floor division, b > 0
@@ -300,7 +299,7 @@ int run_bilateral_grid(halide_buffer_t *input, float r_sigma, halide_buffer_t *o
         const int V = p.nz * 2;
         const int cols = (p.gw - 4) * V;
         int rows = 16;
-        while (rows > 2 && (int64_t)((cols + 255) / 256) * ((p.gh - 4 + rows - 1) / rows) < 148 * 4) rows >>= 1;
+        while (rows > 2 && (int64_t)((cols + 255) / 256) * ((p.gh - 4 + rows - 1) / rows) < 132 * 4) rows >>= 1;
         dim3 g2((cols + 255) / 256, (p.gh - 4 + rows - 1) / rows);
         HB_LAUNCH("bg_blur_xy", bg_blur_xy_kernel, g2, 256, 0, s, p, rows);
         const int tx0 = ox & ~(S - 1), ty0 = oy & ~(S - 1);

@@ -12,9 +12,9 @@
 // bottom with the last two blur_x rows in registers, several input rows in flight per lane":
 //   * blur3x3_u16_quad_kernel — frames whose rows keep pixel pairs 4-byte aligned (even row strides: the harness and
 //     RunGen frames): a lane owns 4 pixels, 32-bit loads, arithmetic in high-half form, ~10 instructions per pixel,
-//     strips sized to fill the resident warps a whole number of times.  29.8 us at 8K (68 % of the measured HBM peak).
+//     strips sized to fill the resident warps a whole number of times.
 //   * blur3x3_u16_kernel — any alignment: a lane owns 8 pixels, aligned 16-byte loads realigned by funnel shifts, the
-//     2-pixel horizontal apron from the neighbouring lane by shuffle.  Bound by the integer pipe (49 us at 8K).
+//     2-pixel horizontal apron from the neighbouring lane by shuffle.  Bound by the integer pipe.
 #include "hb_common.h"
 
 namespace {
@@ -150,7 +150,7 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) blur3x3_u16_kernel(BlurAr
 
 // ---- fast path: frames whose rows keep pixel pairs 4-byte aligned (even strides, aligned bases) ----------------------
 // The kernel above pays for arbitrary row misalignment with funnel shifts and selects and is bound by the integer
-// pipe, not by HBM (ALU 63 %, issue 66 %, DRAM 20 % at 8K: profiles/r02_other_pipelines_ncu.md).  When every row starts
+// pipe, not by HBM.  When every row starts
 // on an even element — the harness and RunGen frames do: dense rows of W + 2 with W even — a lane can own two aligned
 // pixel PAIRS (4 pixels): two 32-bit loads per row, the pair to its right from the next lane by shuffle (lane 31 loads
 // it), and all arithmetic in "high-half form" (a u16 value v held as v << 16): 32-bit adds of such values wrap mod 2^16
@@ -298,7 +298,7 @@ const halide_filter_argument_t kArgs[2] = {
     {"input", halide_argument_kind_input_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
     {"blur_y", halide_argument_kind_output_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
 };
-const halide_filter_metadata_t kMeta = {1, 2, kArgs, "x86-64-linux-cuda-cuda_capability_100-b200_native", "halide_blur"};
+const halide_filter_metadata_t kMeta = {1, 2, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "halide_blur"};
 
 }  // namespace
 
@@ -349,11 +349,11 @@ extern "C" int halide_blur(halide_buffer_t *input, halide_buffer_t *blur_y) {
     a.in_lo = lo - origin;
     a.in_hi = hi - origin;
 
-    // Enough warps to cover 148 SMs a few times over, but strips tall enough to amortise the
+    // Enough warps to cover the 132 SMs of an H100 a few times over, but strips tall enough to amortise the
     // two-row vertical apron.
     int strips_x = (w + kStripW - 1) / kStripW;
     int rows = 32;
-    while (rows > 4 && (int64_t)strips_x * ((h + rows - 1) / rows) < 148 * 8) rows >>= 1;
+    while (rows > 4 && (int64_t)strips_x * ((h + rows - 1) / rows) < 132 * 8) rows >>= 1;
     a.rows_per_warp = rows;
     int warps_y = (h + rows - 1) / rows;
     dim3 grid(strips_x, (warps_y + kWarpsPerBlock - 1) / kWarpsPerBlock);
@@ -366,14 +366,13 @@ extern "C" int halide_blur(halide_buffer_t *input, halide_buffer_t *blur_y) {
         hb::CallTimer timer(s);
         if (pair_ok) {
             // strips of 128 columns; height such that the strips fill the resident warps a whole number of times
-            // (six rows in flight per lane: nine — 86 registers, five blocks per SM — measured slower, 33.5 vs 29.3 us at 8K)
             static int resident = 0;  // blocks per SM x SMs (per process: one device per process)
             if (!resident) {
                 int per_sm = 0, dev = 0, sms = 0;
                 cudaGetDevice(&dev);
                 cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
                 cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, blur3x3_u16_quad_kernel<6>, 32 * kQuadWarps, 0);
-                resident = (per_sm > 0 ? per_sm : 8) * (sms > 0 ? sms : 148);
+                resident = (per_sm > 0 ? per_sm : 8) * (sms > 0 ? sms : 132);
             }
             const int sxq = (w + kQuadW - 1) / kQuadW;
             const int64_t slots = (int64_t)resident * kQuadWarps;

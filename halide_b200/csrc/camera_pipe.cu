@@ -1,5 +1,5 @@
 // camera_pipe.cu — camera_pipe(input, matrix_3200, matrix_7000, color_temp, gamma, contrast,
-// sharpen_strength, blackLevel, whiteLevel, processed) for sm_100a.
+// sharpen_strength, blackLevel, whiteLevel, processed) for sm_90a.
 //
 // Reference algorithm: apps/camera_pipe/camera_pipe_generator.cpp — shift(16,12) :412, hot-pixel suppression
 // :240-249, GRBG deinterleave :251-261, gradient-directed demosaic :57-146, 3x4 Q8.8 colour matrix :263-295,
@@ -255,8 +255,8 @@ const halide_filter_argument_t kArgs[10] = {
     {"whiteLevel", halide_argument_kind_input_scalar, 0, {halide_type_int, 32, 0}, nullptr, nullptr, nullptr, &sv[5], nullptr},
     {"processed", halide_argument_kind_output_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, est_out_p},
 };
-const halide_filter_metadata_t kMeta = {1, 10, kArgs, "x86-64-linux-cuda-cuda_capability_100-b200_native", "camera_pipe"};
-const halide_filter_metadata_t kMetaAuto = {1, 10, kArgs, "x86-64-linux-cuda-cuda_capability_100-b200_native",
+const halide_filter_metadata_t kMeta = {1, 10, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "camera_pipe"};
+const halide_filter_metadata_t kMetaAuto = {1, 10, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native",
                                             "camera_pipe_auto_schedule"};
 
 inline int fdiv(int a, int b) {

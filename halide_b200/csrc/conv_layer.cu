@@ -1,4 +1,4 @@
-// conv_layer.cu — conv_layer(input, filter, bias, relu) for sm_100a.
+// conv_layer.cu — conv_layer(input, filter, bias, relu) for sm_90a.
 //
 // Reference algorithm: apps/conv_layer/conv_layer_generator.cpp:17-27 with the fixed shapes the generator pins
 // by constraints (:35-50): input (CI=128, W+2=102, H+2=82, N=5) channel-innermost, filter (CO=128, 3, 3, CI)
@@ -7,8 +7,8 @@
 // Float pipeline: parity bar 1e-4 relative against oracle/oracle_conv_layer.cpp (a tiled contraction necessarily
 // changes the summation order; the harness data are all positive so there is no cancellation).
 //
-// This round ships the FP32 SIMT contraction (register-tiled implicit GEMM, FFMA): M = 40 000 output pixels,
-// N = 128, K = 1152, 11.8 GFLOP.  It is the baseline the tcgen05 path has to beat (DESIGN.md §9): TF32 tensor
+// Two contractions: the tensor-core implicit GEMM of conv_layer_tc.cu (the default) and this FP32 SIMT kernel
+// (register-tiled implicit GEMM, FFMA): M = 40 000 output pixels, N = 128, K = 1152, 11.8 GFLOP.  TF32 tensor
 // cores need a 3-term split to hold 1e-4 on rand()-scale inputs because the conversion truncates.
 // Block = 10x8 output pixels x 128 output channels, 256 threads, each thread 5 pixels x 8 channels in registers;
 // per (ci-chunk of 32, ky, kx) one 16 KB filter slab is staged in shared memory; the input patch (12x10 pixels
@@ -18,12 +18,12 @@
 
 #include "hb_common.h"
 
-// tcgen05 / TMEM / TMA implementation (conv_layer_tc.cu)
+// wgmma / TMA implementation (conv_layer_tc.cu)
 int conv_layer_tc_run(const float *din, const float *df, const float *db, float *dout, cudaStream_t s);
 
 namespace {
 
-// Which contraction runs: the tcgen05 implicit GEMM (3xTF32 split) or the FP32 SIMT kernel.  HALIDE_B200_CONV=simt|tc
+// Which contraction runs: the wgmma implicit GEMM (3xTF32 split) or the FP32 SIMT kernel.  HALIDE_B200_CONV=simt|tc
 // picks at start-up; halide_b200_conv_use_tensor_cores() switches at run time (tests cover both).
 bool g_use_tc = [] {
     const char *e = getenv("HALIDE_B200_CONV");
@@ -120,8 +120,8 @@ const halide_filter_argument_t kArgs[4] = {
     {"bias", halide_argument_kind_input_buffer, 1, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_b},
     {"relu", halide_argument_kind_output_buffer, 4, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_out},
 };
-const halide_filter_metadata_t kMeta = {1, 4, kArgs, "x86-64-linux-cuda-cuda_capability_100-b200_native", "conv_layer"};
-const halide_filter_metadata_t kMetaAuto = {1, 4, kArgs, "x86-64-linux-cuda-cuda_capability_100-b200_native",
+const halide_filter_metadata_t kMeta = {1, 4, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "conv_layer"};
+const halide_filter_metadata_t kMetaAuto = {1, 4, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native",
                                             "conv_layer_auto_schedule"};
 
 struct Shape {

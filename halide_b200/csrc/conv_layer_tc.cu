@@ -1,4 +1,4 @@
-// conv_layer_tc.cu — conv_layer's dense contraction on the 5th-generation tensor cores (tcgen05 + TMEM + TMA).
+// conv_layer_tc.cu — conv_layer's dense contraction on the Hopper tensor cores (wgmma + TMA + mbarrier).
 //
 // Same contract as conv_layer.cu (apps/conv_layer/conv_layer_generator.cpp:17-50); this is the only pipeline of the
 // seven whose hot loop is GEMM-shaped: M = output pixels, N = 128 output channels, K = 3*3*128.
@@ -8,19 +8,16 @@
 // row feeding output q at tap (ky,kx) is simply q + ky*102 + kx: every tap is the same 2-D tile shifted by a constant
 // number of rows, so the implicit-GEMM A operand of a 128-pixel tile is one TMA box load per (tap, 32-channel chunk)
 // — no im2col.  The filter is re-laid once per call as Bt[(ky*3+kx)*128 + co][ci] (K-major).
-// Precision.  kind::tf32 reads 10 mantissa bits, not enough for the 1e-4 bar on rand()-scale data (SURVEY.md R8), so
-// both operands are split hi = tf32(x), lo = x - hi and three products are accumulated (hi*hi + hi*lo + lo*hi) into the
-// same fp32 TMEM accumulator: relative error ~2^-19 per product.
+// Precision.  TF32 MMAs read 10 mantissa bits, not enough for the 1e-4 bar on rand()-scale data (SURVEY.md R8), so
+// both operands are split hi = tf32(x), lo = x - hi and three products are accumulated (hi*hi + hi*lo + lo*hi) into
+// fp32 accumulators: relative error ~2^-19 per product.
 //
-// Kernel: one CTA per (128-pixel tile, image), 192 threads, warp-specialised:
-//   warp 0   TMA producer: per K step 4 box loads (A_hi, A_lo, B_hi, B_lo: 128 rows x 32 floats, SWIZZLE_128B) into a
-//            3-stage shared-memory ring, mbarrier complete_tx
-//   warp 1   TMEM allocation (4 x 128 columns) and MMA issue: one elected lane, 4 x 3 tcgen05.mma (M128 N128 K8) per stage,
-//            tcgen05.commit -> the stage's "empty" barrier / the accumulator's "full" barrier
-//   warps 2-5 epilogue: tcgen05.ld (32 lanes x 32 columns per instruction), + bias, relu, 128-byte row stores
+// Kernel: one CTA per (128-pixel tile, image), 288 threads, warp-specialised:
+//   warp 8       TMA producer: per K step 4 box loads (A_hi, A_lo, B_hi, B_lo: rows x 32 floats, SWIZZLE_128B) into a
+//                3-stage shared-memory ring, mbarrier complete_tx
+//   warps 0-7    two consumer warpgroups, one per 64-pixel half of the tile: 4 x 3 wgmma.m64n128k8 (TF32, both operands
+//                from shared memory) per stage into register accumulators, then + bias, relu and the stores
 #include <cuda.h>
-#include <stdlib.h>
-
 #include "hb_common.h"
 
 namespace {
@@ -29,21 +26,16 @@ constexpr int N = 5, CI = 128, CO = 128, W = 100, H = 80;
 constexpr int WP = W + 2, HP = H + 2;
 constexpr int ROWS_PER_IMAGE = HP * WP;          // 8364 input rows per image
 constexpr int A_ROWS = N * ROWS_PER_IMAGE;       // 41820
-constexpr int TILE_M = 128, TILE_K = 32;  // 32 tf32 = 128 bytes = one swizzle row; the N tile is a template parameter (64 or 128)
+constexpr int TILE_M = 128, TILE_N = CO, TILE_K = 32;  // 32 tf32 = 128 bytes = one swizzle row
 constexpr int TILES_PER_IMAGE = (H * WP + TILE_M - 1) / TILE_M;  // 64 (outputs enumerated over the padded width)
 constexpr int K_STEPS = 9 * (CI / TILE_K);       // 36
 constexpr int STAGES = 3;
+constexpr int CONSUMER_WARPS = 8;                // two warpgroups of 64 output pixels each
+constexpr int THREADS = (CONSUMER_WARPS + 1) * 32;
 constexpr int A_TILE_BYTES = TILE_M * TILE_K * 4;  // 16 KB
-constexpr int ACCS = 4;                          // partial accumulators (see the MMA issuer)
-template<int NT> struct Cfg {
-    static constexpr int B_TILE_BYTES = NT * TILE_K * 4;
-    static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;  // A_hi, A_lo, B_hi, B_lo
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*alignment slack*/ + 256 /*barriers*/;
-    static constexpr uint32_t TMEM_COLS = ACCS * NT;  // 512 (the whole tensor memory of the SM) or 256
-    static constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(NT >> 3) << 17) | ((uint32_t)(TILE_M >> 4) << 24);
-};
-// instruction descriptor (cute/arch/mma_sm100_desc.hpp: InstrDescriptor): c=F32 [4,6)=1, a=TF32 [7,10)=2, b=TF32 [10,13)=2,
-// a/b K-major (bits 15,16 = 0), N>>3 at [17,23), M>>4 at [24,29)
+constexpr int B_TILE_BYTES = TILE_N * TILE_K * 4;  // 16 KB
+constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;  // A_hi, A_lo, B_hi, B_lo
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*alignment slack*/ + 256 /*barriers*/;
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -52,6 +44,9 @@ __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
     asm volatile(
@@ -67,22 +62,27 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, u
                  "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
                  : "memory");
 }
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp: SmemDescriptor): start address >> 4,
-// LBO = 1 (unused for swizzled K-major), SBO = 1024 B between 8-row groups, version 1 (Blackwell), layout type 2.
-__device__ __forceinline__ uint64_t umma_desc(const void *tile) {
-    return (uint64_t)((smem_u32(tile) & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
+// K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma (PTX ISA "Matrix Descriptor Format"): start address >> 4
+// in [0,14), leading byte offset (unused for swizzled K-major, 1) in [16,30), stride byte offset 1024 B between 8-row
+// groups in [32,46), layout type 1 = 128-byte swizzle in [62,64).  The tile base must be 1024-byte aligned.
+__device__ __forceinline__ uint64_t wgmma_desc(const void *tile) {
+    return (uint64_t)((smem_u32(tile) & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t accumulate, uint32_t IDESC) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}" ::"r"(tmem_d),
-        "l"(a_desc), "l"(b_desc), "r"(IDESC), "r"(accumulate), "r"(0u)
-        : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template<int PENDING>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+
+#define HB_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+// d[64] += A(64 x 8, tf32) * B(8 x 128, tf32)^T, both K-major in shared memory.  Accumulator fragment of thread t of the
+// warpgroup: d[4j + {0,1}] = (row 16*(t/32) + (t%32)/4, columns 8j + 2*(t%4) + {0,1}), d[4j + {2,3}] = the same 8 rows down.
+__device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, 1, 1, 1;"
+                 : HB_D8(0), HB_D8(8), HB_D8(16), HB_D8(24), HB_D8(32), HB_D8(40), HB_D8(48), HB_D8(56)
+                 : "l"(a_desc), "l"(b_desc)
+                 : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
+#undef HB_D8
 
 // ---- operand preparation ----------------------------------------------------------------------------------------------
 __global__ void conv_split_input_kernel(const float4 *__restrict__ in, float4 *__restrict__ hi, float4 *__restrict__ lo, size_t n4) {
@@ -109,21 +109,38 @@ __global__ void conv_prep_filter_kernel(const float *__restrict__ f, float *__re
 }
 
 // ---- the GEMM ---------------------------------------------------------------------------------------------------------
-template<int NT>
-__global__ void __launch_bounds__(192, 1) conv_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
-                                                               const __grid_constant__ CUtensorMap map_a_lo,
-                                                               const __grid_constant__ CUtensorMap map_b_hi,
-                                                               const __grid_constant__ CUtensorMap map_b_lo,
-                                                               const float *__restrict__ bias, float *__restrict__ out) {
-    constexpr int TILE_N = NT, TILE_BYTES = A_TILE_BYTES, STAGE_BYTES = Cfg<NT>::STAGE_BYTES;
-    constexpr uint32_t TMEM_COLS = Cfg<NT>::TMEM_COLS, IDESC = Cfg<NT>::IDESC;
-    const int n0 = blockIdx.z * NT;  // first output channel of this CTA
+// One K step (32 input channels of one tap) of one consumer warpgroup into accumulator d; releases the stage of the
+// previous K step once the MMAs that read it have completed.
+__device__ __forceinline__ void consume_step(float (&d)[64], const uint8_t *tiles, uint64_t *full_bar, uint64_t *empty_bar, int it, int wg,
+                                             int lane) {
+    const int s = it % STAGES;
+    mbar_wait(&full_bar[s], (it / STAGES) & 1);
+    const uint8_t *st = tiles + s * STAGE_BYTES;
+    const int a_off = wg * 64 * TILE_K * 4;  // this warpgroup's 64 rows of the A tiles (8 KB, a multiple of the 1024-byte swizzle atom)
+    const uint64_t a_hi = wgmma_desc(st + a_off), a_lo = wgmma_desc(st + A_TILE_BYTES + a_off);
+    const uint64_t b_hi = wgmma_desc(st + 2 * A_TILE_BYTES), b_lo = wgmma_desc(st + 2 * A_TILE_BYTES + B_TILE_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < TILE_K / 8; k++) {  // K = 8 tf32 = 32 bytes per MMA: advance the start addresses by 2 (16-byte units)
+        const uint64_t adv = (uint64_t)(2 * k);
+        wgmma_m64n128k8_tf32(d, a_hi + adv, b_hi + adv);
+        wgmma_m64n128k8_tf32(d, a_hi + adv, b_lo + adv);
+        wgmma_m64n128k8_tf32(d, a_lo + adv, b_hi + adv);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();  // the previous K step's MMAs are done: its stage can be refilled
+    if (it > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+}
+
+__global__ void __launch_bounds__(THREADS, 1) conv_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
+                                                                   const __grid_constant__ CUtensorMap map_a_lo,
+                                                                   const __grid_constant__ CUtensorMap map_b_hi,
+                                                                   const __grid_constant__ CUtensorMap map_b_lo,
+                                                                   const float *__restrict__ bias, float *__restrict__ out) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *tiles = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);  // SWIZZLE_128B needs 1024-byte alignment
     uint64_t *full_bar = (uint64_t *)(tiles + STAGES * STAGE_BYTES);
     uint64_t *empty_bar = full_bar + STAGES;
-    uint64_t *acc_bar = empty_bar + STAGES;
-    uint32_t *tmem_slot = (uint32_t *)(acc_bar + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x, img = blockIdx.y;
@@ -132,21 +149,13 @@ __global__ void __launch_bounds__(192, 1) conv_layer_tc_kernel(const __grid_cons
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; s++) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], CONSUMER_WARPS);  // one arrival per consumer warp
         }
-        mbar_init(acc_bar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {  // TMEM allocation is a warp-wide operation; the same warp frees it at the end
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == CONSUMER_WARPS) {
         if (lane == 0) {
             // ===== TMA producer =====
             for (int it = 0; it < K_STEPS; it++) {
@@ -156,83 +165,46 @@ __global__ void __launch_bounds__(192, 1) conv_layer_tc_kernel(const __grid_cons
                 const int ky = tap / 3, kx = tap - ky * 3;
                 uint8_t *st = tiles + s * STAGE_BYTES;
                 mbar_expect_tx(&full_bar[s], STAGE_BYTES);
-                tma_load_2d(st + 0 * TILE_BYTES, &map_a_hi, &full_bar[s], kc * TILE_K, a_row0 + ky * WP + kx);
-                tma_load_2d(st + 1 * TILE_BYTES, &map_a_lo, &full_bar[s], kc * TILE_K, a_row0 + ky * WP + kx);
-                tma_load_2d(st + 2 * TILE_BYTES, &map_b_hi, &full_bar[s], kc * TILE_K, tap * CO + n0);
-                tma_load_2d(st + 2 * TILE_BYTES + Cfg<NT>::B_TILE_BYTES, &map_b_lo, &full_bar[s], kc * TILE_K, tap * CO + n0);
+                tma_load_2d(st, &map_a_hi, &full_bar[s], kc * TILE_K, a_row0 + ky * WP + kx);
+                tma_load_2d(st + A_TILE_BYTES, &map_a_lo, &full_bar[s], kc * TILE_K, a_row0 + ky * WP + kx);
+                tma_load_2d(st + 2 * A_TILE_BYTES, &map_b_hi, &full_bar[s], kc * TILE_K, tap * CO);
+                tma_load_2d(st + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_b_lo, &full_bar[s], kc * TILE_K, tap * CO);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ===== MMA issuer =====
-            for (int it = 0; it < K_STEPS; it++) {
-                const int s = it % STAGES, round = it / STAGES;
-                mbar_wait(&full_bar[s], round & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint8_t *st = tiles + s * STAGE_BYTES;
-                const uint64_t a_hi = umma_desc(st + 0 * TILE_BYTES), a_lo = umma_desc(st + 1 * TILE_BYTES);
-                const uint64_t b_hi = umma_desc(st + 2 * TILE_BYTES), b_lo = umma_desc(st + 2 * TILE_BYTES + Cfg<NT>::B_TILE_BYTES);
-                // The tensor core adds into the fp32 accumulator with truncation; 432 chained adds biased the result by
-                // ~-2.5e-5 relative (measured).  Four partial accumulators (K steps round-robin) cut the chain to 108 adds
-                // each; the epilogue sums them in round-to-nearest.
-                const uint32_t acc = tmem_base + (uint32_t)((it % ACCS) * TILE_N);
-#pragma unroll
-                for (int k = 0; k < TILE_K / 8; k++) {  // UMMA_K = 8 tf32 = 32 bytes: advance the start address by 2 (16-byte units)
-                    const uint64_t adv = (uint64_t)(2 * k);
-                    umma_tf32(acc, a_hi + adv, b_hi + adv, (it >= ACCS) || (k != 0), IDESC);
-                    umma_tf32(acc, a_hi + adv, b_lo + adv, 1, IDESC);
-                    umma_tf32(acc, a_lo + adv, b_hi + adv, 1, IDESC);
-                }
-                umma_commit(&empty_bar[s]);  // frees the stage once these MMAs have consumed it
-            }
-            umma_commit(acc_bar);  // accumulator complete
-        }
-    } else {
-        // ===== epilogue: warps 2..5 own TMEM lanes 32*(warp%4) .. +31 =====
-        mbar_wait(acc_bar, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int lane_base = 32 * (warp & 3);
-        const int q = tile * TILE_M + lane_base + lane;  // output index over the padded width
-        const int y = q / WP, x = q - y * WP;
-        const bool valid = (y < H) && (x < W);
-        float *orow = out + (((size_t)img * H + y) * W + x) * CO;
-#pragma unroll 1
-        for (int c0 = 0; c0 < TILE_N; c0 += 32) {
-            float r[32];
-#pragma unroll
-            for (int a = 0; a < ACCS; a++) {
-                uint32_t t[32];
-                const uint32_t taddr = tmem_base + ((uint32_t)lane_base << 16) + (uint32_t)(a * TILE_N + c0);
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, "
-                    "%20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(t[0]), "=r"(t[1]), "=r"(t[2]), "=r"(t[3]), "=r"(t[4]), "=r"(t[5]), "=r"(t[6]), "=r"(t[7]), "=r"(t[8]), "=r"(t[9]),
-                      "=r"(t[10]), "=r"(t[11]), "=r"(t[12]), "=r"(t[13]), "=r"(t[14]), "=r"(t[15]), "=r"(t[16]), "=r"(t[17]), "=r"(t[18]),
-                      "=r"(t[19]), "=r"(t[20]), "=r"(t[21]), "=r"(t[22]), "=r"(t[23]), "=r"(t[24]), "=r"(t[25]), "=r"(t[26]), "=r"(t[27]),
-                      "=r"(t[28]), "=r"(t[29]), "=r"(t[30]), "=r"(t[31])
-                    : "r"(taddr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                for (int j = 0; j < 32; j++) r[j] = a == 0 ? __uint_as_float(t[j]) : r[j] + __uint_as_float(t[j]);
-            }
-            if (valid) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    float4 b = __ldg(reinterpret_cast<const float4 *>(bias + n0 + c0 + j));
-                    float4 v;
-                    v.x = fmaxf(r[j] + b.x, 0.f);
-                    v.y = fmaxf(r[j + 1] + b.y, 0.f);
-                    v.z = fmaxf(r[j + 2] + b.z, 0.f);
-                    v.w = fmaxf(r[j + 3] + b.w, 0.f);
-                    *reinterpret_cast<float4 *>(orow + n0 + c0 + j) = v;
-                }
-            }
-        }
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
+
+    // ===== consumers: warpgroup wg owns output rows 64*wg .. 64*wg+63 of the tile =====
+    const int wg = warp >> 2;
+    // Two accumulators, K steps alternating between them, summed in round-to-nearest at the end: the tensor core's own
+    // fp32 accumulation does not round to nearest, and halving the chain of 432 MMA additions halves that bias.
+    float acc0[64], acc1[64];
+#pragma unroll
+    for (int j = 0; j < 64; j++) acc0[j] = acc1[j] = 0.f;
+#pragma unroll 1
+    for (int it = 0; it < K_STEPS; it += 2) {
+        consume_step(acc0, tiles, full_bar, empty_bar, it, wg, lane);
+        consume_step(acc1, tiles, full_bar, empty_bar, it + 1, wg, lane);
+    }
+    wgmma_wait<0>();
+
+    // ===== epilogue: + bias, relu, float2 stores of the valid pixels =====
+    const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        const int q = tile * TILE_M + r0 + 8 * h;  // output index over the padded width
+        const int y = q / WP, x = q - y * WP;
+        if (y >= H || x >= W) continue;
+        float *orow = out + (((size_t)img * H + y) * W + x) * CO;
+#pragma unroll
+        for (int j = 0; j < TILE_N / 8; j++) {
+            const int c = 8 * j + 2 * (lane & 3);
+            const float2 b = __ldg(reinterpret_cast<const float2 *>(bias + c));
+            float2 v;
+            v.x = fmaxf((acc0[4 * j + 2 * h] + acc1[4 * j + 2 * h]) + b.x, 0.f);
+            v.y = fmaxf((acc0[4 * j + 2 * h + 1] + acc1[4 * j + 2 * h + 1]) + b.y, 0.f);
+            *reinterpret_cast<float2 *>(orow + c) = v;
+        }
     }
 }
 
@@ -269,31 +241,17 @@ int conv_layer_tc_run(const float *din, const float *df, const float *db, float 
     float *a_hi = scratch.get<float>(a_elems), *a_lo = scratch.get<float>(a_elems);
     float *b_hi = scratch.get<float>(b_elems), *b_lo = scratch.get<float>(b_elems);
     if (!a_hi || !a_lo || !b_hi || !b_lo) return hb::fail(halide_error_code_device_malloc_failed, "conv_layer: scratch allocation failed");
-    // Tile width: 128x128 (320 CTAs, 2.16 waves) measured 84.7 us per call; 128x64 (640 CTAs, 4.3 waves, selectable with
-    // HALIDE_B200_CONV_NT=64) removes the tail wave but measured 114.5 us — the narrower MMA re-reads A twice from shared memory.
-    static const int nt = [] {
-        const char *e = getenv("HALIDE_B200_CONV_NT");
-        return (e && atoi(e) == 64) ? 64 : 128;
-    }();
     CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
     if (make_map(enc, &ma_hi, a_hi, A_ROWS, TILE_M) || make_map(enc, &ma_lo, a_lo, A_ROWS, TILE_M) ||
-        make_map(enc, &mb_hi, b_hi, 9 * CO, nt) || make_map(enc, &mb_lo, b_lo, 9 * CO, nt)) {
+        make_map(enc, &mb_hi, b_hi, 9 * CO, TILE_N) || make_map(enc, &mb_lo, b_lo, 9 * CO, TILE_N)) {
         return hb::fail(halide_error_code_generic_error, "conv_layer: cuTensorMapEncodeTiled failed");
     }
     static hb::PerDeviceOnce attr;
-    attr.run([] {
-        cudaFuncSetAttribute(conv_layer_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::SMEM_BYTES);
-        cudaFuncSetAttribute(conv_layer_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::SMEM_BYTES);
-    });
+    attr.run([] { cudaFuncSetAttribute(conv_layer_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES); });
     HB_LAUNCH("conv_split_input", conv_split_input_kernel, (unsigned)((a_elems / 4 + 255) / 256), 256, 0, s, (const float4 *)din, (float4 *)a_hi,
               (float4 *)a_lo, a_elems / 4);
     HB_LAUNCH("conv_prep_filter", conv_prep_filter_kernel, (unsigned)((b_elems + 255) / 256), 256, 0, s, df, b_hi, b_lo);
-    if (nt == 64) {
-        HB_LAUNCH("conv_layer_tc", conv_layer_tc_kernel<64>, dim3(TILES_PER_IMAGE, N, 2), 192, Cfg<64>::SMEM_BYTES, s, ma_hi, ma_lo, mb_hi,
-                  mb_lo, db, dout);
-    } else {
-        HB_LAUNCH("conv_layer_tc", conv_layer_tc_kernel<128>, dim3(TILES_PER_IMAGE, N, 1), 192, Cfg<128>::SMEM_BYTES, s, ma_hi, ma_lo, mb_hi,
-                  mb_lo, db, dout);
-    }
+    HB_LAUNCH("conv_layer_tc", conv_layer_tc_kernel, dim3(TILES_PER_IMAGE, N), THREADS, SMEM_BYTES, s, ma_hi, ma_lo, mb_hi, mb_lo, db,
+              dout);
     return 0;
 }

@@ -1,5 +1,5 @@
 // hb_runtime.cu — the slice of the Halide runtime that the AOT filters and the reference
-// harnesses call, rebuilt on the CUDA runtime API for a single B200 per process.
+// harnesses call, rebuilt on the CUDA runtime API for a single GPU per process.
 //
 // Replaces (behaviour, not code): src/runtime/cuda.cpp (device malloc/free pool :760-870, copies
 // :884-1017, sync), src/runtime/device_interface.cpp (dirty-bit protocol :30-56,154-205),
@@ -780,7 +780,7 @@ uint64_t halide_b200_kernel_launch_count(void) {
     return g_launches.load();
 }
 const char *halide_b200_target(void) {
-    return "x86-64-linux-cuda-cuda_capability_100-b200_native";
+    return "x86-64-linux-cuda-cuda_capability_90-h100_native";
 }
 
 void halide_b200_set_timing(int enable) {

@@ -1,4 +1,4 @@
-// local_laplacian.cu — host side of local_laplacian(input, levels, alpha, beta, output) for sm_100a:
+// local_laplacian.cu — host side of local_laplacian(input, levels, alpha, beta, output) for sm_90a:
 // the C-ABI entry points (reference: apps/local_laplacian/local_laplacian_generator.cpp:12-16,287 and
 // the harness apps/local_laplacian/process.cpp:31), argument validation, pyramid geometry, scratch
 // allocation, the launch sequence, and the row-sharded multi-GPU variant.  Kernels: ll_kernels.cuh.
@@ -51,8 +51,8 @@ const halide_filter_argument_t kArgs[5] = {
     {"beta", halide_argument_kind_input_scalar, 0, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, &sv_beta, nullptr},
     {"output", halide_argument_kind_output_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
-const halide_filter_metadata_t kMeta = {1, 5, kArgs, "x86-64-linux-cuda-cuda_capability_100-b200_native", "local_laplacian"};
-const halide_filter_metadata_t kMetaAuto = {1, 5, kArgs, "x86-64-linux-cuda-cuda_capability_100-b200_native",
+const halide_filter_metadata_t kMeta = {1, 5, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "local_laplacian"};
+const halide_filter_metadata_t kMetaAuto = {1, 5, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native",
                                             "local_laplacian_auto_schedule"};
 
 
@@ -202,7 +202,7 @@ const dim3 kBlk(32, 8);
 dim3 grid_for(int w, int h) { return dim3((w + 31) / 32, (h + 7) / 8); }
 
 // Resident block slots of a kernel on the current device.  The driver queries behind it (function attribute,
-// occupancy) cost several microseconds each — at eight ranks a whole frame is ~0.8 ms of GPU time and ~17 launches — so
+// occupancy) cost several microseconds each — a sharded frame is only ~17 short launches per rank — so
 // the answer is cached per (kernel, device, shared-memory size); a process may drive several devices.
 struct SlotKey {
     const void *kern;
@@ -223,7 +223,7 @@ int resident_slots(Kern kern, int threads, size_t smem) {
     std::lock_guard<std::mutex> lock(g_slots_mu);
     auto it = g_slots.find(key);
     if (it != g_slots.end()) return it->second;
-    int sms = 148, per_sm = 0;
+    int sms = 132, per_sm = 0;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem) != cudaSuccess || per_sm < 1) {
@@ -303,9 +303,8 @@ void launch_final(Plan &p, cudaStream_t s) {
     if (p.f.nrows <= 0) return;
     if (p.J > 1 && p.K == 8 && !(g_force_naive & 4) && p.f.C <= 3) {
         const LLFrame &f = p.f;
-        // 48-row tiles (hook bit 256) were measured SLOWER than 32-row tiles although they spread the per-block fixed work
-        // over 6 rows per thread instead of 4 (16K: 1.63 vs 1.52 ms, 4K: 61.9 vs 57.8 us): the kernel wants the fourth block
-        // per SM more than it wants fewer instructions.  Kept selectable for A/B runs (tools/ab_masks.py) and tested.
+        // 48-row tiles (hook bit 256) spread the per-block fixed work over 6 rows per thread instead of 4 at the cost of
+        // the fourth block per SM; 32-row tiles are the default.  Kept selectable for A/B runs (tools/ab_masks.py) and tested.
         const bool tall = (g_force_naive & 256) && !(g_force_naive & 128);
         const int th = tall ? kUpTHTall : kUpTH;
         // the common layout takes the kernel's ALIGNED path (32-bit addressing, one aligned word per thread and channel)
@@ -364,7 +363,7 @@ bool launch_coarse_fused(Plan &p, int j0, cudaStream_t s) {
         }
     }
     const int slots = resident_slots(ll_coarse_fused_kernel, 256, 0);  // sms * blocks per SM
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int max_blocks = coop ? (slots > 2 * sms ? 2 * sms : slots) : 0;
     if (max_blocks <= 0) return false;
@@ -383,9 +382,6 @@ bool launch_coarse_fused(Plan &p, int j0, cudaStream_t s) {
 
 // Levels from_level+1 .. J-1 down, then J-1 .. from_level+1 up: the part of the sweep that runs on whole levels
 // (everything on one GPU; the replicated coarse levels when row-sharded).  Small levels share one cooperative launch.
-// (Tried and dropped: the levels of <= 12 K pixels as one 8-CTA thread-block cluster with hardware cluster barriers
-// instead of grid barriers — 41 us against 35 us for the cooperative kernel at 4K: eight SMs' worth of threads cannot
-// cover the L2 latency of these phases, the barriers were not the cost.)
 void run_coarse_sweep(Plan &p, int from_level, cudaStream_t s) {
     int j0 = p.J - 1;
     if (!(g_force_naive & 8)) {
@@ -440,8 +436,7 @@ int choose_coarse_level(const ll::Geom &whole, int nranks, int J, int K) {
     // The gathered level trades the two messages of a call against each other: gathering a finer level means a bigger
     // all-to-all (a rank receives (N-1)/N of the level: gPyramid + inGPyramid, (K + 1) floats per pixel) but a smaller
     // input halo (about 3 * 2^j frame rows of three uint16 channels per rank, which also is the recomputed work).  Pick the
-    // level with the fewest bytes received per rank; ties go to the finer level (less recompute).  Measured on 4 x B200,
-    // 16K frame: level 6 cost 65 + 55 us of NCCL time per frame, the 18.6 MB input halo alone being bandwidth-bound.
+    // level with the fewest bytes received per rank; ties go to the finer level (less recompute).
     const double frame_row_bytes = (double)whole.lv[0].sx.n() * 3 * sizeof(uint16_t);
     int best = J - 1;
     double best_bytes = 1e300;
@@ -738,7 +733,7 @@ extern "C" int halide_b200_ll_shard_plan_level(int32_t frame_w, int32_t frame_h,
     return choose_coarse_level(ll::make_geom(fx, fy, fx, fy, ll::kMaxJ), nranks, ll::kMaxJ, 8);
 }
 
-// Row-sharded entry point (B200 extension; see run_local_laplacian_sharded).
+// Row-sharded entry point (library extension; see run_local_laplacian_sharded).
 extern "C" int halide_b200_local_laplacian_sharded(halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                                    halide_buffer_t *output, int32_t frame_y_min, int32_t frame_y_extent) {
     return run_local_laplacian_sharded(input, levels, alpha, beta, output, frame_y_min, frame_y_extent);
@@ -772,7 +767,7 @@ extern "C" long long halide_b200_selftest_arith(unsigned long long n, unsigned l
     if (cudaMalloc(&bad, sizeof(*bad)) != cudaSuccess) return -1;
     cudaMemset(bad, 0, sizeof(*bad));
     cudaStream_t s = hb::stream();
-    HB_LAUNCH("ll_selftest", ll_selftest_kernel, 148 * 8, 256, 0, s, n, seed, bad);
+    HB_LAUNCH("ll_selftest", ll_selftest_kernel, 132 * 8, 256, 0, s, n, seed, bad);
     if (cudaMemcpyAsync(&host, bad, sizeof(host), cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) {
         cudaFree(bad);
         return -1;

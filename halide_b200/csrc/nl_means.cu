@@ -1,4 +1,4 @@
-// nl_means.cu — nl_means(input, patch_size, search_area, sigma, output) for sm_100a.
+// nl_means.cu — nl_means(input, patch_size, search_area, sigma, output) for sm_90a.
 //
 // Reference algorithm: apps/nl_means/nl_means_generator.cpp:24-63
 //   d(x,y,dx,dy)  = sum_c (I(x,y,c) - I(x+dx,y+dy,c))^2            (clamped coordinates, c = 0..2)
@@ -207,7 +207,7 @@ constexpr size_t nl_window_smem() {
     return (size_t)(3 * (TY + P + S - 2) * (TX + P + S - 2) + S * TY * (TX + P - 1)) * sizeof(float);
 }
 
-constexpr bool kDefaultWindow = true;  // (the register-window kernel: bit-identical to the first kernel on hardware, profiles/r02_ab_variants.log)
+constexpr bool kDefaultWindow = true;  // (the register-window kernel: bit-identical to the first kernel, tests/test_nl_means_gpu.py)
 int g_variant = 0;  // test / A-B hook (halide_b200_nl_means_variant): 0 = default, 1 = generic kernel, 2 = register-window kernel
 
 const hb::ArgSpec kIn = {"input", halide_type_float, 32, 3, false};
@@ -229,8 +229,8 @@ const halide_filter_argument_t kArgs[5] = {
     {"sigma", halide_argument_kind_input_scalar, 0, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, &sv_sigma, nullptr},
     {"non_local_means", halide_argument_kind_output_buffer, 3, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
-const halide_filter_metadata_t kMeta = {1, 5, kArgs, "x86-64-linux-cuda-cuda_capability_100-b200_native", "nl_means"};
-const halide_filter_metadata_t kMetaAuto = {1, 5, kArgs, "x86-64-linux-cuda-cuda_capability_100-b200_native",
+const halide_filter_metadata_t kMeta = {1, 5, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "nl_means"};
+const halide_filter_metadata_t kMetaAuto = {1, 5, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native",
                                             "nl_means_auto_schedule"};
 
 int run_nl_means(halide_buffer_t *input, int patch_size, int search_area, float sigma, halide_buffer_t *output) {

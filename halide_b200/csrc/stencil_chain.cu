@@ -224,7 +224,7 @@ __global__ void __launch_bounds__(256) stencil_chain_window_kernel(Plane p) {
     }
 }
 
-constexpr bool kDefaultWindow = true;  // (the register-window kernel: bit-identical to the first kernel on hardware, profiles/r02_ab_variants.log)
+constexpr bool kDefaultWindow = true;  // (the register-window kernel: bit-identical to the first kernel, tests/test_stencil_chain_gpu.py)
 int g_variant = 0;  // test / A-B hook (halide_b200_stencil_chain_variant): 0 = default, 1 = one-pixel-per-thread kernel, 2 = register-window kernel
 
 const hb::ArgSpec kIn = {"input", halide_type_uint, 16, 2, false};
@@ -235,8 +235,8 @@ const halide_filter_argument_t kArgs[2] = {
     {"input", halide_argument_kind_input_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
     {"output", halide_argument_kind_output_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
-const halide_filter_metadata_t kMeta = {1, 2, kArgs, "x86-64-linux-cuda-cuda_capability_100-b200_native", "stencil_chain"};
-const halide_filter_metadata_t kMetaAuto = {1, 2, kArgs, "x86-64-linux-cuda-cuda_capability_100-b200_native",
+const halide_filter_metadata_t kMeta = {1, 2, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "stencil_chain"};
+const halide_filter_metadata_t kMetaAuto = {1, 2, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native",
                                             "stencil_chain_auto_schedule"};
 
 int run_stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {

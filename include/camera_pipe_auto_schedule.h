@@ -3,7 +3,7 @@
  *  src/CodeGen_C.cpp:675-721 for the _argv and _metadata companions).
  * Generator: /root/reference/apps/camera_pipe/camera_pipe_generator.cpp:218-238,622
  * `camera_pipe_auto_schedule` is the second AOT variant the harness links (the app harness, when built without
- * -DNO_AUTO_SCHEDULE calls it); here it is the same sm_100a implementation under the second name.
+ * -DNO_AUTO_SCHEDULE calls it); here it is the same sm_90a implementation under the second name.
  * Returns 0 or a negative halide_error_code_t (include/halide_b200_runtime.h).
  */
 #ifndef HALIDE_B200_CAMERA_PIPE_AUTO_SCHEDULE_H

@@ -1,4 +1,4 @@
-/* halide_b200_runtime.h — the C ABI boundary of the B200-native Halide apps library.
+/* halide_b200_runtime.h — the C ABI boundary of the H100-native Halide apps library.
  *
  * This header re-declares (it does not copy) the binary layout a Halide AOT filter and its
  * harness agree on, so that `apps/<app>/process.cpp|filter.cpp|test.cpp` of the reference link
@@ -236,7 +236,7 @@ int halide_cuda_detach_device_ptr(void *user_context, struct halide_buffer_t *bu
 uintptr_t halide_cuda_get_device_ptr(void *user_context, struct halide_buffer_t *buf);
 int halide_cuda_release_unused_device_allocations(void *user_context);
 
-/* ---- B200 library extensions (no reference equivalent; plain pointers and sizes only) ---- */
+/* ---- library extensions (no reference equivalent; plain pointers and sizes only) ---- */
 
 /* Stream every kernel and copy of this thread's subsequent filter calls is issued on
  * (a cudaStream_t passed as void*; NULL = the legacy default stream, which is also torch's
@@ -251,7 +251,7 @@ int halide_b200_stream_destroy(void *cuda_stream);
 int halide_b200_set_device(int ordinal);
 /* Number of kernels this library has launched since process start (bench.py's gpu_launches). */
 uint64_t halide_b200_kernel_launch_count(void);
-/* Library/target identification string, e.g. "x86-64-linux-cuda-cuda_capability_100-b200_native". */
+/* Library/target identification string, e.g. "x86-64-linux-cuda-cuda_capability_90-h100_native". */
 const char *halide_b200_target(void);
 /* Bracket the kernels of one filter call with CUDA events on the library stream and report the
  * device time of the most recent call in milliseconds (negative if timing is disabled). */
@@ -305,7 +305,7 @@ void halide_b200_blur_force_general(int enable);
 void halide_b200_nl_means_variant(int variant);
 /* stencil_chain test / A-B hook: 0 = default kernel, 1 = one-pixel-per-thread tile kernel, 2 = register-window tile kernel. */
 void halide_b200_stencil_chain_variant(int variant);
-/* conv_layer: 1 = tcgen05/TMEM/TMA implicit GEMM (3xTF32 split), 0 = FP32 SIMT kernel (also HALIDE_B200_CONV=tc|simt). */
+/* conv_layer: 1 = wgmma/TMA implicit GEMM (3xTF32 split), 0 = FP32 SIMT kernel (also HALIDE_B200_CONV=tc|simt). */
 void halide_b200_conv_use_tensor_cores(int enable);
 /* Device self-test of the fast kernels' arithmetic shortcuts; returns mismatches vs div.rn / cvt, or -1. */
 long long halide_b200_selftest_arith(unsigned long long n, unsigned long long seed);

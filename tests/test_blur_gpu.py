@@ -17,11 +17,14 @@ def test_blur_matches_oracle(hb, oracle, h, w, seed):
 
 def test_blur_matches_reference_c_on_harness_shape(hb, oracle):
     """apps/blur/test.cpp:162-191: 2568x1922 input, rand() & 0xfff, compared on the interior
-    against the reference's own C implementations (oracle/_ref)."""
-    if not oracle.ref_blur_available():
-        pytest.skip("oracle/_ref/libref_blur.so not present")
+    against the reference's own C implementations (oracle/_ref) — or, where that is not built, what both returned for
+    this input (tests/golden/reference_digests.json)."""
+    from util import array_digest, reference_digest
     inp = u16_frame((1922, 2568), 7, bits=12)
     got = run_blur(hb, inp, (1920, 2560))
+    if not oracle.ref_blur_available():
+        assert array_digest(got) == reference_digest("ref_blur/1922x2568/0") == reference_digest("ref_blur/1922x2568/1")
+        return
     assert np.array_equal(got, oracle.ref_blur(inp, fast=False))
     assert np.array_equal(got, oracle.ref_blur(inp, fast=True))
 

@@ -56,7 +56,7 @@ def test_wrong_shape_is_a_constraint_violation(hb):
 
 @pytest.mark.parametrize("seed,scale", [(3, 1.0), (4, 2147483648.0)])
 def test_simt_path_matches_oracle(hb, oracle, seed, scale):
-    """The default path is the tcgen05 implicit GEMM (TMA + TMEM, 3xTF32 split); the FP32 SIMT kernel it replaced stays
+    """The default path is the wgmma implicit GEMM (TMA + mbarrier ring, 3xTF32 split); the FP32 SIMT kernel it replaced stays
     selectable (HALIDE_B200_CONV=simt) and must meet the same 1e-4 bar."""
     l = hb.load_library()
     inp, filt, bias = make(seed, scale)

@@ -30,7 +30,6 @@ def test_input_halo_filters_sharded_match_single_gpu():
     """blur / nl_means / stencil_chain / bilateral_grid / camera_pipe row-sharded over 2 GPUs (NCCL row exchange +
     the ordinary filter on the extended band) equal the whole-frame call on one GPU (bit for bit for the integer
     pipelines, 1e-4 relative for the float ones)."""
-    # (first hardware run: profiles/r02_dist_rows_check_n2.log)
     if _ngpu() < 2:
         pytest.skip("needs 2 GPUs")
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",

@@ -1,14 +1,16 @@
 """halide_b200/image_io.py against the reference's own image I/O header (tools/halide_image_io.h), which is compiled in
 place into oracle/_ref/ref_image_io (oracle/ref_image_io_tool.cpp): element conversions for every type pair, every
 format both ways (the reference writes / we read, we write / the reference reads), and the type / dimensionality choice
-of convert_and_save_image.  Where the reference binary is not available (a box without /root/reference and without
-a prebuilt oracle/_ref), the committed golden vectors (tests/golden/image_io_golden.npz, made by
-tests/golden/make_image_io_golden.py with the same binary) stand in for it."""
+of convert_and_save_image.  Where the reference binary is not available (oracle/_ref is built only where the reference
+source tree is), what it produced for every one of these cases stands in for it: SHA-256 digests in
+tests/golden/reference_digests.json (tests/golden/make_reference_digests.py) and the golden vectors of
+tests/golden/image_io_golden.npz (tests/golden/make_image_io_golden.py), both made with the same binary."""
 import os
 import subprocess
 
 import numpy as np
 import pytest
+from util import array_digest, bytes_digest, reference_digest
 
 from halide_b200 import image_io
 
@@ -18,7 +20,8 @@ GOLDEN = os.path.join(ROOT, "tests", "golden", "image_io_golden.npz")
 NAMES = {"u8": np.uint8, "u16": np.uint16, "u32": np.uint32, "u64": np.uint64, "i8": np.int8, "i16": np.int16,
          "i32": np.int32, "i64": np.int64, "f32": np.float32, "f64": np.float64}
 TNAME = {np.dtype(v): k for k, v in NAMES.items()}
-have_ref = pytest.mark.skipif(not os.path.exists(REF), reason="oracle/_ref/ref_image_io not built")
+IMAGES = os.path.join(ROOT, "tests", "golden", "images")   # small images from the reference's apps/images
+HAVE_REF = os.path.exists(REF)
 
 
 def samples(dtype, n=2048, seed=0):
@@ -58,13 +61,15 @@ def read_dump(path):
     return np.frombuffer(b[nl + 1:], dtype=NAMES[parts[0]]).reshape(tuple(reversed(ext))).copy()
 
 
-@have_ref
 @pytest.mark.parametrize("src", list(NAMES))
 def test_convert_matches_reference_for_every_target(src, tmp_path):
     a = samples(NAMES[src], seed=len(src))
     for dst in NAMES:
-        want = ref_convert(a, dst, tmp_path)
         got = image_io.convert(a, NAMES[dst])
+        if not HAVE_REF:
+            assert array_digest(got) == reference_digest(f"convert/{src}/{dst}"), (src, dst)
+            continue
+        want = ref_convert(a, dst, tmp_path)
         assert got.dtype == want.dtype
         assert np.array_equal(got.view(np.uint8), want.view(np.uint8)), (src, dst, a[np.flatnonzero(got != want)[:4]])
 
@@ -108,7 +113,10 @@ def random_image(dtype, shape, seed):
     return rng.integers(info.min, info.max, shape, dtype=dt, endpoint=True)
 
 
-@have_ref
+def format_case_key(fmt, dtype, shape):
+    return f"{fmt}/{TNAME[np.dtype(dtype)]}/{'x'.join(map(str, shape))}"
+
+
 @pytest.mark.parametrize("fmt,dtype,shape", FORMAT_CASES)
 def test_formats_round_trip_through_the_reference(fmt, dtype, shape, tmp_path):
     a = random_image(dtype, shape, len(shape) * 7 + np.dtype(dtype).itemsize)
@@ -116,6 +124,13 @@ def test_formats_round_trip_through_the_reference(fmt, dtype, shape, tmp_path):
     (tmp_path / "o").mkdir()
     # (same base name in two directories: a .mat file carries its own file name as the variable name)
     dump, ref_file, our_file, back = (str(tmp_path / n) for n in ("a.dump", "r/img." + fmt, "o/img." + fmt, "b.dump"))
+    if not HAVE_REF:
+        # every format here is written byte for byte as the reference writes it, so our file stands for the reference's
+        image_io.save(a, our_file)
+        assert bytes_digest(open(our_file, "rb").read()) == reference_digest("save/" + format_case_key(fmt, dtype, shape))
+        got = image_io.load(our_file)
+        assert got.dtype == a.dtype and np.array_equal(got, a)
+        return
     # the reference writes, we read
     write_dump(a, dump)
     subprocess.run([REF, "save", dump, ref_file], check=True)
@@ -129,15 +144,22 @@ def test_formats_round_trip_through_the_reference(fmt, dtype, shape, tmp_path):
         assert open(our_file, "rb").read() == open(ref_file, "rb").read()
 
 
-@have_ref
+AUTOSAVE_SHAPES = {"pgm": [(6, 7)], "ppm": [(3, 6, 7)], "npy": [(5,), (6, 7), (3, 6, 7)], "tmp": [(6, 7), (3, 6, 7), (2, 3, 6, 7)],
+                   "mat": [(6, 7), (3, 6, 7)]}
+
+
 @pytest.mark.parametrize("fmt", ["pgm", "ppm", "npy", "tmp", "mat"])
 def test_convert_and_save_picks_the_reference_type(fmt, tmp_path):
-    shapes = {"pgm": [(6, 7)], "ppm": [(3, 6, 7)], "npy": [(5,), (6, 7), (3, 6, 7)], "tmp": [(6, 7), (3, 6, 7), (2, 3, 6, 7)],
-              "mat": [(6, 7), (3, 6, 7)]}[fmt]
-    for shape in shapes:
+    for shape in AUTOSAVE_SHAPES[fmt]:
         for src in NAMES.values():
             a = random_image(src, shape, 3)
             dump, ref_file, our_file, d1, d2 = (str(tmp_path / n) for n in ("a.dump", "ref." + fmt, "ours." + fmt, "r.dump", "o.dump"))
+            if not HAVE_REF:
+                # what the reference's reader found in the file its convert_and_save_image wrote, against ours read back
+                image_io.convert_and_save_image(a, our_file)
+                assert array_digest(image_io.load(our_file)) == reference_digest("autosave/" + format_case_key(fmt, src, shape)), \
+                    (fmt, shape, src)
+                continue
             write_dump(a, dump)
             subprocess.run([REF, "autosave", dump, ref_file], check=True)
             image_io.convert_and_save_image(a, our_file)
@@ -148,17 +170,20 @@ def test_convert_and_save_picks_the_reference_type(fmt, tmp_path):
             assert np.array_equal(got.view(np.uint8), want.view(np.uint8)), (fmt, shape, src)
 
 
-@have_ref
+LOADCONV_CASES = (("gray_crop.pgm", ("u8", "u16", "f32")), ("matrix_3200.mat", ("f32",)), ("matrix_7000.mat", ("f32", "f64")))
+
+
 def test_load_and_convert_of_the_reference_images(tmp_path):
-    """apps/images/gray_small.pgm and the camera_pipe colour matrices, loaded into every type the harnesses ask for."""
-    images = "/root/reference/apps/images"
-    if not os.path.isdir(images):
-        pytest.skip("reference images not present")
-    for name, types in (("gray_small.pgm", ("u8", "u16", "f32")), ("matrix_3200.mat", ("f32",)), ("matrix_7000.mat", ("f32", "f64"))):
+    """A crop of apps/images/gray_small.pgm (written by the reference) and the camera_pipe colour matrices, loaded into
+    every type the harnesses ask for."""
+    for name, types in LOADCONV_CASES:
         for t in types:
+            got = image_io.load_and_convert_image(os.path.join(IMAGES, name), NAMES[t])
+            if not HAVE_REF:
+                assert array_digest(got) == reference_digest(f"loadconv/{name}/{t}"), (name, t)
+                continue
             out = str(tmp_path / "x.dump")
-            subprocess.run([REF, "loadconv", os.path.join(images, name), t, out], check=True)
-            got = image_io.load_and_convert_image(os.path.join(images, name), NAMES[t])
+            subprocess.run([REF, "loadconv", os.path.join(IMAGES, name), t, out], check=True)
             want = read_dump(out)
             assert got.dtype == want.dtype and np.array_equal(got, want), (name, t)
 
@@ -217,19 +242,21 @@ def test_png_codec_round_trip_and_cross_check(tmp_path):
         assert np.array_equal(pure, arr) and np.array_equal(image_io.load(p), arr)
 
 
+# crops of the reference's sample images apps/images/*_small*.png, re-encoded by OpenCV (tests/golden/make_reference_digests.py)
+PNG_CROPS = {"rgb_small_crop.png": "rgb_small.png", "rgb_small16_crop.png": "rgb_small16.png", "bayer_small_crop.png": "bayer_small.png"}
+
+
 def test_reference_png_images_decode_the_same_both_ways():
-    """The reference's small sample images (apps/images/*_small*.png: 8-bit gray and RGB, 16-bit RGB, 16-bit Bayer raw)
-    through the pure-Python decoder and through OpenCV; gray_small.png must equal gray_small.pgm, which the reference's
-    own reader decodes (test_load_and_convert_of_the_reference_images)."""
-    images = "/root/reference/apps/images"
-    if not os.path.isdir(images):
-        pytest.skip("reference images not present")
+    """The reference's sample images through the pure-Python decoder and through OpenCV: gray_small.png (8-bit gray, as
+    the reference ships it) and crops of rgb_small.png, rgb_small16.png and bayer_small.png (8-bit RGB, 16-bit RGB,
+    16-bit Bayer raw, encoded by OpenCV).  gray_small.png must equal gray_small.pgm as the reference's own reader decodes
+    it, and each crop the same region of the reference's PNG decoded in full."""
     try:
         import cv2  # noqa: F401
     except Exception:
         pytest.skip("OpenCV not importable: nothing to cross-check against")
-    for name in ("gray_small.png", "rgb_small.png", "rgb_small16.png", "bayer_small.png"):
-        p = os.path.join(images, name)
+    for name in ("gray_small.png",) + tuple(PNG_CROPS):
+        p = os.path.join(IMAGES, name)
         fast = image_io.load(p)
         os.environ["HALIDE_B200_PNG_PURE"] = "1"
         try:
@@ -237,21 +264,28 @@ def test_reference_png_images_decode_the_same_both_ways():
         finally:
             del os.environ["HALIDE_B200_PNG_PURE"]
         assert fast.dtype == pure.dtype and np.array_equal(fast, pure), name
-    assert np.array_equal(image_io.load(os.path.join(images, "gray_small.png")), image_io.load(os.path.join(images, "gray_small.pgm")))
+        if name in PNG_CROPS:
+            assert array_digest(pure) == reference_digest(f"png_crop/{name}"), name
+    assert array_digest(image_io.load(os.path.join(IMAGES, "gray_small.png"))) == reference_digest("loadconv/gray_small.pgm/u8")
 
 
-@have_ref
-@pytest.mark.parametrize("dtype,shape", [(np.uint8, (9, 14)), (np.uint16, (3, 9, 14)), (np.float32, (4, 5, 6)), (np.int32, (7,)),
-                                         (np.float64, (2, 3, 4, 5)), (np.uint8, (6, 3, 4)), (np.int16, (1, 2, 8, 9))])
+TIFF_CASES = [(np.uint8, (9, 14)), (np.uint16, (3, 9, 14)), (np.float32, (4, 5, 6)), (np.int32, (7,)), (np.float64, (2, 3, 4, 5)),
+              (np.uint8, (6, 3, 4)), (np.int16, (1, 2, 8, 9))]
+
+
+@pytest.mark.parametrize("dtype,shape", TIFF_CASES)
 def test_tiff_writer_is_byte_identical(dtype, shape, tmp_path):
     """The reference writes (uncompressed, planar) TIFF and cannot read it back; ours must produce the same bytes —
     including the rule that folds a third dimension below 5 into the channel count."""
     a = random_image(dtype, shape, 11)
     dump, ref_file, our_file = (str(tmp_path / n) for n in ("a.dump", "ref.tiff", "ours.tiff"))
-    write_dump(a, dump)
-    subprocess.run([REF, "save", dump, ref_file], check=True)
     image_io.save(a, our_file)
-    assert open(our_file, "rb").read() == open(ref_file, "rb").read()
+    if HAVE_REF:
+        write_dump(a, dump)
+        subprocess.run([REF, "save", dump, ref_file], check=True)
+        assert open(our_file, "rb").read() == open(ref_file, "rb").read()
+    else:
+        assert bytes_digest(open(our_file, "rb").read()) == reference_digest("save/" + format_case_key("tiff", dtype, shape))
     with pytest.raises(ValueError):
         image_io.load(our_file)
 
@@ -261,13 +295,7 @@ def test_natural_image_flow_like_process_cpp(tmp_path):
     filter (the CPU oracle stands in for it here — the GPU parity tests cover the filter itself), convert_and_save_image
     to a 16-bit PNG, reload: the file holds exactly the filter's output, and an 8-bit source enters as x * 257."""
     from oracle import pyoracle
-    images = "/root/reference/apps/images"
-    src = os.path.join(images, "rgb_small.png")
-    if not os.path.exists(src):
-        yy, xx = np.mgrid[0:48, 0:64]
-        rgb = np.stack([(np.sin(xx / 6.0) * 100 + 128), (np.cos(yy / 5.0) * 90 + 120), ((xx + yy) * 2 % 256)]).astype(np.uint8)
-        src = str(tmp_path / "synthetic.png")
-        image_io.save(rgb, src)
+    src = os.path.join(IMAGES, "rgb_crop.png")   # a 128x96 crop of apps/images/rgb_small.png
     native = image_io.load(src)
     assert native.dtype == np.uint8 and native.ndim == 3 and native.shape[0] == 3
     frame = image_io.load_and_convert_image(src, np.uint16)

@@ -1,5 +1,28 @@
-"""Shared helpers for the parity tests: seeded synthetic frames and C-ABI call wrappers."""
+"""Shared helpers for the parity tests: seeded synthetic frames, C-ABI call wrappers and the stored digests of what the
+reference produced."""
+import hashlib
+import json
+import os
+
 import numpy as np
+
+DIGESTS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_digests.json")
+
+
+def array_digest(a):
+    """SHA-256 of an array's type, shape and bytes: the form in which golden/reference_digests.json holds what the reference
+    produced (golden/make_reference_digests.py)."""
+    a = np.ascontiguousarray(a)
+    return hashlib.sha256(f"{a.dtype.str} {a.shape}".encode() + a.tobytes()).hexdigest()
+
+
+def bytes_digest(b):
+    return hashlib.sha256(b).hexdigest()
+
+
+def reference_digest(key):
+    with open(DIGESTS) as f:
+        return json.load(f)[key]
 
 
 def u16_frame(shape, seed, bits=16):

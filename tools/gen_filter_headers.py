@@ -29,7 +29,7 @@ def emit(name):
         guard = "HALIDE_B200_" + fn.upper() + "_H"
         note = "" if not suffix else (
             f" * `{fn}` is the second AOT variant the harness links (the app harness, when built without\n"
-            f" * -DNO_AUTO_SCHEDULE calls it); here it is the same sm_100a implementation under the second name.\n")
+            f" * -DNO_AUTO_SCHEDULE calls it); here it is the same sm_90a implementation under the second name.\n")
         with open(os.path.join(ROOT, "include", fn + ".h"), "w") as f:
             f.write(f"""/* {fn}.h — stands in for the header Halide's AOT compiler emits for this filter
  * (src/CodeGen_C.cpp:1083-1108 argument order: generator inputs in declaration order, then outputs;
