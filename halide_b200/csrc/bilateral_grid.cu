@@ -209,46 +209,30 @@ __global__ void __launch_bounds__(256) bg_slice_kernel(BGParams p) {
     }
 }
 
-const hb::ArgSpec kIn = {"input", halide_type_float, 32, 2, false};
-const hb::ArgSpec kOut = {"bilateral_grid", halide_type_float, 32, 2, true};
 int64_t est_i[2][2] = {{0, 1536}, {0, 2560}};
 const int64_t *const est_ptrs[4] = {&est_i[0][0], &est_i[0][1], &est_i[1][0], &est_i[1][1]};
-halide_scalar_value_t sv_rsigma;
-struct InitScalars {
-    InitScalars() { sv_rsigma.u.i64 = 0; sv_rsigma.u.f32 = 0.1f; }
-} init_scalars;
+const halide_scalar_value_t sv_rsigma = hb::scalar_f32(0.1f);
 const halide_filter_argument_t kArgs[3] = {
     {"input", halide_argument_kind_input_buffer, 2, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
     {"r_sigma", halide_argument_kind_input_scalar, 0, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, &sv_rsigma, nullptr},
     {"bilateral_grid", halide_argument_kind_output_buffer, 2, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
-const halide_filter_metadata_t kMeta = {1, 3, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "bilateral_grid"};
-const halide_filter_metadata_t kMetaAuto = {1, 3, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native",
-                                            "bilateral_grid_auto_schedule"};
 
 inline int fdiv(int a, int b) {  // floor division, b > 0
     int q = a / b;
     return (a % b != 0 && a < 0) ? q - 1 : q;
 }
 
-int run_bilateral_grid(halide_buffer_t *input, float r_sigma, halide_buffer_t *output) {
+}  // namespace
+
+extern "C" int bilateral_grid(halide_buffer_t *input, float r_sigma, halide_buffer_t *output) {
     int r;
-    if ((r = hb::check_arg(input, kIn))) return r;
-    if ((r = hb::check_arg(output, kOut))) return r;
-    bool query = false;
-    {
-        // the slice reads input(x,y) unclamped (generator :50): the input must cover the output region
-        int mins[2] = {output->dim[0].min, output->dim[1].min};
-        int ext[2] = {output->dim[0].extent, output->dim[1].extent};
-        if (hb::is_bounds_query(input)) { hb::propose_shape(input, mins, ext); query = true; }
-        if (hb::is_bounds_query(output)) { hb::propose_shape(output, mins, ext); query = true; }
-    }
-    if (query) return 0;
-    if ((r = hb::check_shape(input, kIn))) return r;
-    if ((r = hb::check_shape(output, kOut))) return r;
-    for (int d = 0; d < 2; d++) {
-        if ((r = hb::check_covers(input, kIn, d, output->dim[d].min, output->dim[d].extent))) return r;
-    }
+    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[2]}};
+    if ((r = hb::check_args(args, 2))) return r;
+    // the slice reads input(x,y) unclamped (generator :50): the input must cover the output region
+    const hb::Region need[2] = {hb::region_of(output, true), hb::region_of(output, false)};
+    if (hb::answer_bounds_query(args, need, 2)) return 0;
+    if ((r = hb::check_shapes(args, 2)) || (r = hb::check_required(args, need, 2))) return r;
     const int W = output->dim[0].extent, H = output->dim[1].extent;
     if (W <= 0 || H <= 0) return 0;
     if (!(r_sigma > 0.0f)) {
@@ -264,16 +248,14 @@ int run_bilateral_grid(halide_buffer_t *input, float r_sigma, halide_buffer_t *o
                         "Parameter r_sigma is %g: more than %d intensity bins are not supported by this build",
                         (double)r_sigma, (int)(200 * 1024 / (2 * 128 * sizeof(float))));
     }
-    void *din = nullptr, *dout = nullptr;
-    if ((r = hb::acquire_input(input, kIn, &din))) return r;
-    if ((r = hb::acquire_output(output, kOut, &dout))) return r;
+    if ((r = hb::acquire(args, 2))) return r;
 
     const int ox = output->dim[0].min, oy = output->dim[1].min;
-    p.in = (const float *)din;
+    p.in = (const float *)args[0].dev;
     p.in_sy = input->dim[1].stride;
     p.in_x0 = input->dim[0].min; p.in_y0 = input->dim[1].min;
     p.in_w = input->dim[0].extent; p.in_h = input->dim[1].extent;
-    p.out = (float *)dout;
+    p.out = (float *)args[1].dev;
     p.out_sy = output->dim[1].stride;
     p.out_x0 = ox; p.out_y0 = oy; p.W = W; p.H = H;
     // cells the slice touches are xi..xi+1; blury/blurx add 2 cells on every side
@@ -308,28 +290,7 @@ int run_bilateral_grid(halide_buffer_t *input, float r_sigma, halide_buffer_t *o
         if (slice_smem > 48 * 1024) cudaFuncSetAttribute(bg_slice_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)slice_smem);
         HB_LAUNCH("bg_slice", bg_slice_kernel, g3, dim3(32, 8), slice_smem, s, p);
     }
-    if ((r = hb::check_cuda(cudaGetLastError(), "bilateral_grid launch", halide_error_code_device_run_failed))) return r;
-    hb::mark_output_written(output);
-    return 0;
+    return hb::finish(args, 2, "bilateral_grid launch");
 }
-
-}  // namespace
-
-extern "C" int bilateral_grid(halide_buffer_t *input, float r_sigma, halide_buffer_t *output) {
-    return run_bilateral_grid(input, r_sigma, output);
-}
-extern "C" int bilateral_grid_argv(void **args) {
-    return run_bilateral_grid((halide_buffer_t *)args[0], *(float *)args[1], (halide_buffer_t *)args[2]);
-}
-extern "C" const halide_filter_metadata_t *bilateral_grid_metadata(void) {
-    return &kMeta;
-}
-extern "C" int bilateral_grid_auto_schedule(halide_buffer_t *input, float r_sigma, halide_buffer_t *output) {
-    return run_bilateral_grid(input, r_sigma, output);
-}
-extern "C" int bilateral_grid_auto_schedule_argv(void **args) {
-    return bilateral_grid_argv(args);
-}
-extern "C" const halide_filter_metadata_t *bilateral_grid_auto_schedule_metadata(void) {
-    return &kMetaAuto;
-}
+HB_EXPORT_FILTER(bilateral_grid, kArgs)
+HB_EXPORT_AUTO_SCHEDULE(bilateral_grid, kArgs)

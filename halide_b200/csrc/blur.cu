@@ -291,54 +291,31 @@ __global__ void __launch_bounds__(32 * kQuadWarps) blur3x3_u16_quad_kernel(BlurA
     }
 }
 
-const hb::ArgSpec kIn = {"input", halide_type_uint, 16, 2, false};
-const hb::ArgSpec kOut = {"blur_y", halide_type_uint, 16, 2, true};
-
 const halide_filter_argument_t kArgs[2] = {
     {"input", halide_argument_kind_input_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
     {"blur_y", halide_argument_kind_output_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
 };
-const halide_filter_metadata_t kMeta = {1, 2, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "halide_blur"};
 
 }  // namespace
 
 extern "C" int halide_blur(halide_buffer_t *input, halide_buffer_t *blur_y) {
     int r;
-    if ((r = hb::check_arg(input, kIn))) return r;
-    if ((r = hb::check_arg(blur_y, kOut))) return r;
-
-    // Bounds query (src/AddImageChecks.cpp:477-496): the input must cover the output region
-    // grown by the 3-tap footprints: [ox, ox+W+1] x [oy, oy+H+1].
+    hb::Arg args[2] = {{input, kArgs[0]}, {blur_y, kArgs[1]}};
+    if ((r = hb::check_args(args, 2))) return r;
+    // The input must cover the output region grown by the 3-tap footprints: [ox, ox+W+1] x [oy, oy+H+1].
     const int ox = blur_y->dim[0].min, oy = blur_y->dim[1].min;
     const int w = blur_y->dim[0].extent, h = blur_y->dim[1].extent;
-    bool query = false;
-    if (hb::is_bounds_query(input)) {
-        int mins[2] = {ox, oy}, ext[2] = {w + 2, h + 2};
-        hb::propose_shape(input, mins, ext);
-        query = true;
-    }
-    if (hb::is_bounds_query(blur_y)) {
-        int mins[2] = {ox, oy}, ext[2] = {w, h};
-        hb::propose_shape(blur_y, mins, ext);
-        query = true;
-    }
-    if (query) return 0;
-
-    if ((r = hb::check_shape(input, kIn))) return r;
-    if ((r = hb::check_shape(blur_y, kOut))) return r;
-    if ((r = hb::check_covers(input, kIn, 0, ox, w + 2))) return r;
-    if ((r = hb::check_covers(input, kIn, 1, oy, h + 2))) return r;
+    const hb::Region need[2] = {{{ox, oy}, {w + 2, h + 2}, true}, hb::region_of(blur_y, false)};
+    if (hb::answer_bounds_query(args, need, 2)) return 0;
+    if ((r = hb::check_shapes(args, 2)) || (r = hb::check_required(args, need, 2))) return r;
     if (w <= 0 || h <= 0) return 0;
-
-    void *din = nullptr, *dout = nullptr;
-    if ((r = hb::acquire_input(input, kIn, &din))) return r;
-    if ((r = hb::acquire_output(blur_y, kOut, &dout))) return r;
+    if ((r = hb::acquire(args, 2))) return r;
 
     BlurArgs a;
     const int64_t isy = input->dim[1].stride;
     const int64_t origin = (int64_t)(ox - input->dim[0].min) + (int64_t)(oy - input->dim[1].min) * isy;
-    a.in = (const uint16_t *)din + origin;
-    a.out = (uint16_t *)dout;
+    a.in = (const uint16_t *)args[0].dev + origin;
+    a.out = (uint16_t *)args[1].dev;
     a.in_stride_y = isy;
     a.out_stride_y = blur_y->dim[1].stride;
     a.w = w;
@@ -395,21 +372,12 @@ extern "C" int halide_blur(halide_buffer_t *input, halide_buffer_t *blur_y) {
             HB_LAUNCH("blur3x3_u16", blur3x3_u16_kernel, grid, 32 * kWarpsPerBlock, 0, s, a);
         }
     }
-    if ((r = hb::check_cuda(cudaGetLastError(), "halide_blur launch", halide_error_code_device_run_failed))) return r;
-    hb::mark_output_written(blur_y);
-    return 0;
+    return hb::finish(args, 2, "halide_blur launch");
 }
+HB_EXPORT_FILTER(halide_blur, kArgs)
 
 // Test hook: 1 = always take the general (any alignment) kernel, so both kernels stay covered by the parity tests;
 // >= 8 = the aligned kernel with strips of that many rows.
 extern "C" void halide_b200_blur_force_general(int enable) {
     g_force_general = enable;
-}
-
-extern "C" int halide_blur_argv(void **args) {
-    return halide_blur((halide_buffer_t *)args[0], (halide_buffer_t *)args[1]);
-}
-
-extern "C" const halide_filter_metadata_t *halide_blur_metadata(void) {
-    return &kMeta;
 }

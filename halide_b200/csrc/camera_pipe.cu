@@ -227,22 +227,12 @@ __global__ void __launch_bounds__(256) camera_pipe_kernel(CPParams p) {
     }
 }
 
-const hb::ArgSpec kIn = {"input", halide_type_uint, 16, 2, false};
-const hb::ArgSpec kM32 = {"matrix_3200", halide_type_float, 32, 2, false};
-const hb::ArgSpec kM70 = {"matrix_7000", halide_type_float, 32, 2, false};
-const hb::ArgSpec kOut = {"processed", halide_type_uint, 8, 3, true};
-
 int64_t est_in[2][2] = {{0, 2592}, {0, 1968}}, est_m[2][2] = {{0, 4}, {0, 3}}, est_out[3][2] = {{0, 2592}, {0, 1968}, {0, 3}};
 const int64_t *const est_in_p[4] = {&est_in[0][0], &est_in[0][1], &est_in[1][0], &est_in[1][1]};
 const int64_t *const est_m_p[4] = {&est_m[0][0], &est_m[0][1], &est_m[1][0], &est_m[1][1]};
 const int64_t *const est_out_p[6] = {&est_out[0][0], &est_out[0][1], &est_out[1][0], &est_out[1][1], &est_out[2][0], &est_out[2][1]};
-halide_scalar_value_t sv[6];
-struct InitScalars {
-    InitScalars() {
-        for (auto &v : sv) v.u.i64 = 0;
-        sv[0].u.f32 = 3700; sv[1].u.f32 = 2.0f; sv[2].u.f32 = 50; sv[3].u.f32 = 1.0f; sv[4].u.i32 = 25; sv[5].u.i32 = 1023;
-    }
-} init_scalars;
+const halide_scalar_value_t sv[6] = {hb::scalar_f32(3700), hb::scalar_f32(2.0f), hb::scalar_f32(50), hb::scalar_f32(1.0f),
+                                     hb::scalar_i32(25), hb::scalar_i32(1023)};
 const halide_filter_argument_t kArgs[10] = {
     {"input", halide_argument_kind_input_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_in_p},
     {"matrix_3200", halide_argument_kind_input_buffer, 2, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_m_p},
@@ -255,76 +245,47 @@ const halide_filter_argument_t kArgs[10] = {
     {"whiteLevel", halide_argument_kind_input_scalar, 0, {halide_type_int, 32, 0}, nullptr, nullptr, nullptr, &sv[5], nullptr},
     {"processed", halide_argument_kind_output_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, est_out_p},
 };
-const halide_filter_metadata_t kMeta = {1, 10, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "camera_pipe"};
-const halide_filter_metadata_t kMetaAuto = {1, 10, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native",
-                                            "camera_pipe_auto_schedule"};
 
 inline int fdiv(int a, int b) {
     int q = a / b;
     return (a % b != 0 && ((a < 0) != (b < 0))) ? q - 1 : q;
 }
 
-int run_camera_pipe(halide_buffer_t *input, halide_buffer_t *m3200, halide_buffer_t *m7000, float color_temp, float gamma,
-                    float contrast, float sharpen_strength, int blackLevel, int whiteLevel, halide_buffer_t *out) {
+}  // namespace
+
+extern "C" int camera_pipe(halide_buffer_t *input, halide_buffer_t *m3200, halide_buffer_t *m7000, float color_temp, float gamma,
+                           float contrast, float sharpen_strength, int32_t blackLevel, int32_t whiteLevel, halide_buffer_t *out) {
     int r;
-    if ((r = hb::check_arg(input, kIn))) return r;
-    if ((r = hb::check_arg(m3200, kM32))) return r;
-    if ((r = hb::check_arg(m7000, kM70))) return r;
-    if ((r = hb::check_arg(out, kOut))) return r;
+    hb::Arg args[4] = {{input, kArgs[0]}, {m3200, kArgs[1]}, {m7000, kArgs[2]}, {out, kArgs[9]}};
+    if ((r = hb::check_args(args, 4))) return r;
     const int ox = out->dim[0].min, oy = out->dim[1].min, W = out->dim[0].extent, H = out->dim[1].extent;
     // Required input region by interval arithmetic over the stencil chain (no boundary condition anywhere):
     // unsharp +-1 -> half-res sites -> demosaic +-1 site -> denoise +-2 -> shift (16,12).
     const int hx0 = fdiv(ox - 1, 2), hx1 = fdiv(ox + W, 2), hy0 = fdiv(oy - 1, 2), hy1 = fdiv(oy + H, 2);
     const int need_x0 = 2 * (hx0 - 1) - 2 + 16, need_x1 = 2 * (hx1 + 1) + 1 + 2 + 16;
     const int need_y0 = 2 * (hy0 - 1) - 2 + 12, need_y1 = 2 * (hy1 + 1) + 1 + 2 + 12;
-    bool query = false;
-    if (hb::is_bounds_query(input)) {
-        int mins[2] = {need_x0, need_y0}, ext[2] = {need_x1 - need_x0 + 1, need_y1 - need_y0 + 1};
-        hb::propose_shape(input, mins, ext);
-        query = true;
-    }
-    for (halide_buffer_t *m : {m3200, m7000}) {
-        if (hb::is_bounds_query(m)) {
-            int mins[2] = {0, 0}, ext[2] = {4, 3};
-            hb::propose_shape(m, mins, ext);
-            query = true;
-        }
-    }
-    if (hb::is_bounds_query(out)) {
-        int mins[3] = {ox, oy, out->dim[2].min}, ext[3] = {W, H, out->dim[2].extent};
-        hb::propose_shape(out, mins, ext);
-        query = true;
-    }
-    if (query) return 0;
-    if ((r = hb::check_shape(input, kIn)) || (r = hb::check_shape(m3200, kM32)) || (r = hb::check_shape(m7000, kM70)) ||
-        (r = hb::check_shape(out, kOut)))
-        return r;
+    const hb::Region matrix = {{0, 0}, {4, 3}, true};
+    const hb::Region need[4] = {{{need_x0, need_y0}, {need_x1 - need_x0 + 1, need_y1 - need_y0 + 1}, true}, matrix, matrix,
+                                hb::region_of(out, false)};
+    if (hb::answer_bounds_query(args, need, 4)) return 0;
+    if ((r = hb::check_shapes(args, 4))) return r;
     if (W <= 0 || H <= 0 || out->dim[2].extent <= 0) return 0;
-    if ((r = hb::check_covers(input, kIn, 0, need_x0, need_x1 - need_x0 + 1))) return r;
-    if ((r = hb::check_covers(input, kIn, 1, need_y0, need_y1 - need_y0 + 1))) return r;
-    for (halide_buffer_t *m : {m3200, m7000}) {
-        const hb::ArgSpec &sp = m == m3200 ? kM32 : kM70;
-        if ((r = hb::check_covers(m, sp, 0, 0, 4)) || (r = hb::check_covers(m, sp, 1, 0, 3))) return r;
-    }
-    if ((r = hb::check_covers(out, kOut, 2, out->dim[2].min, out->dim[2].extent))) return r;
+    if ((r = hb::check_required(args, need, 4))) return r;
     if (out->dim[2].min < 0 || out->dim[2].min + out->dim[2].extent > 3) {
         return hb::fail(halide_error_code_access_out_of_bounds, "Output buffer processed channel range [%d,%d) is outside [0,3)",
                         out->dim[2].min, out->dim[2].min + out->dim[2].extent);
     }
-    void *din = nullptr, *d32 = nullptr, *d70 = nullptr, *dout = nullptr;
-    if ((r = hb::acquire_input(input, kIn, &din)) || (r = hb::acquire_input(m3200, kM32, &d32)) ||
-        (r = hb::acquire_input(m7000, kM70, &d70)) || (r = hb::acquire_output(out, kOut, &dout)))
-        return r;
+    if ((r = hb::acquire(args, 4))) return r;
     hb::Scratch scratch;
     CPTables *tab = scratch.get<CPTables>(1);
     if (!tab) return hb::fail(halide_error_code_device_malloc_failed, "camera_pipe: scratch allocation failed");
 
     CPParams p;
-    p.in = (const u16 *)din;
+    p.in = (const u16 *)args[0].dev;
     p.in_sy = input->dim[1].stride;
     p.in_x0 = input->dim[0].min; p.in_y0 = input->dim[1].min;
     p.in_w = input->dim[0].extent; p.in_h = input->dim[1].extent;
-    p.out = (u8 *)dout;
+    p.out = (u8 *)args[3].dev;
     p.out_sy = out->dim[1].stride; p.out_sc = out->dim[2].stride;
     p.out_x0 = ox; p.out_y0 = oy; p.W = W; p.H = H; p.C = out->dim[2].extent; p.out_c0 = out->dim[2].min;
     p.tab = tab;
@@ -332,8 +293,8 @@ int run_camera_pipe(halide_buffer_t *input, halide_buffer_t *m3200, halide_buffe
     const float c_diff = 1.0f / 7000 - 1.0f / 3200;
     const float inv_c_diff = (float)(1.0 / (double)c_diff);
     // offsets of matrix element (0,0)
-    const float *m32p = (const float *)d32 - m3200->dim[0].min * (int64_t)m3200->dim[0].stride - m3200->dim[1].min * (int64_t)m3200->dim[1].stride;
-    const float *m70p = (const float *)d70 - m7000->dim[0].min * (int64_t)m7000->dim[0].stride - m7000->dim[1].min * (int64_t)m7000->dim[1].stride;
+    const float *m32p = (const float *)args[1].dev - m3200->dim[0].min * (int64_t)m3200->dim[0].stride - m3200->dim[1].min * (int64_t)m3200->dim[1].stride;
+    const float *m70p = (const float *)args[2].dev - m7000->dim[0].min * (int64_t)m7000->dim[0].stride - m7000->dim[1].min * (int64_t)m7000->dim[1].stride;
     cudaStream_t s = hb::stream();
     {
         hb::CallTimer timer(s);
@@ -343,35 +304,7 @@ int run_camera_pipe(halide_buffer_t *input, halide_buffer_t *m3200, halide_buffe
         dim3 grid((W + TW - 1) / TW, (H + TH - 1) / TH);
         HB_LAUNCH("camera_pipe", camera_pipe_kernel, grid, 256, 0, s, p);
     }
-    if ((r = hb::check_cuda(cudaGetLastError(), "camera_pipe launch", halide_error_code_device_run_failed))) return r;
-    hb::mark_output_written(out);
-    return 0;
+    return hb::finish(args, 4, "camera_pipe launch");
 }
-
-}  // namespace
-
-extern "C" int camera_pipe(halide_buffer_t *input, halide_buffer_t *matrix_3200, halide_buffer_t *matrix_7000, float color_temp,
-                           float gamma, float contrast, float sharpen_strength, int32_t blackLevel, int32_t whiteLevel,
-                           halide_buffer_t *processed) {
-    return run_camera_pipe(input, matrix_3200, matrix_7000, color_temp, gamma, contrast, sharpen_strength, blackLevel, whiteLevel,
-                           processed);
-}
-extern "C" int camera_pipe_argv(void **a) {
-    return run_camera_pipe((halide_buffer_t *)a[0], (halide_buffer_t *)a[1], (halide_buffer_t *)a[2], *(float *)a[3], *(float *)a[4],
-                           *(float *)a[5], *(float *)a[6], *(int32_t *)a[7], *(int32_t *)a[8], (halide_buffer_t *)a[9]);
-}
-extern "C" const halide_filter_metadata_t *camera_pipe_metadata(void) {
-    return &kMeta;
-}
-extern "C" int camera_pipe_auto_schedule(halide_buffer_t *input, halide_buffer_t *matrix_3200, halide_buffer_t *matrix_7000,
-                                         float color_temp, float gamma, float contrast, float sharpen_strength, int32_t blackLevel,
-                                         int32_t whiteLevel, halide_buffer_t *processed) {
-    return run_camera_pipe(input, matrix_3200, matrix_7000, color_temp, gamma, contrast, sharpen_strength, blackLevel, whiteLevel,
-                           processed);
-}
-extern "C" int camera_pipe_auto_schedule_argv(void **a) {
-    return camera_pipe_argv(a);
-}
-extern "C" const halide_filter_metadata_t *camera_pipe_auto_schedule_metadata(void) {
-    return &kMetaAuto;
-}
+HB_EXPORT_FILTER(camera_pipe, kArgs)
+HB_EXPORT_AUTO_SCHEDULE(camera_pipe, kArgs)

@@ -103,11 +103,6 @@ __global__ void __launch_bounds__(256) conv_layer_kernel(const float *__restrict
     }
 }
 
-const hb::ArgSpec kIn = {"input", halide_type_float, 32, 4, false};
-const hb::ArgSpec kFilt = {"filter", halide_type_float, 32, 4, false};
-const hb::ArgSpec kBias = {"bias", halide_type_float, 32, 1, false};
-const hb::ArgSpec kOut = {"relu", halide_type_float, 32, 4, true};
-
 // estimates = the fixed shapes (generator :52-68)
 int64_t e_zero = 0, e_ci = CI, e_co = CO, e_wp = W + 2, e_hp = H + 2, e_w = W, e_h = H, e_n = N, e_3 = 3;
 const int64_t *const est_in[8] = {&e_zero, &e_ci, &e_zero, &e_wp, &e_zero, &e_hp, &e_zero, &e_n};
@@ -120,22 +115,18 @@ const halide_filter_argument_t kArgs[4] = {
     {"bias", halide_argument_kind_input_buffer, 1, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_b},
     {"relu", halide_argument_kind_output_buffer, 4, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_out},
 };
-const halide_filter_metadata_t kMeta = {1, 4, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "conv_layer"};
-const halide_filter_metadata_t kMetaAuto = {1, 4, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native",
-                                            "conv_layer_auto_schedule"};
+// the generator's set_bounds / set_stride constraints (:35-50): every buffer is exactly this region, densely packed
+const hb::Region kShapes[4] = {{{0}, {CI, W + 2, H + 2, N}, false}, {{0}, {CO, 3, 3, CI}, false}, {{0}, {CO}, false},
+                               {{0}, {CO, W, H, N}, false}};
 
-struct Shape {
-    int ext[4];
-};
-// the generator's set_bounds / set_stride constraints (:35-50)
-const Shape kInShape = {{CI, W + 2, H + 2, N}}, kFiltShape = {{CO, 3, 3, CI}}, kOutShape = {{CO, W, H, N}};
-
-int check_fixed(const halide_buffer_t *b, const hb::ArgSpec &spec, const int *ext, int nd) {
+int check_fixed(const hb::Arg &a, const hb::Region &shape) {
+    const halide_buffer_t *b = a.b;
+    const int *ext = shape.extent;
     int64_t stride = 1;
-    for (int d = 0; d < nd; d++) {
+    for (int d = 0; d < b->dimensions; d++) {
         if (b->dim[d].min != 0 || b->dim[d].extent != ext[d] || b->dim[d].stride != stride) {
             return hb::fail(halide_error_code_constraint_violated,
-                            "Constraint violated: %s.dim(%d) is (min %d, extent %d, stride %d) but must be (0, %d, %lld)", spec.name, d,
+                            "Constraint violated: %s.dim(%d) is (min %d, extent %d, stride %d) but must be (0, %d, %lld)", a.meta.name, d,
                             b->dim[d].min, b->dim[d].extent, b->dim[d].stride, ext[d], (long long)stride);
         }
         stride *= ext[d];
@@ -143,65 +134,34 @@ int check_fixed(const halide_buffer_t *b, const hb::ArgSpec &spec, const int *ex
     return 0;
 }
 
-int run_conv_layer(halide_buffer_t *input, halide_buffer_t *filter, halide_buffer_t *bias, halide_buffer_t *relu) {
+}  // namespace
+
+extern "C" int conv_layer(halide_buffer_t *input, halide_buffer_t *filter, halide_buffer_t *bias, halide_buffer_t *relu) {
     int r;
-    if ((r = hb::check_arg(input, kIn)) || (r = hb::check_arg(filter, kFilt)) || (r = hb::check_arg(bias, kBias)) ||
-        (r = hb::check_arg(relu, kOut)))
+    hb::Arg args[4] = {{input, kArgs[0]}, {filter, kArgs[1]}, {bias, kArgs[2]}, {relu, kArgs[3]}};
+    if ((r = hb::check_args(args, 4))) return r;
+    if (hb::answer_bounds_query(args, kShapes, 4)) return 0;
+    if ((r = hb::check_shapes(args, 4))) return r;
+    if ((r = check_fixed(args[3], kShapes[3])) || (r = check_fixed(args[0], kShapes[0])) || (r = check_fixed(args[1], kShapes[1])) ||
+        (r = check_fixed(args[2], kShapes[2])))
         return r;
-    bool query = false;
-    const int zero4[4] = {0, 0, 0, 0};
-    const int bias_ext[1] = {CO};
-    if (hb::is_bounds_query(input)) { hb::propose_shape(input, zero4, kInShape.ext); query = true; }
-    if (hb::is_bounds_query(filter)) { hb::propose_shape(filter, zero4, kFiltShape.ext); query = true; }
-    if (hb::is_bounds_query(bias)) { hb::propose_shape(bias, zero4, bias_ext); query = true; }
-    if (hb::is_bounds_query(relu)) { hb::propose_shape(relu, zero4, kOutShape.ext); query = true; }
-    if (query) return 0;
-    if ((r = hb::check_shape(input, kIn)) || (r = hb::check_shape(filter, kFilt)) || (r = hb::check_shape(bias, kBias)) ||
-        (r = hb::check_shape(relu, kOut)))
-        return r;
-    if ((r = check_fixed(relu, kOut, kOutShape.ext, 4)) || (r = check_fixed(input, kIn, kInShape.ext, 4)) ||
-        (r = check_fixed(filter, kFilt, kFiltShape.ext, 4)) || (r = check_fixed(bias, kBias, bias_ext, 1)))
-        return r;
-    void *din = nullptr, *df = nullptr, *db = nullptr, *dout = nullptr;
-    if ((r = hb::acquire_input(input, kIn, &din)) || (r = hb::acquire_input(filter, kFilt, &df)) ||
-        (r = hb::acquire_input(bias, kBias, &db)) || (r = hb::acquire_output(relu, kOut, &dout)))
-        return r;
+    if ((r = hb::acquire(args, 4))) return r;
+    const float *din = (const float *)args[0].dev, *df = (const float *)args[1].dev, *db = (const float *)args[2].dev;
+    float *dout = (float *)args[3].dev;
     cudaStream_t s = hb::stream();
     {
         hb::CallTimer timer(s);
         if (g_use_tc) {
-            if ((r = conv_layer_tc_run((const float *)din, (const float *)df, (const float *)db, (float *)dout, s))) return r;
+            if ((r = conv_layer_tc_run(din, df, db, dout, s))) return r;
         } else {
             dim3 grid(W / TX, H / TY, N);
-            HB_LAUNCH("conv_layer_f32", conv_layer_kernel, grid, 256, 0, s, (const float *)din, (const float *)df, (const float *)db,
-                      (float *)dout);
+            HB_LAUNCH("conv_layer_f32", conv_layer_kernel, grid, 256, 0, s, din, df, db, dout);
         }
     }
-    if ((r = hb::check_cuda(cudaGetLastError(), "conv_layer launch", halide_error_code_device_run_failed))) return r;
-    hb::mark_output_written(relu);
-    return 0;
+    return hb::finish(args, 4, "conv_layer launch");
 }
-
-}  // namespace
-
-extern "C" int conv_layer(halide_buffer_t *input, halide_buffer_t *filter, halide_buffer_t *bias, halide_buffer_t *relu) {
-    return run_conv_layer(input, filter, bias, relu);
-}
-extern "C" int conv_layer_argv(void **a) {
-    return run_conv_layer((halide_buffer_t *)a[0], (halide_buffer_t *)a[1], (halide_buffer_t *)a[2], (halide_buffer_t *)a[3]);
-}
-extern "C" const halide_filter_metadata_t *conv_layer_metadata(void) {
-    return &kMeta;
-}
-extern "C" int conv_layer_auto_schedule(halide_buffer_t *input, halide_buffer_t *filter, halide_buffer_t *bias, halide_buffer_t *relu) {
-    return run_conv_layer(input, filter, bias, relu);
-}
-extern "C" int conv_layer_auto_schedule_argv(void **a) {
-    return conv_layer_argv(a);
-}
-extern "C" const halide_filter_metadata_t *conv_layer_auto_schedule_metadata(void) {
-    return &kMetaAuto;
-}
+HB_EXPORT_FILTER(conv_layer, kArgs)
+HB_EXPORT_AUTO_SCHEDULE(conv_layer, kArgs)
 
 extern "C" void halide_b200_conv_use_tensor_cores(int enable) {
     g_use_tc = enable != 0;

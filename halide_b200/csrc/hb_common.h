@@ -1,15 +1,21 @@
 // hb_common.h — internal helpers shared by the filter translation units of libhalide_b200.so.
 //
-// Host side of the drop-in boundary: argument validation in the order a Halide-generated
-// filter prologue performs it (reference: src/AddImageChecks.cpp:311-347,404-476,560-686),
-// bounds-query mode (src/AddImageChecks.cpp:477-496,710-716), host/device residency
-// (src/InjectHostDevBufferCopies.cpp, src/runtime/device_interface.cpp:154-205) and the
-// kernel-launch bookkeeping.  Nothing here computes pixels.
+// Host side of the drop-in boundary, owned here once for every filter: the call sequence of a
+// Halide-generated filter prologue over the buffer arguments (reference:
+// src/AddImageChecks.cpp:311-347,404-476,560-686), bounds-query mode (src/AddImageChecks.cpp:477-496,
+// 710-716), host/device residency (src/InjectHostDevBufferCopies.cpp,
+// src/runtime/device_interface.cpp:154-205), the F_argv / F_metadata / F_auto_schedule exports
+// (HB_EXPORT_FILTER, HB_EXPORT_AUTO_SCHEDULE) and the kernel-launch bookkeeping.  The argument
+// records the checks read are the filter's metadata (halide_filter_argument_t).  A filter adds only
+// its required regions, its own parameter checks and its launches.  Nothing here computes pixels.
 #pragma once
 
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+
+#include <type_traits>
+#include <utility>
 
 #include "../../include/halide_b200_runtime.h"
 
@@ -69,45 +75,86 @@ struct Scratch {  // frees everything it handed out when the filter call returns
     }
 };
 
-// ---- buffer validation -----------------------------------------------------------------------
-struct ArgSpec {
-    const char *name;  // "Input buffer input", "Output buffer output" style prefix is added by fail()
-    uint8_t code;      // halide_type_uint / halide_type_float ...
-    uint8_t bits;
-    int dimensions;
-    bool is_output;
+// ---- the call boundary of a filter ------------------------------------------------------------
+// A filter entry point runs, in this order: check_args; answer_bounds_query (return 0 if it did);
+// check_shapes; its required-region and parameter checks (check_required + its own); acquire; its
+// launches; finish.  Every step before acquire returns before any CUDA call.
+constexpr const char *kTarget = "x86-64-linux-cuda-cuda_capability_90-h100_native";
+
+// One buffer argument: the caller's buffer, its record in the filter's metadata (name, type,
+// dimensions, input or output) and, once acquired, the device address of its element at the mins.
+struct Arg {
+    halide_buffer_t *b;
+    const halide_filter_argument_t &meta;
+    void *dev = nullptr;
 };
 
-inline bool is_bounds_query(const halide_buffer_t *b) {
-    return b->host == nullptr && b->device == 0;  // HalideRuntime.h:1851-1853
+// The part of a buffer a call touches: proposed by a bounds query, and required of the caller's
+// buffer when must_cover (reads without a boundary condition).
+struct Region {
+    int min[4], extent[4];
+    bool must_cover;
+};
+Region region_of(const halide_buffer_t *b, bool must_cover);  // the buffer's own min/extent
+
+// null → -12, type → -3, dimensions → -43, buffer by buffer in argument order.
+int check_args(const Arg *a, int n);
+// Bounds-query mode (HalideRuntime.h:1851-1853): every buffer with neither host nor device memory
+// gets need[i] with dense strides (src/AddImageChecks.cpp:386-436,477-496).  True if any did.
+bool answer_bounds_query(Arg *a, const Region *need, int n);
+// negative extent → -28, |extent*stride| and extent product limits → -5/-6, stride[0] != 1 → -8.
+int check_shapes(const Arg *a, int n);
+// every must_cover region must lie inside its buffer, dimension by dimension → else -4.
+int check_required(const Arg *a, const Region *need, int n);
+// Inputs: device allocation + H2D when host-dirty or not yet on the device; outputs: allocation
+// only.  Sets a[i].dev.  Returns 0 or a negative halide_error_code_t.
+int acquire(Arg *a, int n);
+// After the launches: a launch error → device_run_failed naming `what`; else the outputs become
+// device-dirty.
+int finish(const Arg *a, int n, const char *what);
+
+// Metadata default of a scalar argument: all 8 bytes zero but the member set.
+halide_scalar_value_t scalar_i32(int32_t v);
+halide_scalar_value_t scalar_f32(float v);
+
+// F_argv: a pointer parameter receives args[i], a scalar parameter *(T *)args[i].
+template<typename T>
+T argv_slot(void *p) {
+    if constexpr (std::is_pointer_v<T>) return static_cast<T>(p);
+    else return *static_cast<T *>(p);
 }
-
-// null → -12, type → -3, dimensions → -43.  (Extent/stride checks need the required region and
-// are done by check_shape after the bounds-query early-out, as in the generated prologue.)
-int check_arg(const halide_buffer_t *b, const ArgSpec &spec);
-
-// negative extent → -28, |extent*stride| and allocation size limits → -5/-6, stride[0] != 1 → -8.
-int check_shape(const halide_buffer_t *b, const ArgSpec &spec);
-
-// required [min, min+extent) per dimension must lie inside the buffer → else -4.
-int check_covers(const halide_buffer_t *b, const ArgSpec &spec, int dim, int req_min, int req_extent);
-
-// Bounds-query answer: write min/extent and dense strides (src/AddImageChecks.cpp:386-436).
-void propose_shape(halide_buffer_t *b, const int *mins, const int *extents);
-
-// ---- residency -------------------------------------------------------------------------------
-// Make the buffer's contents available on the device and return the device address of the
-// element at the mins.  Inputs: allocate + H2D when host_dirty or no device allocation yet.
-// Outputs: allocate only.  Returns 0 or a negative halide_error_code_t.
-int acquire_input(halide_buffer_t *b, const ArgSpec &spec, void **dev_ptr);
-int acquire_output(halide_buffer_t *b, const ArgSpec &spec, void **dev_ptr);
-void mark_output_written(halide_buffer_t *b);
+template<typename... A, size_t... I>
+int call_argv(int (*f)(A...), void **args, std::index_sequence<I...>) {
+    return f(argv_slot<A>(args[I])...);
+}
+template<typename... A>
+int call_argv(int (*f)(A...), void **args) {
+    return call_argv(f, args, std::index_sequence_for<A...>{});
+}
 
 inline size_t elem_bytes(const halide_buffer_t *b) {
     return (b->type.bits + 7) / 8;
 }
 
 }  // namespace hb
+
+// The exports of a Halide AOT filter F besides F itself: F_argv and F_metadata, whose record lists
+// ARGS (the filter's halide_filter_argument_t array).
+#define HB_METADATA(NAME, ARGS)                                                                       \
+    extern "C" const halide_filter_metadata_t *NAME##_metadata(void) {                               \
+        static const halide_filter_metadata_t m = {1, (int32_t)(sizeof(ARGS) / sizeof(ARGS[0])), ARGS, \
+                                                   hb::kTarget, #NAME};                               \
+        return &m;                                                                                    \
+    }
+#define HB_EXPORT_FILTER(F, ARGS)                                      \
+    extern "C" int F##_argv(void **args) { return hb::call_argv(F, args); } \
+    HB_METADATA(F, ARGS)
+// The harnesses' second AOT variant (apps/*/process.cpp link F_auto_schedule too): the same code
+// under the other names.
+#define HB_EXPORT_AUTO_SCHEDULE(F, ARGS)                                                 \
+    extern "C" decltype(F) F##_auto_schedule __attribute__((alias(#F)));                \
+    extern "C" int F##_auto_schedule_argv(void **) __attribute__((alias(#F "_argv"))); \
+    HB_METADATA(F##_auto_schedule, ARGS)
 
 // Launch macro: counts the launch, optionally brackets it with events for the per-kernel
 // profile (halide_b200_profile_*), and surfaces launch-configuration errors immediately.

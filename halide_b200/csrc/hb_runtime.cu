@@ -517,112 +517,163 @@ void scratch_free(void *p) {
     pool().free(p);
 }
 
-static const char *kind(const ArgSpec &s) {
-    return s.is_output ? "Output" : "Input";
+static bool is_output(const halide_filter_argument_t &m) {
+    return m.kind == halide_argument_kind_output_buffer;
+}
+static const char *kind(const halide_filter_argument_t &m) {
+    return is_output(m) ? "Output" : "Input";
 }
 
-int check_arg(const halide_buffer_t *b, const ArgSpec &spec) {
-    if (!b) {
-        return fail(halide_error_code_buffer_argument_is_null, "Buffer argument %s is nullptr", spec.name);
-    }
-    // Compare code+bits only: this reference keeps the upper 16 bits reserved=0 while Halide
-    // releases store lanes=1 there (SURVEY.md §8b "Type word").
-    if (b->type.code != spec.code || b->type.bits != spec.bits) {
-        return fail(halide_error_code_bad_type, "%s buffer %s has type code %d bits %d but expected code %d bits %d",
-                    kind(spec), spec.name, b->type.code, b->type.bits, spec.code, spec.bits);
-    }
-    if (b->dimensions != spec.dimensions) {
-        return fail(halide_error_code_bad_dimensions, "%s buffer %s requires a buffer of exactly %d dimensions, but the buffer passed in has %d dimensions",
-                    kind(spec), spec.name, spec.dimensions, b->dimensions);
-    }
-    if (b->dimensions > 0 && !b->dim) {
-        return fail(halide_error_code_buffer_is_null, "%s buffer %s has a null dim array", kind(spec), spec.name);
-    }
-    return 0;
-}
-
-int check_shape(const halide_buffer_t *b, const ArgSpec &spec) {
-    int64_t total = 1;
+Region region_of(const halide_buffer_t *b, bool must_cover) {
+    Region r = {};
     for (int d = 0; d < b->dimensions; d++) {
-        const halide_dimension_t &dm = b->dim[d];
-        if (dm.extent < 0) {
-            return fail(halide_error_code_buffer_extents_negative, "The extents for buffer %s dimension %d is negative (%d)",
-                        spec.name, d, dm.extent);
-        }
-        int64_t stride = dm.stride < 0 ? -(int64_t)dm.stride : dm.stride;
-        int64_t sz = (int64_t)dm.extent * stride;
-        if (sz > 0x7fffffffLL) {
-            return fail(halide_error_code_buffer_allocation_too_large,
-                        "Total allocation for buffer %s is %lld, which exceeds the maximum size of 2147483647",
-                        spec.name, (long long)sz);
-        }
-        total *= dm.extent;
-        if (total > 0x7fffffffLL) {
-            return fail(halide_error_code_buffer_extents_too_large,
-                        "Product of extents for buffer %s is %lld, which exceeds the maximum size of 2147483647",
-                        spec.name, (long long)total);
-        }
+        r.min[d] = b->dim[d].min;
+        r.extent[d] = b->dim[d].extent;
     }
-    if (b->dimensions > 0 && b->dim[0].stride != 1) {
-        return fail(halide_error_code_constraint_violated, "Constraint violated: %s.stride.0 (%d) == 1 (1)",
-                    spec.name, b->dim[0].stride);
+    r.must_cover = must_cover;
+    return r;
+}
+
+int check_args(const Arg *a, int n) {
+    for (int i = 0; i < n; i++) {
+        const halide_buffer_t *b = a[i].b;
+        const halide_filter_argument_t &m = a[i].meta;
+        if (!b) {
+            return fail(halide_error_code_buffer_argument_is_null, "Buffer argument %s is nullptr", m.name);
+        }
+        // Compare code+bits only: this reference keeps the upper 16 bits reserved=0 while Halide
+        // releases store lanes=1 there (SURVEY.md §8b "Type word").
+        if (b->type.code != m.type.code || b->type.bits != m.type.bits) {
+            return fail(halide_error_code_bad_type, "%s buffer %s has type code %d bits %d but expected code %d bits %d",
+                        kind(m), m.name, b->type.code, b->type.bits, m.type.code, m.type.bits);
+        }
+        if (b->dimensions != m.dimensions) {
+            return fail(halide_error_code_bad_dimensions, "%s buffer %s requires a buffer of exactly %d dimensions, but the buffer passed in has %d dimensions",
+                        kind(m), m.name, m.dimensions, b->dimensions);
+        }
+        if (b->dimensions > 0 && !b->dim) {
+            return fail(halide_error_code_buffer_is_null, "%s buffer %s has a null dim array", kind(m), m.name);
+        }
     }
     return 0;
 }
 
-int check_covers(const halide_buffer_t *b, const ArgSpec &spec, int d, int req_min, int req_extent) {
-    if (req_extent <= 0) return 0;
-    const halide_dimension_t &dm = b->dim[d];
-    int req_max = req_min + req_extent - 1;
-    int have_max = dm.min + dm.extent - 1;
-    if (req_min < dm.min || req_max > have_max) {
-        return fail(halide_error_code_access_out_of_bounds,
-                    "%s buffer %s is accessed at %d, which is %s the %s (%d) in dimension %d",
-                    kind(spec), spec.name, req_min < dm.min ? req_min : req_max,
-                    req_min < dm.min ? "before" : "beyond", req_min < dm.min ? "min" : "max",
-                    req_min < dm.min ? dm.min : have_max, d);
+bool answer_bounds_query(Arg *a, const Region *need, int n) {
+    bool query = false;
+    for (int i = 0; i < n; i++) {
+        halide_buffer_t *b = a[i].b;
+        if (b->host != nullptr || b->device != 0) continue;
+        int64_t stride = 1;
+        for (int d = 0; d < b->dimensions; d++) {
+            b->dim[d].min = need[i].min[d];
+            b->dim[d].extent = need[i].extent[d];
+            b->dim[d].stride = (int32_t)stride;
+            stride *= need[i].extent[d];
+        }
+        query = true;
+    }
+    return query;
+}
+
+int check_shapes(const Arg *a, int n) {
+    for (int i = 0; i < n; i++) {
+        const halide_buffer_t *b = a[i].b;
+        const char *name = a[i].meta.name;
+        int64_t total = 1;
+        for (int d = 0; d < b->dimensions; d++) {
+            const halide_dimension_t &dm = b->dim[d];
+            if (dm.extent < 0) {
+                return fail(halide_error_code_buffer_extents_negative, "The extents for buffer %s dimension %d is negative (%d)",
+                            name, d, dm.extent);
+            }
+            int64_t stride = dm.stride < 0 ? -(int64_t)dm.stride : dm.stride;
+            int64_t sz = (int64_t)dm.extent * stride;
+            if (sz > 0x7fffffffLL) {
+                return fail(halide_error_code_buffer_allocation_too_large,
+                            "Total allocation for buffer %s is %lld, which exceeds the maximum size of 2147483647",
+                            name, (long long)sz);
+            }
+            total *= dm.extent;
+            if (total > 0x7fffffffLL) {
+                return fail(halide_error_code_buffer_extents_too_large,
+                            "Product of extents for buffer %s is %lld, which exceeds the maximum size of 2147483647",
+                            name, (long long)total);
+            }
+        }
+        if (b->dimensions > 0 && b->dim[0].stride != 1) {
+            return fail(halide_error_code_constraint_violated, "Constraint violated: %s.stride.0 (%d) == 1 (1)",
+                        name, b->dim[0].stride);
+        }
     }
     return 0;
 }
 
-void propose_shape(halide_buffer_t *b, const int *mins, const int *extents) {
-    int64_t stride = 1;
-    for (int d = 0; d < b->dimensions; d++) {
-        b->dim[d].min = mins[d];
-        b->dim[d].extent = extents[d];
-        b->dim[d].stride = (int32_t)stride;
-        stride *= extents[d];
+int check_required(const Arg *a, const Region *need, int n) {
+    for (int i = 0; i < n; i++) {
+        if (!need[i].must_cover) continue;
+        const halide_filter_argument_t &m = a[i].meta;
+        for (int d = 0; d < a[i].b->dimensions; d++) {
+            const int req_min = need[i].min[d], req_extent = need[i].extent[d];
+            if (req_extent <= 0) continue;
+            const halide_dimension_t &dm = a[i].b->dim[d];
+            int req_max = req_min + req_extent - 1;
+            int have_max = dm.min + dm.extent - 1;
+            if (req_min < dm.min || req_max > have_max) {
+                return fail(halide_error_code_access_out_of_bounds,
+                            "%s buffer %s is accessed at %d, which is %s the %s (%d) in dimension %d",
+                            kind(m), m.name, req_min < dm.min ? req_min : req_max,
+                            req_min < dm.min ? "before" : "beyond", req_min < dm.min ? "min" : "max",
+                            req_min < dm.min ? dm.min : have_max, d);
+            }
+        }
     }
+    return 0;
 }
 
-int acquire_input(halide_buffer_t *b, const ArgSpec &spec, void **dev_ptr) {
-    if (b->device && b->device_interface != &g_cuda_interface) {
-        return fail(halide_error_code_incompatible_device_interface,
-                    "Input buffer %s has a device allocation of a different device interface", spec.name);
+int acquire(Arg *a, int n) {
+    for (int i = 0; i < n; i++) {
+        halide_buffer_t *b = a[i].b;
+        const halide_filter_argument_t &m = a[i].meta;
+        if (b->device && b->device_interface != &g_cuda_interface) {
+            return fail(halide_error_code_incompatible_device_interface,
+                        "%s buffer %s has a device allocation of a different device interface", kind(m), m.name);
+        }
+        int r;
+        if (is_output(m)) {
+            r = if_device_malloc(nullptr, b, &g_cuda_interface);
+        } else if (!b->device && !b->host) {
+            r = fail(halide_error_code_host_is_null, "Input buffer %s has neither host nor device memory", m.name);
+        } else {
+            r = if_copy_to_device(nullptr, b, &g_cuda_interface);
+        }
+        if (r) return r;
+        a[i].dev = (void *)b->device;
     }
-    if (!b->device && !b->host) {
-        return fail(halide_error_code_host_is_null, "Input buffer %s has neither host nor device memory", spec.name);
-    }
-    int r = if_copy_to_device(nullptr, b, &g_cuda_interface);
+    return 0;
+}
+
+int finish(const Arg *a, int n, const char *what) {
+    int r = check_cuda(cudaGetLastError(), what, halide_error_code_device_run_failed);
     if (r) return r;
-    *dev_ptr = (void *)b->device;
-    return 0;
-}
-
-int acquire_output(halide_buffer_t *b, const ArgSpec &spec, void **dev_ptr) {
-    if (b->device && b->device_interface != &g_cuda_interface) {
-        return fail(halide_error_code_incompatible_device_interface,
-                    "Output buffer %s has a device allocation of a different device interface", spec.name);
+    for (int i = 0; i < n; i++) {
+        if (!is_output(a[i].meta)) continue;
+        a[i].b->flags &= ~(uint64_t)halide_buffer_flag_host_dirty;
+        a[i].b->flags |= halide_buffer_flag_device_dirty;
     }
-    int r = if_device_malloc(nullptr, b, &g_cuda_interface);
-    if (r) return r;
-    *dev_ptr = (void *)b->device;
     return 0;
 }
 
-void mark_output_written(halide_buffer_t *b) {
-    b->flags &= ~(uint64_t)halide_buffer_flag_host_dirty;
-    b->flags |= halide_buffer_flag_device_dirty;
+halide_scalar_value_t scalar_i32(int32_t v) {
+    halide_scalar_value_t s;
+    memset(&s, 0, sizeof(s));
+    s.u.i32 = v;
+    return s;
+}
+halide_scalar_value_t scalar_f32(float v) {
+    halide_scalar_value_t s;
+    memset(&s, 0, sizeof(s));
+    s.u.f32 = v;
+    return s;
 }
 
 }  // namespace hb
@@ -780,7 +831,7 @@ uint64_t halide_b200_kernel_launch_count(void) {
     return g_launches.load();
 }
 const char *halide_b200_target(void) {
-    return "x86-64-linux-cuda-cuda_capability_90-h100_native";
+    return hb::kTarget;
 }
 
 void halide_b200_set_timing(int enable) {

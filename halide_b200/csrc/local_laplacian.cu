@@ -30,19 +30,9 @@ using namespace llk;
 int g_shard_coarse_level = 0;  // halide_b200_ll_shard_coarse_level: 0 = choose by size, n >= 2 = gather level n
 int g_force_naive = 0;  // test hook bitmask (halide_b200_ll_force_generic): 1 = generic down kernels, 2 = generic up, 4 = generic final, 8 = no fused coarse launch, 16 = general-layout final kernel, 64 = no TMA frame tile in the final kernel, 256 = 48-row tiles in the TMA final kernel (default 32; 128 = 32 rows explicitly)
 
-const hb::ArgSpec kIn = {"input", halide_type_uint, 16, 3, false};
-const hb::ArgSpec kOut = {"output", halide_type_uint, 16, 3, true};
-
 int64_t est_i[3][2] = {{0, 1536}, {0, 2560}, {0, 3}};
 const int64_t *const est_ptrs[6] = {&est_i[0][0], &est_i[0][1], &est_i[1][0], &est_i[1][1], &est_i[2][0], &est_i[2][1]};
-halide_scalar_value_t sv_levels, sv_alpha, sv_beta;
-struct InitScalars {
-    InitScalars() {
-        sv_levels.u.i64 = 0; sv_levels.u.i32 = 8;
-        sv_alpha.u.i64 = 0; sv_alpha.u.f32 = 1.0f;
-        sv_beta.u.i64 = 0; sv_beta.u.f32 = 1.0f;
-    }
-} init_scalars;
+const halide_scalar_value_t sv_levels = hb::scalar_i32(8), sv_alpha = hb::scalar_f32(1.0f), sv_beta = hb::scalar_f32(1.0f);
 // Argument records as the generator declares them (generator :12-16, estimates :92-99).
 const halide_filter_argument_t kArgs[5] = {
     {"input", halide_argument_kind_input_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
@@ -51,10 +41,6 @@ const halide_filter_argument_t kArgs[5] = {
     {"beta", halide_argument_kind_input_scalar, 0, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, &sv_beta, nullptr},
     {"output", halide_argument_kind_output_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
-const halide_filter_metadata_t kMeta = {1, 5, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "local_laplacian"};
-const halide_filter_metadata_t kMetaAuto = {1, 5, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native",
-                                            "local_laplacian_auto_schedule"};
-
 
 // Everything one call needs on the device: frame description + per-level buffers.
 struct Plan {
@@ -66,32 +52,18 @@ struct Plan {
     float *lut;
 };
 
-int check_and_query(halide_buffer_t *input, int levels, halide_buffer_t *output, bool *done) {
+// The checks local_laplacian and its sharded variant share, on args = {input, output}.  *done: return r now (an error,
+// a bounds query or an empty output).
+int check_and_query(hb::Arg *args, int levels, bool *done) {
     int r;
     *done = true;
-    if ((r = hb::check_arg(input, kIn))) return r;
-    if ((r = hb::check_arg(output, kOut))) return r;
-    // Bounds query: the only access that bypasses repeat_edge is input(x,y,c) in `color`
-    // (generator :84), so the input must cover exactly the output region.
-    bool query = false;
-    {
-        int mins[3] = {output->dim[0].min, output->dim[1].min, output->dim[2].min};
-        int ext[3] = {output->dim[0].extent, output->dim[1].extent, output->dim[2].extent};
-        if (hb::is_bounds_query(input)) {
-            hb::propose_shape(input, mins, ext);
-            query = true;
-        }
-        if (hb::is_bounds_query(output)) {
-            hb::propose_shape(output, mins, ext);
-            query = true;
-        }
-    }
-    if (query) return 0;
-    if ((r = hb::check_shape(input, kIn))) return r;
-    if ((r = hb::check_shape(output, kOut))) return r;
-    for (int d = 0; d < 3; d++) {
-        if ((r = hb::check_covers(input, kIn, d, output->dim[d].min, output->dim[d].extent))) return r;
-    }
+    if ((r = hb::check_args(args, 2))) return r;
+    // The only access that bypasses repeat_edge is input(x,y,c) in `color` (generator :84), so the input must cover
+    // exactly the output region.
+    const halide_buffer_t *output = args[1].b;
+    const hb::Region need[2] = {hb::region_of(output, true), hb::region_of(output, false)};
+    if (hb::answer_bounds_query(args, need, 2)) return 0;
+    if ((r = hb::check_shapes(args, 2)) || (r = hb::check_required(args, need, 2))) return r;
     if (levels < 2 || levels > 32) {
         // 1/(levels-1) (generator :41) is meaningless below 2; the reference does not check, we do.
         return hb::fail(levels < 2 ? halide_error_code_param_too_small : halide_error_code_param_too_large,
@@ -102,17 +74,17 @@ int check_and_query(halide_buffer_t *input, int levels, halide_buffer_t *output,
     return 0;
 }
 
-void fill_frame(Plan &p, halide_buffer_t *input, halide_buffer_t *output, void *din, void *dout, int levels, float alpha,
-                float beta) {
+void fill_frame(Plan &p, const hb::Arg *args, int levels, float alpha, float beta) {
+    const halide_buffer_t *input = args[0].b, *output = args[1].b;
     LLFrame &f = p.f;
-    f.in = (const uint16_t *)din;
+    f.in = (const uint16_t *)args[0].dev;
     f.in_sy = input->dim[1].stride; f.in_sc = input->dim[2].stride;
     f.in_x0 = input->dim[0].min; f.in_y0 = input->dim[1].min; f.in_c0 = input->dim[2].min;
     f.in_w = input->dim[0].extent; f.in_h = input->dim[1].extent; f.in_c = input->dim[2].extent;
     f.clamp_y0 = f.in_y0; f.clamp_h = f.in_h;
     f.halo_top = f.halo_bot = nullptr;
     f.halo_top_rows = f.halo_bot_rows = f.halo_pitch = 0;
-    f.out = (uint16_t *)dout;
+    f.out = (uint16_t *)args[1].dev;
     f.out_sy = output->dim[1].stride; f.out_sc = output->dim[2].stride;
     f.out_x0 = output->dim[0].min; f.out_y0 = output->dim[1].min; f.out_c0 = output->dim[2].min;
     f.W = output->dim[0].extent; f.H = output->dim[1].extent; f.C = output->dim[2].extent;
@@ -400,16 +372,17 @@ void run_coarse_sweep(Plan &p, int from_level, cudaStream_t s) {
     for (int j = j0; j > from_level; j--) launch_up(p, j, s);
 }
 
-int run_local_laplacian(halide_buffer_t *input, int levels, float alpha, float beta, halide_buffer_t *output) {
+}  // namespace
+
+extern "C" int local_laplacian(halide_buffer_t *input, int32_t levels, float alpha, float beta, halide_buffer_t *output) {
     int r;
     bool done;
-    if ((r = check_and_query(input, levels, output, &done)) || done) return r;
-    void *din = nullptr, *dout = nullptr;
-    if ((r = hb::acquire_input(input, kIn, &din))) return r;
-    if ((r = hb::acquire_output(output, kOut, &dout))) return r;
+    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[4]}};
+    if ((r = check_and_query(args, levels, &done)) || done) return r;
+    if ((r = hb::acquire(args, 2))) return r;
 
     Plan p;
-    fill_frame(p, input, output, din, dout, levels, alpha, beta);
+    fill_frame(p, args, levels, alpha, beta);
     const int W = p.f.W, H = p.f.H;
     Span outx = {p.f.out_x0, p.f.out_x0 + W - 1}, outy = {p.f.out_y0, p.f.out_y0 + H - 1};
     Span inx = {p.f.in_x0, p.f.in_x0 + p.f.in_w - 1}, iny = {p.f.in_y0, p.f.in_y0 + p.f.in_h - 1};
@@ -424,10 +397,13 @@ int run_local_laplacian(halide_buffer_t *input, int levels, float alpha, float b
         run_coarse_sweep(p, 0, s);
         launch_final(p, s);
     }
-    if ((r = hb::check_cuda(cudaGetLastError(), "local_laplacian launch", halide_error_code_device_run_failed))) return r;
-    hb::mark_output_written(output);
-    return 0;
+    return hb::finish(args, 2, "local_laplacian launch");
 }
+HB_EXPORT_FILTER(local_laplacian, kArgs)
+// The harness's second AOT variant (apps/local_laplacian/process.cpp:44-48): same implementation.
+HB_EXPORT_AUTO_SCHEDULE(local_laplacian, kArgs)
+
+namespace {
 
 // Row-sharded path: the level gathered all-to-all (levels from it upwards are replicated on every rank).
 // Depends only on the whole frame's geometry and the rank count, so every rank computes the same value.
@@ -471,7 +447,8 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
                                 int frame_y_min, int frame_y_extent) {
     int r;
     bool done;
-    if ((r = check_and_query(input, levels, output, &done)) || done) return r;
+    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[4]}};
+    if ((r = check_and_query(args, levels, &done)) || done) return r;
     if (!hbdist::active()) {
         return hb::fail(halide_error_code_generic_error, "local_laplacian_sharded: call halide_b200_dist_init first");
     }
@@ -491,12 +468,10 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
     if (input->dim[0].min != output->dim[0].min || input->dim[0].extent != output->dim[0].extent) {
         return hb::fail(halide_error_code_constraint_violated, "local_laplacian_sharded: input and output bands must span the same columns");
     }
-    void *din = nullptr, *dout = nullptr;
-    if ((r = hb::acquire_input(input, kIn, &din))) return r;
-    if ((r = hb::acquire_output(output, kOut, &dout))) return r;
+    if ((r = hb::acquire(args, 2))) return r;
 
     Plan p;
-    fill_frame(p, input, output, din, dout, levels, alpha, beta);
+    fill_frame(p, args, levels, alpha, beta);
     const int W = p.f.W, C = p.f.in_c;
     Span outx = {p.f.out_x0, p.f.out_x0 + W - 1};
     Span inx = {p.f.in_x0, p.f.in_x0 + p.f.in_w - 1};
@@ -598,7 +573,7 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
             hbdist::Msg msgs[4];
             int n = 0;
             for (int c = 0; c < C; c++) {
-                const uint16_t *plane = (const uint16_t *)din + (int64_t)c * p.f.in_sc;
+                const uint16_t *plane = p.f.in + (int64_t)c * p.f.in_sc;
                 if (up_need) {
                     cudaMemcpy2DAsync(send_up + (size_t)c * up_need * p.f.in_w, rowb, plane, (size_t)p.f.in_sy * sizeof(uint16_t), rowb,
                                       up_need, cudaMemcpyDeviceToDevice, xs);
@@ -686,34 +661,10 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
         for (int j = jr - 1; j >= 1; j--) launch_up(p, j, s);
         launch_final(p, s);
     }
-    if ((r = hb::check_cuda(cudaGetLastError(), "local_laplacian_sharded launch", halide_error_code_device_run_failed))) return r;
-    hb::mark_output_written(output);
-    return 0;
+    return hb::finish(args, 2, "local_laplacian_sharded launch");
 }
 
 }  // namespace
-
-extern "C" int local_laplacian(halide_buffer_t *input, int32_t levels, float alpha, float beta, halide_buffer_t *output) {
-    return run_local_laplacian(input, levels, alpha, beta, output);
-}
-extern "C" int local_laplacian_argv(void **args) {
-    return run_local_laplacian((halide_buffer_t *)args[0], *(int32_t *)args[1], *(float *)args[2], *(float *)args[3],
-                               (halide_buffer_t *)args[4]);
-}
-extern "C" const halide_filter_metadata_t *local_laplacian_metadata(void) {
-    return &kMeta;
-}
-// The harness's second AOT variant (apps/local_laplacian/process.cpp:44-48): same implementation.
-extern "C" int local_laplacian_auto_schedule(halide_buffer_t *input, int32_t levels, float alpha, float beta,
-                                             halide_buffer_t *output) {
-    return run_local_laplacian(input, levels, alpha, beta, output);
-}
-extern "C" int local_laplacian_auto_schedule_argv(void **args) {
-    return local_laplacian_argv(args);
-}
-extern "C" const halide_filter_metadata_t *local_laplacian_auto_schedule_metadata(void) {
-    return &kMetaAuto;
-}
 
 // Test hook: route K == 8 calls through the generic (any `levels`) kernels so both paths stay covered.
 extern "C" void halide_b200_ll_force_generic(int enable) {

@@ -210,18 +210,9 @@ constexpr size_t nl_window_smem() {
 constexpr bool kDefaultWindow = true;  // (the register-window kernel: bit-identical to the first kernel, tests/test_nl_means_gpu.py)
 int g_variant = 0;  // test / A-B hook (halide_b200_nl_means_variant): 0 = default, 1 = generic kernel, 2 = register-window kernel
 
-const hb::ArgSpec kIn = {"input", halide_type_float, 32, 3, false};
-const hb::ArgSpec kOut = {"non_local_means", halide_type_float, 32, 3, true};
 int64_t est_i[3][2] = {{0, 1536}, {0, 2560}, {0, 3}};
 const int64_t *const est_ptrs[6] = {&est_i[0][0], &est_i[0][1], &est_i[1][0], &est_i[1][1], &est_i[2][0], &est_i[2][1]};
-halide_scalar_value_t sv_patch, sv_search, sv_sigma;
-struct InitScalars {
-    InitScalars() {
-        sv_patch.u.i64 = 0; sv_patch.u.i32 = 7;
-        sv_search.u.i64 = 0; sv_search.u.i32 = 7;
-        sv_sigma.u.i64 = 0; sv_sigma.u.f32 = 0.12f;
-    }
-} init_scalars;
+const halide_scalar_value_t sv_patch = hb::scalar_i32(7), sv_search = hb::scalar_i32(7), sv_sigma = hb::scalar_f32(0.12f);
 const halide_filter_argument_t kArgs[5] = {
     {"input", halide_argument_kind_input_buffer, 3, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
     {"patch_size", halide_argument_kind_input_scalar, 0, {halide_type_int, 32, 0}, nullptr, nullptr, nullptr, &sv_patch, nullptr},
@@ -229,25 +220,21 @@ const halide_filter_argument_t kArgs[5] = {
     {"sigma", halide_argument_kind_input_scalar, 0, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, &sv_sigma, nullptr},
     {"non_local_means", halide_argument_kind_output_buffer, 3, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
-const halide_filter_metadata_t kMeta = {1, 5, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "nl_means"};
-const halide_filter_metadata_t kMetaAuto = {1, 5, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native",
-                                            "nl_means_auto_schedule"};
+}  // namespace
 
-int run_nl_means(halide_buffer_t *input, int patch_size, int search_area, float sigma, halide_buffer_t *output) {
+extern "C" void halide_b200_nl_means_variant(int v) {
+    g_variant = v;
+}
+
+extern "C" int nl_means(halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma, halide_buffer_t *output) {
     int r;
-    if ((r = hb::check_arg(input, kIn))) return r;
-    if ((r = hb::check_arg(output, kOut))) return r;
-    bool query = false;
-    {
-        // every input access is clamped: a query is answered with the output's x/y region and 3 channels
-        int mins[3] = {output->dim[0].min, output->dim[1].min, 0};
-        int ext[3] = {output->dim[0].extent, output->dim[1].extent, 3};
-        if (hb::is_bounds_query(input)) { hb::propose_shape(input, mins, ext); query = true; }
-        if (hb::is_bounds_query(output)) { hb::propose_shape(output, mins, ext); query = true; }
-    }
-    if (query) return 0;
-    if ((r = hb::check_shape(input, kIn))) return r;
-    if ((r = hb::check_shape(output, kOut))) return r;
+    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[4]}};
+    if ((r = hb::check_args(args, 2))) return r;
+    // every input access is clamped: a query is answered with the output's x/y region and 3 channels
+    const hb::Region region = {{output->dim[0].min, output->dim[1].min, 0}, {output->dim[0].extent, output->dim[1].extent, 3}, false};
+    const hb::Region need[2] = {region, region};
+    if (hb::answer_bounds_query(args, need, 2)) return 0;
+    if ((r = hb::check_shapes(args, 2))) return r;
     // explicit constraint: non_local_means.dim(2).set_bounds(0, 3) (generator :68)
     if (output->dim[2].min != 0 || output->dim[2].extent != 3) {
         return hb::fail(halide_error_code_constraint_violated,
@@ -264,16 +251,14 @@ int run_nl_means(halide_buffer_t *input, int patch_size, int search_area, float 
                         "nl_means: patch_size %d / search_area %d outside the supported range [1,31] / [1,63]", patch_size,
                         search_area);
     }
-    void *din = nullptr, *dout = nullptr;
-    if ((r = hb::acquire_input(input, kIn, &din))) return r;
-    if ((r = hb::acquire_output(output, kOut, &dout))) return r;
+    if ((r = hb::acquire(args, 2))) return r;
 
     NLParams q;
-    q.in = (const float *)din;
+    q.in = (const float *)args[0].dev;
     q.in_sy = input->dim[1].stride; q.in_sc = input->dim[2].stride;
     q.in_x0 = input->dim[0].min; q.in_y0 = input->dim[1].min; q.in_c0 = input->dim[2].min;
     q.in_w = input->dim[0].extent; q.in_h = input->dim[1].extent; q.in_c = input->dim[2].extent;
-    q.out = (float *)dout;
+    q.out = (float *)args[1].dev;
     q.out_sy = output->dim[1].stride; q.out_sc = output->dim[2].stride;
     q.out_x0 = output->dim[0].min; q.out_y0 = output->dim[1].min; q.W = W; q.H = H;
     q.p = patch_size; q.s = search_area;
@@ -311,34 +296,7 @@ int run_nl_means(halide_buffer_t *input, int patch_size, int search_area, float 
             HB_LAUNCH("nl_means", nl_means_kernel, grid, 256, smem, s, q);
         }
     }
-    if ((r = hb::check_cuda(cudaGetLastError(), "nl_means launch", halide_error_code_device_run_failed))) return r;
-    hb::mark_output_written(output);
-    return 0;
+    return hb::finish(args, 2, "nl_means launch");
 }
-
-}  // namespace
-
-extern "C" void halide_b200_nl_means_variant(int v) {
-    g_variant = v;
-}
-
-extern "C" int nl_means(halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma, halide_buffer_t *output) {
-    return run_nl_means(input, patch_size, search_area, sigma, output);
-}
-extern "C" int nl_means_argv(void **args) {
-    return run_nl_means((halide_buffer_t *)args[0], *(int32_t *)args[1], *(int32_t *)args[2], *(float *)args[3],
-                        (halide_buffer_t *)args[4]);
-}
-extern "C" const halide_filter_metadata_t *nl_means_metadata(void) {
-    return &kMeta;
-}
-extern "C" int nl_means_auto_schedule(halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma,
-                                      halide_buffer_t *output) {
-    return run_nl_means(input, patch_size, search_area, sigma, output);
-}
-extern "C" int nl_means_auto_schedule_argv(void **args) {
-    return nl_means_argv(args);
-}
-extern "C" const halide_filter_metadata_t *nl_means_auto_schedule_metadata(void) {
-    return &kMetaAuto;
-}
+HB_EXPORT_FILTER(nl_means, kArgs)
+HB_EXPORT_AUTO_SCHEDULE(nl_means, kArgs)

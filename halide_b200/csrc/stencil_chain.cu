@@ -227,42 +227,33 @@ __global__ void __launch_bounds__(256) stencil_chain_window_kernel(Plane p) {
 constexpr bool kDefaultWindow = true;  // (the register-window kernel: bit-identical to the first kernel, tests/test_stencil_chain_gpu.py)
 int g_variant = 0;  // test / A-B hook (halide_b200_stencil_chain_variant): 0 = default, 1 = one-pixel-per-thread kernel, 2 = register-window kernel
 
-const hb::ArgSpec kIn = {"input", halide_type_uint, 16, 2, false};
-const hb::ArgSpec kOut = {"output", halide_type_uint, 16, 2, true};
 int64_t est_i[2][2] = {{0, 1536}, {0, 2560}};
 const int64_t *const est_ptrs[4] = {&est_i[0][0], &est_i[0][1], &est_i[1][0], &est_i[1][1]};
 const halide_filter_argument_t kArgs[2] = {
     {"input", halide_argument_kind_input_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
     {"output", halide_argument_kind_output_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
-const halide_filter_metadata_t kMeta = {1, 2, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native", "stencil_chain"};
-const halide_filter_metadata_t kMetaAuto = {1, 2, kArgs, "x86-64-linux-cuda-cuda_capability_90-h100_native",
-                                            "stencil_chain_auto_schedule"};
+}  // namespace
 
-int run_stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
+extern "C" void halide_b200_stencil_chain_variant(int v) {
+    g_variant = v;
+}
+
+extern "C" int stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
     int r;
-    if ((r = hb::check_arg(input, kIn))) return r;
-    if ((r = hb::check_arg(output, kOut))) return r;
-    bool query = false;
-    {
-        // every access to the input goes through repeat_edge: nothing beyond a non-empty buffer is
-        // required; a query is answered with the output region.
-        int mins[2] = {output->dim[0].min, output->dim[1].min};
-        int ext[2] = {output->dim[0].extent, output->dim[1].extent};
-        if (hb::is_bounds_query(input)) { hb::propose_shape(input, mins, ext); query = true; }
-        if (hb::is_bounds_query(output)) { hb::propose_shape(output, mins, ext); query = true; }
-    }
-    if (query) return 0;
-    if ((r = hb::check_shape(input, kIn))) return r;
-    if ((r = hb::check_shape(output, kOut))) return r;
+    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[1]}};
+    if ((r = hb::check_args(args, 2))) return r;
+    // every access to the input goes through repeat_edge: nothing beyond a non-empty buffer is
+    // required; a query is answered with the output region.
+    const hb::Region need[2] = {hb::region_of(output, false), hb::region_of(output, false)};
+    if (hb::answer_bounds_query(args, need, 2)) return 0;
+    if ((r = hb::check_shapes(args, 2))) return r;
     const int W = output->dim[0].extent, H = output->dim[1].extent;
     if (W <= 0 || H <= 0) return 0;
     if (input->dim[0].extent <= 0 || input->dim[1].extent <= 0) {
         return hb::fail(halide_error_code_access_out_of_bounds, "Input buffer input is empty");
     }
-    void *din = nullptr, *dout = nullptr;
-    if ((r = hb::acquire_input(input, kIn, &din))) return r;
-    if ((r = hb::acquire_output(output, kOut, &dout))) return r;
+    if ((r = hb::acquire(args, 2))) return r;
 
     // ping-pong buffers for the intermediate stages on their grown regions
     const int groups = (kStages + kFuse - 1) / kFuse;
@@ -290,7 +281,7 @@ int run_stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
             p.src_w = W + 2 * Rin;
             p.src_h = H + 2 * Rin;
             if (g == 0) {
-                p.src = (const uint16_t *)din;
+                p.src = (const uint16_t *)args[0].dev;
                 p.src_sy = input->dim[1].stride;
                 p.do_clamp = 1;
                 // source-region local (0,0) is absolute (ox - Rin, oy - Rin); buffer-relative = minus input min
@@ -305,7 +296,7 @@ int run_stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
                 p.clamp_x0 = p.clamp_y0 = p.clamp_w = p.clamp_h = 0;
             }
             if (g == groups - 1) {
-                p.dst = (uint16_t *)dout;
+                p.dst = (uint16_t *)args[1].dev;
                 p.dst_sy = output->dim[1].stride;
             } else {
                 p.dst = buf[g & 1];
@@ -323,32 +314,7 @@ int run_stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
             done += fuse;
         }
     }
-    if ((r = hb::check_cuda(cudaGetLastError(), "stencil_chain launch", halide_error_code_device_run_failed))) return r;
-    hb::mark_output_written(output);
-    return 0;
+    return hb::finish(args, 2, "stencil_chain launch");
 }
-
-}  // namespace
-
-extern "C" void halide_b200_stencil_chain_variant(int v) {
-    g_variant = v;
-}
-
-extern "C" int stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
-    return run_stencil_chain(input, output);
-}
-extern "C" int stencil_chain_argv(void **args) {
-    return run_stencil_chain((halide_buffer_t *)args[0], (halide_buffer_t *)args[1]);
-}
-extern "C" const halide_filter_metadata_t *stencil_chain_metadata(void) {
-    return &kMeta;
-}
-extern "C" int stencil_chain_auto_schedule(halide_buffer_t *input, halide_buffer_t *output) {
-    return run_stencil_chain(input, output);
-}
-extern "C" int stencil_chain_auto_schedule_argv(void **args) {
-    return stencil_chain_argv(args);
-}
-extern "C" const halide_filter_metadata_t *stencil_chain_auto_schedule_metadata(void) {
-    return &kMetaAuto;
-}
+HB_EXPORT_FILTER(stencil_chain, kArgs)
+HB_EXPORT_AUTO_SCHEDULE(stencil_chain, kArgs)
