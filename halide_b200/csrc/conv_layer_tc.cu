@@ -17,8 +17,8 @@
 //                3-stage shared-memory ring, mbarrier complete_tx
 //   warps 0-7    two consumer warpgroups, one per 64-pixel half of the tile: 4 x 3 wgmma.m64n128k8 (TF32, both operands
 //                from shared memory) per stage into register accumulators, then + bias, relu and the stores
-#include <cuda.h>
 #include "hb_common.h"
+#include "hb_tma.cuh"
 
 namespace {
 
@@ -37,36 +37,11 @@ constexpr int B_TILE_BYTES = TILE_N * TILE_K * 4;  // 16 KB
 constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;  // A_hi, A_lo, B_hi, B_lo
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*alignment slack*/ + 256 /*barriers*/;
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE_%=;\n\t"
-        "bra WAIT_%=;\n\t"
-        "DONE_%=:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(dst)),
-                 "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-                 : "memory");
-}
 // K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma (PTX ISA "Matrix Descriptor Format"): start address >> 4
 // in [0,14), leading byte offset (unused for swizzled K-major, 1) in [16,30), stride byte offset 1024 B between 8-row
 // groups in [32,46), layout type 1 = 128-byte swizzle in [62,64).  The tile base must be 1024-byte aligned.
 __device__ __forceinline__ uint64_t wgmma_desc(const void *tile) {
-    return (uint64_t)((smem_u32(tile) & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
+    return (uint64_t)((tma::smem_u32(tile) & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -114,7 +89,7 @@ __global__ void conv_prep_filter_kernel(const float *__restrict__ f, float *__re
 __device__ __forceinline__ void consume_step(float (&d)[64], const uint8_t *tiles, uint64_t *full_bar, uint64_t *empty_bar, int it, int wg,
                                              int lane) {
     const int s = it % STAGES;
-    mbar_wait(&full_bar[s], (it / STAGES) & 1);
+    tma::mbar_wait(&full_bar[s], (it / STAGES) & 1);
     const uint8_t *st = tiles + s * STAGE_BYTES;
     const int a_off = wg * 64 * TILE_K * 4;  // this warpgroup's 64 rows of the A tiles (8 KB, a multiple of the 1024-byte swizzle atom)
     const uint64_t a_hi = wgmma_desc(st + a_off), a_lo = wgmma_desc(st + A_TILE_BYTES + a_off);
@@ -129,7 +104,7 @@ __device__ __forceinline__ void consume_step(float (&d)[64], const uint8_t *tile
     }
     wgmma_commit();
     wgmma_wait<1>();  // the previous K step's MMAs are done: its stage can be refilled
-    if (it > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+    if (it > 0 && lane == 0) tma::mbar_arrive(&empty_bar[(it - 1) % STAGES]);
 }
 
 __global__ void __launch_bounds__(THREADS, 1) conv_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
@@ -148,10 +123,10 @@ __global__ void __launch_bounds__(THREADS, 1) conv_layer_tc_kernel(const __grid_
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; s++) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], CONSUMER_WARPS);  // one arrival per consumer warp
+            tma::mbar_init(&full_bar[s], 1);
+            tma::mbar_init(&empty_bar[s], CONSUMER_WARPS);  // one arrival per consumer warp
         }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        tma::fence_barrier_init();
     }
     __syncthreads();
 
@@ -160,15 +135,15 @@ __global__ void __launch_bounds__(THREADS, 1) conv_layer_tc_kernel(const __grid_
             // ===== TMA producer =====
             for (int it = 0; it < K_STEPS; it++) {
                 const int s = it % STAGES, round = it / STAGES;
-                if (round > 0) mbar_wait(&empty_bar[s], (round - 1) & 1);
+                if (round > 0) tma::mbar_wait(&empty_bar[s], (round - 1) & 1);
                 const int tap = it / (CI / TILE_K), kc = it % (CI / TILE_K);
                 const int ky = tap / 3, kx = tap - ky * 3;
                 uint8_t *st = tiles + s * STAGE_BYTES;
-                mbar_expect_tx(&full_bar[s], STAGE_BYTES);
-                tma_load_2d(st, &map_a_hi, &full_bar[s], kc * TILE_K, a_row0 + ky * WP + kx);
-                tma_load_2d(st + A_TILE_BYTES, &map_a_lo, &full_bar[s], kc * TILE_K, a_row0 + ky * WP + kx);
-                tma_load_2d(st + 2 * A_TILE_BYTES, &map_b_hi, &full_bar[s], kc * TILE_K, tap * CO);
-                tma_load_2d(st + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_b_lo, &full_bar[s], kc * TILE_K, tap * CO);
+                tma::mbar_expect_tx(&full_bar[s], STAGE_BYTES);
+                tma::load_2d(st, &map_a_hi, &full_bar[s], kc * TILE_K, a_row0 + ky * WP + kx);
+                tma::load_2d(st + A_TILE_BYTES, &map_a_lo, &full_bar[s], kc * TILE_K, a_row0 + ky * WP + kx);
+                tma::load_2d(st + 2 * A_TILE_BYTES, &map_b_hi, &full_bar[s], kc * TILE_K, tap * CO);
+                tma::load_2d(st + 2 * A_TILE_BYTES + B_TILE_BYTES, &map_b_lo, &full_bar[s], kc * TILE_K, tap * CO);
             }
         }
         return;
@@ -208,42 +183,26 @@ __global__ void __launch_bounds__(THREADS, 1) conv_layer_tc_kernel(const __grid_
     }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                                  const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-int make_map(EncodeTiledFn enc, CUtensorMap *m, void *base, uint64_t rows, int box_rows) {
-    cuuint64_t dims[2] = {(cuuint64_t)CI, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)CI * sizeof(float)};
-    cuuint32_t box[2] = {(cuuint32_t)TILE_K, (cuuint32_t)box_rows};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS ? 0 : (int)r;
+bool make_map(CUtensorMap *m, void *base, uint64_t rows, uint32_t box_rows) {
+    const uint64_t dims[2] = {(uint64_t)CI, rows};
+    const int64_t strides[1] = {(int64_t)(CI * sizeof(float))};
+    const uint32_t box[2] = {(uint32_t)TILE_K, box_rows};
+    return tma::encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 }  // namespace
 
 // Returns 0 on success, a negative halide error code otherwise.  din/df/db/dout are device pointers in the generator's layouts.
 int conv_layer_tc_run(const float *din, const float *df, const float *db, float *dout, cudaStream_t s) {
-    static EncodeTiledFn enc = nullptr;
-    if (!enc) {
-        void *fn = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || !fn) {
-            cudaGetLastError();
-            return hb::fail(halide_error_code_generic_error, "conv_layer: cuTensorMapEncodeTiled is not available");
-        }
-        enc = (EncodeTiledFn)fn;
-    }
+    if (!tma::encoder()) return hb::fail(halide_error_code_generic_error, "conv_layer: cuTensorMapEncodeTiled is not available");
     hb::Scratch scratch;
     const size_t a_elems = (size_t)A_ROWS * CI, b_elems = (size_t)9 * CO * CI;
     float *a_hi = scratch.get<float>(a_elems), *a_lo = scratch.get<float>(a_elems);
     float *b_hi = scratch.get<float>(b_elems), *b_lo = scratch.get<float>(b_elems);
     if (!a_hi || !a_lo || !b_hi || !b_lo) return hb::fail(halide_error_code_device_malloc_failed, "conv_layer: scratch allocation failed");
     CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
-    if (make_map(enc, &ma_hi, a_hi, A_ROWS, TILE_M) || make_map(enc, &ma_lo, a_lo, A_ROWS, TILE_M) ||
-        make_map(enc, &mb_hi, b_hi, 9 * CO, TILE_N) || make_map(enc, &mb_lo, b_lo, 9 * CO, TILE_N)) {
+    if (!make_map(&ma_hi, a_hi, A_ROWS, TILE_M) || !make_map(&ma_lo, a_lo, A_ROWS, TILE_M) || !make_map(&mb_hi, b_hi, 9 * CO, TILE_N) ||
+        !make_map(&mb_lo, b_lo, 9 * CO, TILE_N)) {
         return hb::fail(halide_error_code_generic_error, "conv_layer: cuTensorMapEncodeTiled failed");
     }
     static hb::PerDeviceOnce attr;

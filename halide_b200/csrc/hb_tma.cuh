@@ -22,12 +22,11 @@ __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
 __device__ __forceinline__ void fence_barrier_init() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// make generic-proxy writes to shared memory visible to the async proxy (before a TMA store reads them)
-__device__ __forceinline__ void fence_proxy_async() {
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
 __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
     asm volatile(
@@ -47,25 +46,6 @@ __device__ __forceinline__ void load_3d(void *dst, const CUtensorMap *map, uint6
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(smem_u32(dst)),
                  "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
                  : "memory");
-}
-__device__ __forceinline__ void store_2d(const CUtensorMap *map, const void *src, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1)
-                 : "memory");
-}
-__device__ __forceinline__ void store_3d(const CUtensorMap *map, const void *src, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(map), "r"(smem_u32(src)), "r"(c0),
-                 "r"(c1), "r"(c2)
-                 : "memory");
-}
-__device__ __forceinline__ void store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// wait until the bulk stores of all but the newest `N` groups have finished READING their shared-memory source
-template<int N>
-__device__ __forceinline__ void store_wait_read() {
-    asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template<int N>
-__device__ __forceinline__ void store_wait() {
-    asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------------
@@ -95,10 +75,10 @@ inline bool strides_ok(const void *base, const int64_t *stride_bytes, int nstrid
     return true;
 }
 
-// rank-`rank` tiled map (no swizzle, no interleave, zero fill out of bounds): dims / box in elements, innermost first;
-// stride_bytes[i] = byte stride of dimension i+1.  Returns false when the driver refuses it.
+// rank-`rank` tiled map (no interleave, zero fill out of bounds): dims / box in elements, innermost first;
+// stride_bytes[i] = byte stride of dimension i+1.  Returns false when the driver refuses it or the encoder is missing.
 inline bool encode(CUtensorMap *m, CUtensorMapDataType type, int rank, void *base, const uint64_t *dims, const int64_t *stride_bytes,
-                   const uint32_t *box) {
+                   const uint32_t *box, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_NONE) {
     EncodeTiledFn enc = encoder();
     if (!enc) return false;
     cuuint64_t d[5], st[4];
@@ -109,7 +89,7 @@ inline bool encode(CUtensorMap *m, CUtensorMapDataType type, int rank, void *bas
         es[i] = 1;
         if (i + 1 < rank) st[i] = (cuuint64_t)stride_bytes[i];
     }
-    return enc(m, type, (cuuint32_t)rank, base, d, st, b, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+    return enc(m, type, (cuuint32_t)rank, base, d, st, b, es, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 

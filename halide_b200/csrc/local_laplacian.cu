@@ -28,7 +28,7 @@ namespace {
 using namespace llk;
 
 int g_shard_coarse_level = 0;  // halide_b200_ll_shard_coarse_level: 0 = choose by size, n >= 2 = gather level n
-int g_force_naive = 0;  // test hook bitmask (halide_b200_ll_force_generic): 1 = generic down kernels, 2 = generic up, 4 = generic final, 8 = no fused coarse launch, 16 = general-layout final kernel, 64 = no TMA frame tile in the final kernel, 256 = 48-row tiles in the TMA final kernel (default 32; 128 = 32 rows explicitly)
+int g_force_naive = 0;  // test hook bitmask (halide_b200_ll_force_generic): 1 = generic down kernels, 2 = generic up, 4 = generic final, 8 = no fused coarse launch, 16 = general-layout final kernel, 64 = no TMA frame tile in the final kernel
 
 int64_t est_i[3][2] = {{0, 1536}, {0, 2560}, {0, 3}};
 const int64_t *const est_ptrs[6] = {&est_i[0][0], &est_i[0][1], &est_i[1][0], &est_i[1][1], &est_i[2][0], &est_i[2][1]};
@@ -252,8 +252,8 @@ void launch_down(Plan &p, int j, cudaStream_t s) {  // produce level j (j >= 1) 
     }
 }
 
-dim3 up_grid(int x_lo, int x_hi, int y_lo, int y_hi, int th = kUpTH) {  // tiles on even absolute origins
-    return dim3((x_hi - (x_lo & ~1) + kUpTW) / kUpTW, (y_hi - (y_lo & ~1) + th) / th);
+dim3 up_grid(int x_lo, int x_hi, int y_lo, int y_hi) {  // tiles on even absolute origins
+    return dim3((x_hi - (x_lo & ~1) + kUpTW) / kUpTW, (y_hi - (y_lo & ~1) + kUpTH) / kUpTH);
 }
 
 void launch_up(Plan &p, int j, cudaStream_t s) {  // produce outGPyramid[j] (1 <= j <= J-1) rows coy
@@ -275,10 +275,6 @@ void launch_final(Plan &p, cudaStream_t s) {
     if (p.f.nrows <= 0) return;
     if (p.J > 1 && p.K == 8 && !(g_force_naive & 4) && p.f.C <= 3) {
         const LLFrame &f = p.f;
-        // 48-row tiles (hook bit 256) spread the per-block fixed work over 6 rows per thread instead of 4 at the cost of
-        // the fourth block per SM; 32-row tiles are the default.  Kept selectable for A/B runs (tools/ab_masks.py) and tested.
-        const bool tall = (g_force_naive & 256) && !(g_force_naive & 128);
-        const int th = tall ? kUpTHTall : kUpTH;
         // the common layout takes the kernel's ALIGNED path (32-bit addressing, one aligned word per thread and channel)
         const int64_t in_span = (int64_t)f.in_h * f.in_sy + 3 * f.in_sc, out_span = (int64_t)f.H * f.out_sy + 3 * f.out_sc;
         const bool aligned = f.C == 3 && f.in_c0 == 0 && f.out_c0 == 0 && f.in_c >= 3 && (f.W & 1) == 0 && (f.out_x0 & 1) == 0 &&
@@ -296,19 +292,17 @@ void launch_final(Plan &p, cudaStream_t s) {
             // (every tile's first column must also start on a 16-byte boundary: crops at other even offsets take the load path)
             if (tma::strides_ok(f.in, strides, 2) && (((f.out_x0 & ~1) - f.in_x0) & 7) == 0) {
                 const uint64_t dims[3] = {(uint64_t)f.in_w, (uint64_t)f.in_h, (uint64_t)f.in_c};
-                const uint32_t box[3] = {kUpInW, (uint32_t)th, 3};
+                const uint32_t box[3] = {kUpInW, kUpTH, 3};
                 use_tma = tma::encode(&in_map, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, (void *)f.in, dims, strides, box);
             }
         }
-        auto launch = [&](auto kern, bool tma_on, int tile_h = kUpTH) {
-            const int smem = up2_smem_bytes(true, tma_on, tile_h);
-            const dim3 g = up_grid(f.out_x0, f.out_x0 + f.W - 1, f.row0, f.row0 + f.nrows - 1, tile_h);
+        auto launch = [&](auto kern, bool tma_on) {
+            const int smem = up2_smem_bytes(true, tma_on);
+            const dim3 g = up_grid(f.out_x0, f.out_x0 + f.W - 1, f.row0, f.row0 + f.nrows - 1);
             (void)resident_slots(kern, 256, smem);  // (sets the > 48 KB shared-memory attribute once per kernel and device)
             HB_LAUNCH("ll_final2", kern, g, 256, smem, s, p.f, lb[1], lb[1], in_map);
         };
-        if (use_tma && beta1 && tall) launch((ll_up2_kernel<true, true, true, true, kUpTHTall>), true, kUpTHTall);
-        else if (use_tma && tall) launch((ll_up2_kernel<true, true, false, true, kUpTHTall>), true, kUpTHTall);
-        else if (use_tma && beta1) launch(ll_up2_kernel<true, true, true, true>, true);
+        if (use_tma && beta1) launch(ll_up2_kernel<true, true, true, true>, true);
         else if (use_tma) launch(ll_up2_kernel<true, true, false, true>, true);
         else if (aligned && beta1) launch(ll_up2_kernel<true, true, true, false>, false);
         else if (aligned) launch(ll_up2_kernel<true, true, false, false>, false);

@@ -207,8 +207,7 @@ constexpr size_t nl_window_smem() {
     return (size_t)(3 * (TY + P + S - 2) * (TX + P + S - 2) + S * TY * (TX + P - 1)) * sizeof(float);
 }
 
-constexpr bool kDefaultWindow = true;  // (the register-window kernel: bit-identical to the first kernel, tests/test_nl_means_gpu.py)
-int g_variant = 0;  // test / A-B hook (halide_b200_nl_means_variant): 0 = default, 1 = generic kernel, 2 = register-window kernel
+int g_variant = 0;  // test hook (halide_b200_nl_means_variant): 1 = generic kernel for every patch / search size
 
 int64_t est_i[3][2] = {{0, 1536}, {0, 2560}, {0, 3}};
 const int64_t *const est_ptrs[6] = {&est_i[0][0], &est_i[0][1], &est_i[1][0], &est_i[1][1], &est_i[2][0], &est_i[2][1]};
@@ -283,7 +282,7 @@ extern "C" int nl_means(halide_buffer_t *input, int32_t patch_size, int32_t sear
         // (the limit is per device; setting it is cheap, so it is simply set for every call that needs it)
         if (smem > 48 * 1024) cudaFuncSetAttribute(nl_means_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         dim3 grid((W + TX - 1) / TX, (H + TY - 1) / TY);
-        const bool window = g_variant == 2 || (g_variant == 0 && kDefaultWindow);
+        const bool window = g_variant != 1;
         if (window && patch_size == 3 && search_area == 7) {
             constexpr size_t sm = nl_window_smem<3, 7>();
             static_assert(sm <= 48 * 1024, "no opt-in needed");

@@ -13,14 +13,14 @@
 //
 // Kernel shape: ALU/shared-memory bound (800 MAC/px in the reference formulation, 4 B/px of
 // compulsory HBM traffic).  kFuse stages run per launch on a shared-memory tile with a 2*kFuse
-// apron, ping-ponging between two uint16 tiles; the frame itself (7.9 MB at the harness size)
-// stays L2-resident between launches.
+// apron; the frame itself (7.9 MB at the harness size) stays L2-resident between launches.
 #include "hb_common.h"
 
 namespace {
 
 constexpr int kStages = 32;  // GeneratorParam `stencils` of the shipped app (generator :9)
 constexpr int kFuse = 4;     // stages per launch
+static_assert(kStages % kFuse == 0, "every launch runs kFuse stages");
 constexpr int kTile = 64;    // output tile edge per block
 constexpr int kTileIn = kTile + 4 * kFuse;  // 80: input tile edge (2 px apron per fused stage, both sides)
 
@@ -32,70 +32,12 @@ struct Plane {
     // when reading the pipeline input: clamp coordinates into the buffer (repeat_edge)
     int clamp_x0, clamp_y0, clamp_w, clamp_h, do_clamp;
     int dst_w, dst_h;
-    int fuse;             // stages in this launch (<= kFuse)
     int src_words, dst_words;  // rows of src / dst keep pixel pairs 4-byte aligned (even stride, aligned base): 32-bit accesses
 };
 
-__global__ void __launch_bounds__(256) stencil_chain_fused_kernel(Plane p) {
-    __shared__ uint16_t A[kTileIn][kTileIn + 2];
-    __shared__ uint16_t B[kTileIn][kTileIn + 2];
-    __shared__ uint16_t C[kTileIn][kTileIn + 2];
-    const int tid = threadIdx.x;
-    const int ox = blockIdx.x * kTile, oy = blockIdx.y * kTile;  // tile origin in dst coordinates
-    const int in_edge = kTile + 4 * p.fuse;
-    // load the source tile: dst (ox,oy) corresponds to src (ox, oy) .. (ox+in_edge, oy+in_edge)
-    for (int t = tid; t < in_edge * in_edge; t += 256) {
-        int ly = t / in_edge, lx = t - ly * in_edge;
-        int sx = ox + lx, sy = oy + ly;
-        uint16_t v = 0;
-        if (p.do_clamp) {
-            // src points at absolute coordinate (src_x0, src_y0) folded into clamp_x0/y0 by the host:
-            int cx = min(max(sx + p.clamp_x0, 0), p.clamp_w - 1);
-            int cy = min(max(sy + p.clamp_y0, 0), p.clamp_h - 1);
-            v = p.src[(int64_t)cy * p.src_sy + cx];
-        } else if (sx < p.src_w && sy < p.src_h) {
-            v = p.src[(int64_t)sy * p.src_sy + sx];
-        }
-        A[ly][lx] = v;
-    }
-    __syncthreads();
-    int edge = in_edge;
-    uint16_t(*cur)[kTileIn + 2] = A;
-    uint16_t(*nxt)[kTileIn + 2] = B;
-    for (int s = 0; s < p.fuse; s++) {
-        // vertical pass: C[y][x] = sum_j (j+3) * cur[y+2+j][x], y in [0, edge-4)
-        const int vh = edge - 4;
-        for (int t = tid; t < vh * edge; t += 256) {
-            int ly = t / edge, lx = t - ly * edge;
-            uint32_t acc = 1u * cur[ly][lx] + 2u * cur[ly + 1][lx] + 3u * cur[ly + 2][lx] + 4u * cur[ly + 3][lx] +
-                           5u * cur[ly + 4][lx];
-            C[ly][lx] = (uint16_t)acc;
-        }
-        __syncthreads();
-        // horizontal pass: nxt[y][x] = sum_i (i+3) * C[y][x+2+i], x in [0, edge-4)
-        for (int t = tid; t < vh * vh; t += 256) {
-            int ly = t / vh, lx = t - ly * vh;
-            uint32_t acc = 1u * C[ly][lx] + 2u * C[ly][lx + 1] + 3u * C[ly][lx + 2] + 4u * C[ly][lx + 3] +
-                           5u * C[ly][lx + 4];
-            nxt[ly][lx] = (uint16_t)acc;
-        }
-        __syncthreads();
-        edge -= 4;
-        uint16_t(*tmp)[kTileIn + 2] = cur; cur = nxt; nxt = tmp;
-    }
-    // edge == kTile now
-    for (int t = tid; t < kTile * kTile; t += 256) {
-        int ly = t / kTile, lx = t - ly * kTile;
-        int dx = ox + lx, dy = oy + ly;
-        if (dx < p.dst_w && dy < p.dst_h) p.dst[(int64_t)dy * p.dst_sy + dx] = cur[ly][lx];
-    }
-}
-
-// ---- register-window version (kFuse stages per launch, same tiles) -----------------------------------------------
-// The kernel above spends ~135 instructions per pixel and stage: one pixel per thread and pass, five 16-bit shared
-// loads per output and an integer division per element for the tile coordinates.  Here the tile lives in shared memory
-// as 32-bit words (two pixels), every edge length is a compile-time constant, and each pass is a sliding window held
-// in registers:
+// ---- register-window kernel (kFuse stages per launch) -------------------------------------------------------------
+// The tile lives in shared memory as 32-bit words (two pixels), every edge length is a compile-time constant, and each
+// pass is a sliding window held in registers:
 //   vertical:   a thread owns a column PAIR on a segment of rows — per row one 32-bit load, eight multiply-adds (four
 //               per pixel: v0 + 2 v1 + 3 v2 + 4 v3 + 5 v4 starts from v0), one PRMT to repack, one 32-bit store;
 //   horizontal: a thread owns a row on a segment of output pairs — per output pair one new word, eight multiply-adds.
@@ -224,9 +166,6 @@ __global__ void __launch_bounds__(256) stencil_chain_window_kernel(Plane p) {
     }
 }
 
-constexpr bool kDefaultWindow = true;  // (the register-window kernel: bit-identical to the first kernel, tests/test_stencil_chain_gpu.py)
-int g_variant = 0;  // test / A-B hook (halide_b200_stencil_chain_variant): 0 = default, 1 = one-pixel-per-thread kernel, 2 = register-window kernel
-
 int64_t est_i[2][2] = {{0, 1536}, {0, 2560}};
 const int64_t *const est_ptrs[4] = {&est_i[0][0], &est_i[0][1], &est_i[1][0], &est_i[1][1]};
 const halide_filter_argument_t kArgs[2] = {
@@ -234,10 +173,6 @@ const halide_filter_argument_t kArgs[2] = {
     {"output", halide_argument_kind_output_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
 }  // namespace
-
-extern "C" void halide_b200_stencil_chain_variant(int v) {
-    g_variant = v;
-}
 
 extern "C" int stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
     int r;
@@ -256,7 +191,7 @@ extern "C" int stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
     if ((r = hb::acquire(args, 2))) return r;
 
     // ping-pong buffers for the intermediate stages on their grown regions
-    const int groups = (kStages + kFuse - 1) / kFuse;
+    const int groups = kStages / kFuse;
     const int maxR = 2 * (kStages - kFuse);
     hb::Scratch scratch;
     const int64_t bw = (W + 2 * maxR + 1) & ~(int64_t)1, bh = H + 2 * maxR;  // (even pitch: intermediate rows keep pixel pairs word-aligned)
@@ -269,13 +204,10 @@ extern "C" int stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
     cudaStream_t s = hb::stream();
     {
         hb::CallTimer timer(s);
-        int done = 0;
         for (int g = 0; g < groups; g++) {
-            const int fuse = (kStages - done) < kFuse ? (kStages - done) : kFuse;
-            const int Rin = 2 * (kStages - done);           // apron of the region this launch reads
-            const int Rout = Rin - 2 * fuse;                // apron of the region it writes
+            const int Rin = 2 * (kStages - g * kFuse);      // apron of the region this launch reads
+            const int Rout = Rin - 2 * kFuse;               // apron of the region it writes
             Plane p;
-            p.fuse = fuse;
             p.dst_w = W + 2 * Rout;
             p.dst_h = H + 2 * Rout;
             p.src_w = W + 2 * Rin;
@@ -305,13 +237,7 @@ extern "C" int stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
             p.src_words = ((reinterpret_cast<uintptr_t>(p.src) & 3) == 0 && (p.src_sy & 1) == 0) ? 1 : 0;
             p.dst_words = ((reinterpret_cast<uintptr_t>(p.dst) & 3) == 0 && (p.dst_sy & 1) == 0) ? 1 : 0;
             dim3 grid((p.dst_w + kTile - 1) / kTile, (p.dst_h + kTile - 1) / kTile);
-            const bool window = fuse == kFuse && (g_variant == 2 || (g_variant == 0 && kDefaultWindow));
-            if (window) {
-                HB_LAUNCH("stencil_chain_window", stencil_chain_window_kernel<kFuse>, grid, 256, 0, s, p);
-            } else {
-                HB_LAUNCH("stencil_chain_fused", stencil_chain_fused_kernel, grid, 256, 0, s, p);
-            }
-            done += fuse;
+            HB_LAUNCH("stencil_chain_window", stencil_chain_window_kernel<kFuse>, grid, 256, 0, s, p);
         }
     }
     return hb::finish(args, 2, "stencil_chain launch");

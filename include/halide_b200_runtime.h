@@ -295,18 +295,14 @@ void halide_b200_ll_shard_coarse_level(int level);
 int halide_b200_ll_shard_plan_level(int32_t frame_w, int32_t frame_h, int32_t nranks);
 /* Test hook: bitmask routing levels==8 calls through the generic kernels (1 down, 2 up, 4 final,
  * 8 no fused coarse launch, 16 general-layout final kernel, 64 no TMA frame tile in the final
- * kernel, 256 = the 48-row-tile variant of the TMA final kernel, 128 = its default 32-row tiles) so
- * every code path stays covered by the parity tests. */
+ * kernel) so every code path stays covered by the parity tests. */
 void halide_b200_ll_force_generic(int mask);
 /* halide_blur test hook: 1 = route 4-byte-aligned frames through the general (any alignment) kernel as well;
  * >= 8 = aligned kernel with strips of that many rows (0 restores the defaults). */
 void halide_b200_blur_force_general(int enable);
-/* nl_means test / A-B hook: 0 = default kernel, 1 = generic kernel, 2 = register-window kernel (patch 3 or 7, search 7). */
+/* nl_means test hook: 1 = generic kernel for every patch / search size, so it can be checked on the sizes the
+ * register-window kernel takes by default (patch 3 or 7, search 7); any other value restores the default. */
 void halide_b200_nl_means_variant(int variant);
-/* stencil_chain test / A-B hook: 0 = default kernel, 1 = one-pixel-per-thread tile kernel, 2 = register-window tile kernel. */
-void halide_b200_stencil_chain_variant(int variant);
-/* conv_layer: 1 = wgmma/TMA implicit GEMM (3xTF32 split), 0 = FP32 SIMT kernel (also HALIDE_B200_CONV=tc|simt). */
-void halide_b200_conv_use_tensor_cores(int enable);
 /* Device self-test of the fast kernels' arithmetic shortcuts; returns mismatches vs div.rn / cvt, or -1. */
 long long halide_b200_selftest_arith(unsigned long long n, unsigned long long seed);
 

@@ -23,7 +23,8 @@ def run(hb, inp, filt, bias):
     return out
 
 
-@pytest.mark.parametrize("seed,scale", [(0, 1.0), (1, 2147483648.0)])  # the harness fills with raw rand() up to 2^31
+# the harness fills with raw rand() up to 2^31
+@pytest.mark.parametrize("seed,scale", [(0, 1.0), (1, 2147483648.0), (3, 1.0), (4, 2147483648.0)])
 def test_matches_oracle(hb, oracle, seed, scale):
     inp, filt, bias = make(seed, scale)
     got = run(hb, inp, filt, bias)
@@ -52,19 +53,3 @@ def test_wrong_shape_is_a_constraint_violation(hb):
     with pytest.raises(HalideError) as e:
         filters.conv_layer(bi, bf, bb, bo)
     assert e.value.code == -8
-
-
-@pytest.mark.parametrize("seed,scale", [(3, 1.0), (4, 2147483648.0)])
-def test_simt_path_matches_oracle(hb, oracle, seed, scale):
-    """The default path is the wgmma implicit GEMM (TMA + mbarrier ring, 3xTF32 split); the FP32 SIMT kernel it replaced stays
-    selectable (HALIDE_B200_CONV=simt) and must meet the same 1e-4 bar."""
-    l = hb.load_library()
-    inp, filt, bias = make(seed, scale)
-    want = oracle.conv_layer(inp, filt, bias)
-    try:
-        l.halide_b200_conv_use_tensor_cores(0)
-        got = run(hb, inp, filt, bias)
-    finally:
-        l.halide_b200_conv_use_tensor_cores(1)
-    err = np.abs(got - want) / np.maximum(np.abs(want), 1e-30)
-    assert np.isfinite(got).all() and err.max() <= 1e-4, err.max()

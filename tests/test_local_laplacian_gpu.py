@@ -141,7 +141,7 @@ def test_generic_kernels_agree_with_fast_path(hb, oracle):
     got_fast = run_local_laplacian(hb, img, 8, 1.0 / 7.0, 1.0)
     assert np.array_equal(got_generic, want) and np.array_equal(got_fast, want)
     # 64: no TMA frame tile in the final kernel
-    for mask in (1, 2, 4, 8, 1 | 8, 2 | 4, 64, 16 | 64, 128, 256):
+    for mask in (1, 2, 4, 8, 1 | 8, 2 | 4, 64, 16 | 64):
         try:
             l.halide_b200_ll_force_generic(mask)
             got = run_local_laplacian(hb, img, 8, 1.0 / 7.0, 1.0)
@@ -189,17 +189,13 @@ def test_final_kernel_simple_and_general_layout_paths(hb, oracle, shape):
     assert np.array_equal(got_crop, want_crop)
 
 
-@pytest.mark.parametrize("mask", [128, 256])
-def test_final_kernel_tile_heights(hb, oracle, mask):
-    """The TMA final kernel exists with 32-row and 48-row tiles (big frames take 48 by default; hook bits 128 / 256 pin
-    either on any frame).  Frames whose rows are 16-byte multiples (TMA-eligible), heights that are no multiple of
-    either tile, beta == 1 and beta != 1, and a crop starting 8 columns / 5 rows inside the input."""
-    l = hb.load_library()
-    try:
-        l.halide_b200_ll_force_generic(mask)
-        for (h, w), beta in (((150, 256), 1.0), ((101, 136), 0.7), ((49, 64), 1.0)):
-            _check(hb, oracle, u16_frame((3, h, w), mask + h), 8, 1.0 / 7.0, beta)
-        img = u16_frame((3, 140, 264), 5)
-        _check(hb, oracle, img, 8, 1.0 / 7.0, 1.0, out_shape=(3, 120, 240), in_mins=(0, 0, 0), out_mins=(8, 5, 0))
-    finally:
-        l.halide_b200_ll_force_generic(0)
+@pytest.mark.parametrize("h,w,beta,crop", [(150, 256, 1.0, False), (101, 136, 0.7, False), (49, 64, 1.0, False),
+                                          (140, 264, 1.0, True)])
+def test_tma_final_kernel(hb, oracle, h, w, beta, crop):
+    """Frames whose rows are 16-byte multiples take the final kernel's TMA frame tile: heights that are no multiple of
+    its 32-row tiles, beta == 1 and beta != 1, and a crop starting 8 columns / 5 rows inside the input."""
+    img = u16_frame((3, h, w), h)
+    if crop:
+        _check(hb, oracle, img, 8, 1.0 / 7.0, beta, out_shape=(3, h - 20, w - 24), in_mins=(0, 0, 0), out_mins=(8, 5, 0))
+    else:
+        _check(hb, oracle, img, 8, 1.0 / 7.0, beta)

@@ -60,21 +60,15 @@ def test_harness_size_regions_vs_oracle(hb, oracle):
         assert np.array_equal(got[y0:y0 + n, x0:x0 + n], want[y0 - ya:y0 - ya + n, x0 - xa:x0 - xa + n])
 
 
-@pytest.mark.parametrize("variant", [1, 2])
-def test_both_tile_kernels_match_oracle(hb, oracle, variant):
-    """The one-pixel-per-thread tile kernel and the register-window tile kernel (hook: halide_b200_stencil_chain_variant)
-    on ragged sizes, odd widths (odd row strides: the 16-bit load / store paths), an output larger than the input and a
+@pytest.mark.parametrize("seed", [100, 200])
+def test_tile_kernel_edge_cases_match_oracle(hb, oracle, seed):
+    """Ragged sizes, odd widths (odd row strides: the 16-bit load / store paths), an output larger than the input and a
     crop with odd offsets."""
-    l = hb.load_library()
-    try:
-        l.halide_b200_stencil_chain_variant(variant)
-        for h, w in ((1, 1), (17, 40), (65, 129), (200, 333), (130, 256)):
-            inp = u16_frame((h, w), variant * 100 + h + w)
-            assert np.array_equal(run(hb, inp), oracle.stencil_chain(inp)), (variant, h, w)
-        inp = u16_frame((40, 50), 3)
-        got = run(hb, inp, out_shape=(60, 80), in_mins=(3, -2), out_mins=(-10, -9))
-        assert np.array_equal(got, oracle.stencil_chain(inp, out_shape=(60, 80), in_mins=(3, -2), out_mins=(-10, -9)))
-        got = run(hb, inp, out_shape=(21, 33), in_mins=(0, 0), out_mins=(7, 5))
-        assert np.array_equal(got, oracle.stencil_chain(inp, out_shape=(21, 33), in_mins=(0, 0), out_mins=(7, 5)))
-    finally:
-        l.halide_b200_stencil_chain_variant(0)
+    for h, w in ((1, 1), (17, 40), (65, 129), (200, 333), (130, 256)):
+        inp = u16_frame((h, w), seed + h + w)
+        assert np.array_equal(run(hb, inp), oracle.stencil_chain(inp)), (seed, h, w)
+    inp = u16_frame((40, 50), 3)
+    got = run(hb, inp, out_shape=(60, 80), in_mins=(3, -2), out_mins=(-10, -9))
+    assert np.array_equal(got, oracle.stencil_chain(inp, out_shape=(60, 80), in_mins=(3, -2), out_mins=(-10, -9)))
+    got = run(hb, inp, out_shape=(21, 33), in_mins=(0, 0), out_mins=(7, 5))
+    assert np.array_equal(got, oracle.stencil_chain(inp, out_shape=(21, 33), in_mins=(0, 0), out_mins=(7, 5)))

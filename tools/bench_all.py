@@ -63,11 +63,6 @@ def main():
     quick = "--quick" in sys.argv
     only = sys.argv[sys.argv.index("--only") + 1].split(",") if "--only" in sys.argv else None
     want = lambda name: only is None or name in only
-    if os.environ.get("BENCH_ALL_VARIANT"):   # A/B: route stencil_chain / nl_means through the chosen kernel variant (hooks)
-        import halide_b200
-        _l = halide_b200.load_library()
-        _l.halide_b200_stencil_chain_variant(int(os.environ["BENCH_ALL_VARIANT"]))
-        _l.halide_b200_nl_means_variant(int(os.environ["BENCH_ALL_VARIANT"]))
     dev = torch.device("cuda", 0)
     g = torch.Generator(device=dev)
     g.manual_seed(7)
