@@ -209,8 +209,8 @@ template<bool BETA1>
 void launch_level1(Plan &p, cudaStream_t s) {
     LevelBuf *lb = p.ls.lv;
     const LLFrame &f = p.f;
+    // one pair table and kDWarps warp stages: one block per SM
     const size_t smem = kPairLutN * sizeof(float2) + kDWarps * sizeof(DownStage);
-    // (the attribute and the occupancy are per device and cheap to query; no process-wide caching)
     const int slots = resident_slots(ll_level1_kernel<BETA1>, kDWarps * 32, smem);
     const int ns = (lb[1].sx.n() + kDCols - 1) / kDCols, nc = (lb[1].cy.n() + kDR - 1) / kDR;
     const long long units = (long long)ns * nc;
