@@ -16,6 +16,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <map>
 #include <mutex>
 #include <vector>
@@ -205,46 +206,71 @@ int resident_slots(Kern kern, int threads, size_t smem) {
     return g_slots[key] = sms * per_sm;
 }
 
+// Levels 1 and 2 from the frame (K == 8): stores level-1 rows cy1 and level-2 rows cy2, reading the frame through f
+// (the row-sharded path narrows both spans, and hides the halo rows from the launch that runs before they arrive).
 template<bool BETA1>
-void launch_level1(Plan &p, cudaStream_t s) {
-    LevelBuf *lb = p.ls.lv;
-    const LLFrame &f = p.f;
+void launch_level12_kernel(Plan &p, const LLFrame &f, Span cy1, Span cy2, cudaStream_t s) {
+    LevelBuf d1 = p.ls.lv[1], d2 = p.ls.lv[2];
+    d1.cy = cy1;
+    d2.cy = cy2;
     // one pair table and kDWarps warp stages: one block per SM
     const size_t smem = kPairLutN * sizeof(float2) + kDWarps * sizeof(DownStage);
     const int slots = resident_slots(ll_level1_kernel<BETA1>, kDWarps * 32, smem);
-    const int ns = (lb[1].sx.n() + kDCols - 1) / kDCols, nc = (lb[1].cy.n() + kDR - 1) / kDR;
-    const long long units = (long long)ns * nc;
-    // one block per resident slot, but never fewer than ~2 units per warp's worth of work per block
-    long long g = (units + 1) / 2;
-    if (g > slots) g = slots;
-    if (g < 1) g = 1;
+    // strips of 28 level-1 columns from xbase == xo (mod 4), far enough left that their level-2 columns (xbase/2 + 14k ..)
+    // reach level 2's first column; chunks of 8 level-1 rows from an odd ybase, over the rows stored and the taps of
+    // the level-2 rows stored
+    const int xbase = d1.xo - ((d1.xo - 2 * d2.sx.lo > 0 ? d1.xo - 2 * d2.sx.lo + 3 : 0) & ~3);
+    const int ns = std::max((d1.sx.hi - xbase) / kDCols + 1, (d2.sx.hi - xbase / 2) / (kDCols / 2) + 1);
+    int lo = INT32_MAX, hi = INT32_MIN;
+    if (cy1.n() > 0) lo = cy1.lo, hi = cy1.hi;
+    if (cy2.n() > 0) lo = std::min(lo, 2 * cy2.lo - 1), hi = std::max(hi, 2 * cy2.hi + 2);
+    if (lo > hi) return;
+    const int ybase = lo - ((lo & 1) ^ 1);
+    const int nc = (hi - ybase) / kDR + 1;
+    // nr chunk ranges per strip: the fewest step-equivalents per warp over the rounds of runs (a lead-in computes 2 of a
+    // chunk's 8 rows: a quarter chunk)
+    const long long nw = (long long)slots * kDWarps;
+    int nr = 1;
+    long long best = -1;
+    for (int r = 1; r <= nc; r++) {
+        const long long cost = ((long long)ns * r + nw - 1) / nw * (4ll * ((nc + r - 1) / r) + 1);
+        if (best < 0 || cost < best) best = cost, nr = r;
+    }
+    const long long runs = (long long)ns * nr;
+    const int g = (int)std::min<long long>(slots, (runs + kDWarps - 1) / kDWarps);
     // aligned 32-bit loads of a column pair / 32-bit element offsets from the buffer's first element
     const int wide = ((uintptr_t)f.in & 3) == 0 && (f.in_sy & 1) == 0 && (f.in_sc & 1) == 0 && (f.in_x0 & 1) == 0 &&
                      ((uintptr_t)f.halo_top & 3) == 0 && ((uintptr_t)f.halo_bot & 3) == 0 && (f.halo_pitch & 1) == 0;
     const int idx32 = f.in_sy > 0 && f.in_sc > 0 && (int64_t)f.in_h * f.in_sy + (int64_t)f.in_c * f.in_sc < (1ll << 31);
-    HB_LAUNCH("ll_level1", (ll_level1_kernel<BETA1>), (int)g, kDWarps * 32, smem, s, p.f, lb[1], ns, nc, wide, idx32);
-    lb[1].has_pair = 1;
+    HB_LAUNCH("ll_level1", (ll_level1_kernel<BETA1>), g, kDWarps * 32, smem, s, f, d1, d2, xbase, ybase, ns, nc, nr, wide, idx32);
 }
+
+void launch_level12(Plan &p, const LLFrame &f, Span cy1, Span cy2, cudaStream_t s) {
+    if (p.f.beta == 1.0f) launch_level12_kernel<true>(p, f, cy1, cy2, s);
+    else launch_level12_kernel<false>(p, f, cy1, cy2, s);
+    p.ls.lv[1].has_pair = 1;
+}
+
+// the fast level-1 kernel also produces level 2
+bool fast_down(const Plan &p) { return p.K == 8 && !(g_force_naive & 1); }
 
 void launch_down(Plan &p, int j, cudaStream_t s) {  // produce level j (j >= 1) rows cy
     LevelBuf *lb = p.ls.lv;
-    if (lb[j].cy.n() <= 0) return;
-    const bool fast = (p.K == 8) && !(g_force_naive & 1);
-    if (fast) {
-        const bool beta1 = p.f.beta == 1.0f;
+    if (fast_down(p)) {
         if (j == 1) {
-            if (beta1) launch_level1<true>(p, s);
-            else launch_level1<false>(p, s);
-        } else {
+            launch_level12(p, p.f, lb[1].cy, lb[2].cy, s);
+        } else if (j > 2 && lb[j].cy.n() > 0) {
             // stored levels: load-bound row-group kernel; no pair plane (the up-sweep of these small levels picks its two
             // planes out of the level itself)
-            const int ns = (lb[j].sx.n() + kDCols - 1) / kDCols, ng = (lb[j].cy.n() + kRG - 1) / kRG;
+            const int ns = (lb[j].sx.n() + kRCols - 1) / kRCols, ng = (lb[j].cy.n() + kRG - 1) / kRG;
             const long long tasks = (long long)ns * ng * 5;
             const int slots = resident_slots(ll_down_rows_kernel, 256, 0);
             long long g = (tasks + 7) / 8;
             if (g > slots) g = slots;
             HB_LAUNCH("ll_down_rows", ll_down_rows_kernel, (int)g, 256, 0, s, lb[j - 1], lb[j], ns, ng);
         }
+    } else if (lb[j].cy.n() <= 0) {
+        return;
     } else if (j == 1) {
         HB_LAUNCH("ll_level1_generic", ll_level1_naive_kernel, grid_for(lb[1].sx.n(), lb[1].cy.n()), kBlk, 0, s, p.f, lb[1]);
     } else {
@@ -333,9 +359,9 @@ bool launch_coarse_fused(Plan &p, int j0, cudaStream_t s) {
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int max_blocks = coop ? (slots > 2 * sms ? 2 * sms : slots) : 0;
     if (max_blocks <= 0) return false;
-    int J = p.J, K = p.K, levels = p.f.levels;
+    int J = p.J, K = p.K, levels = p.f.levels, jd = fast_down(p) && j0 < 2 ? 2 : j0;
     float flm1 = p.f.flm1;
-    void *args[] = {&p.ls, &J, &j0, &K, &flm1, &levels};
+    void *args[] = {&p.ls, &J, &j0, &jd, &K, &flm1, &levels};
     hb::count_launch("ll_coarse_fused", s);
     cudaError_t e = cudaLaunchCooperativeKernel((void *)ll_coarse_fused_kernel, dim3(max_blocks), dim3(256), args, 0, s);
     hb::after_launch(s);
@@ -351,7 +377,8 @@ bool launch_coarse_fused(Plan &p, int j0, cudaStream_t s) {
 void run_coarse_sweep(Plan &p, int from_level, cudaStream_t s) {
     int j0 = p.J - 1;
     if (!(g_force_naive & 8)) {
-        // (level 1 always has its own launch: it is built from the frame, not from a stored level)
+        // (level 1 always has its own launch: it is built from the frame, not from a stored level; on the fast path that
+        // launch also builds level 2, and the fused tail's down-sweep starts after it)
         const int j_min = from_level < 1 ? 1 : from_level;
         while (j0 > j_min && (int64_t)p.ls.lv[j0].sx.n() * p.ls.lv[j0].sy.n() <= 40 * 1024) j0--;
     }
@@ -593,32 +620,28 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
             }
         }
         LevelBuf *lb = p.ls.lv;
-        if (exchanged_async && p.K == 8 && !(g_force_naive & 1)) {
-            // level 1 in up to three launches: interior rows (taps 2y-1 .. 2y+2 all inside the band) now, edge rows after the halo
-            const Span cy = lb[1].cy;
-            int i_lo = (p.f.in_y0 + 2) >> 1;                    // smallest y with 2y-1 >= in_y0
-            int i_hi = (p.f.in_y0 + p.f.in_h - 3) >> 1;          // largest y with 2y+2 <= in_y0 + in_h - 1
-            if (i_lo < cy.lo) i_lo = cy.lo;
-            if (i_hi > cy.hi) i_hi = cy.hi;
-            if (i_lo <= i_hi) {
-                lb[1].cy = {i_lo, i_hi};
-                launch_down(p, 1, s);
-            }
-            cudaStreamWaitEvent(s, ev_halo, 0);
+        if (exchanged_async && fast_down(p)) {
+            // levels 1 and 2 in up to three launches: the interior rows (every source row inside the band) now, with the
+            // halo rows hidden from the kernel, and the rows at each edge after the halo
+            const Span cy = lb[1].cy, cy2 = lb[2].cy;
+            const int i_lo = std::max(cy.lo, (p.f.in_y0 + 2) >> 1);                // smallest y with 2y-1 >= in_y0
+            const int i_hi = std::min(cy.hi, (p.f.in_y0 + p.f.in_h - 3) >> 1);      // largest y with 2y+2 <= in_y0 + in_h - 1
             if (i_lo > i_hi) {  // (band too thin to have interior rows)
-                lb[1].cy = cy;
+                cudaStreamWaitEvent(s, ev_halo, 0);
                 launch_down(p, 1, s);
             } else {
-                if (cy.lo < i_lo) {
-                    lb[1].cy = {cy.lo, i_lo - 1};
-                    launch_down(p, 1, s);
-                }
-                if (i_hi < cy.hi) {
-                    lb[1].cy = {i_hi + 1, cy.hi};
-                    launch_down(p, 1, s);
-                }
+                // level-2 rows whose taps 2y-1 .. 2y+2 are all interior level-1 rows
+                const Span c2 = {std::max(cy2.lo, (i_lo + 2) >> 1), std::min(cy2.hi, (i_hi - 2) >> 1)};
+                const Span top2 = {cy2.lo, std::min(cy2.hi, c2.lo - 1)};
+                const Span bot2 = {std::max(c2.hi, top2.hi) + 1, cy2.hi};
+                LLFrame fi = p.f;
+                fi.halo_top = fi.halo_bot = nullptr;
+                fi.halo_top_rows = fi.halo_bot_rows = 0;
+                launch_level12(p, fi, {i_lo, i_hi}, c2, s);
+                cudaStreamWaitEvent(s, ev_halo, 0);
+                if (cy.lo < i_lo || top2.n() > 0) launch_level12(p, p.f, {cy.lo, i_lo - 1}, top2, s);
+                if (i_hi < cy.hi || bot2.n() > 0) launch_level12(p, p.f, {i_hi + 1, cy.hi}, bot2, s);
             }
-            lb[1].cy = cy;
         } else {
             if (exchanged_async) cudaStreamWaitEvent(s, ev_halo, 0);
             launch_down(p, 1, s);
