@@ -15,6 +15,8 @@ struct Msg {
 bool active();
 int rank();
 int size();
+// Changes whenever the calling thread joins a communicator: state kept per geometry is only valid within one.
+int epoch();
 // One ncclGroup of point-to-point messages enqueued on stream `s` (ordered with the kernels on it).
 int exchange(const Msg *msgs, int n, cudaStream_t s);
 

@@ -458,11 +458,11 @@ int choose_coarse_level(const ll::Geom &whole, int nranks, int J, int K) {
 // needs beyond itself is recomputed from them) and ONE all-to-all gather of the coarse level jr; both are NCCL
 // point-to-point groups on the compute stream.  Everything else is the single-GPU kernels on this rank's rows.
 struct ShardPlan {  // per geometry: every rank's band (gathered once), reused call after call
-    int key[10];
+    int key[11];
     bool valid = false;
     std::vector<int> bands;  // [lo, hi] per rank
 };
-ShardPlan g_shard;
+thread_local ShardPlan g_shard;  // (per thread: the ranks of an in-process loopback group are threads of one process)
 
 int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha, float beta, halide_buffer_t *output,
                                 int frame_y_min, int frame_y_extent) {
@@ -499,10 +499,12 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
     const ll::Geom whole = ll::make_geom(outx, frame_y, inx, frame_y, p.J);
     const int jr = choose_coarse_level(whole, nranks, p.J, p.K);
 
-    // every rank's band: gathered once per geometry (collective on first use / change)
-    const int key[10] = {W, band.lo, band.hi, frame_y.lo, frame_y.hi, rank, nranks, C, jr, levels};
+    // every rank's band: gathered once per geometry (collective on first use / change) and per communicator (a rank
+    // that kept its plan from an earlier group would skip the gather its new peers enter)
+    const int key[11] = {W, band.lo, band.hi, frame_y.lo, frame_y.hi, rank, nranks, C, jr, levels, hbdist::epoch()};
     if (!g_shard.valid || memcmp(g_shard.key, key, sizeof(key)) != 0) {
         int mine[2] = {band.lo, band.hi};
+        g_shard.valid = false;  // (until the gather succeeds)
         g_shard.bands.assign(2 * (size_t)nranks, 0);
         if ((r = hbdist::allgather_bytes(mine, g_shard.bands.data(), sizeof(mine)))) return r;
         for (int q = 0; q + 1 < nranks; q++) {
@@ -519,15 +521,29 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
     auto rows_of = [&](int q, ll::ShardLevel *sl, Span *need) {
         ll::compute_shard_rows(whole, frame_y, band_of(q), q == 0, q == nranks - 1, jr, sl, need);
     };
+    // Bands too thin to shard: checked for every rank, not only this one, so that all ranks refuse the same frame
+    // (a rank refusing alone would leave its neighbours waiting in the exchange).  need[q]: input rows rank q reads.
+    std::vector<Span> need(nranks);
+    for (int q = 0; q < nranks; q++) {
+        ll::ShardLevel t[ll::kMaxJ];
+        rows_of(q, t, &need[q]);
+        for (int j = 1; j <= jr && j < p.J; j++) {
+            if (t[j].own.n() < 1) {
+                return hb::fail(halide_error_code_constraint_violated,
+                                "local_laplacian_sharded: rank %d's band of %d rows is too small for %d ranks (level %d owns no row)", q,
+                                band_of(q).n(), nranks, j);
+            }
+        }
+        const int above = band_of(q).lo - need[q].lo, below = need[q].hi - band_of(q).hi;
+        if (above > (q == 0 ? 0 : band_of(q - 1).n()) || below > (q == nranks - 1 ? 0 : band_of(q + 1).n())) {
+            return hb::fail(halide_error_code_constraint_violated,
+                            "local_laplacian_sharded: rank %d's input halo (%d rows above, %d below) is larger than the bands next to it", q,
+                            above, below);
+        }
+    }
     ll::ShardLevel sl[ll::kMaxJ];
     Span in_need;
     rows_of(rank, sl, &in_need);
-    for (int j = 1; j <= jr && j < p.J; j++) {
-        if (sl[j].own.n() < 1) {
-            return hb::fail(halide_error_code_constraint_violated,
-                            "local_laplacian_sharded: band of %d rows is too small for %d ranks (level %d owns no row)", band.n(), nranks, j);
-        }
-    }
     p.geom = ll::make_shard_geom(whole, sl, jr);
     p.f.clamp_y0 = frame_y.lo;
     p.f.clamp_h = frame_y.n();
@@ -538,23 +554,9 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
     const int ht = band.lo - in_need.lo, hbn = in_need.hi - band.hi;
     const size_t rowb = (size_t)p.f.in_w * sizeof(uint16_t);
     uint16_t *halo_top = nullptr, *halo_bot = nullptr, *send_up = nullptr, *send_dn = nullptr;
-    int up_need = 0, dn_need = 0;  // rows the rank below needs from my bottom / the rank above needs from my top
-    if (!first) {
-        ll::ShardLevel t[ll::kMaxJ];
-        Span n;
-        rows_of(rank - 1, t, &n);
-        up_need = n.hi - band_of(rank - 1).hi;  // its bottom halo = my first rows
-    }
-    if (!last) {
-        ll::ShardLevel t[ll::kMaxJ];
-        Span n;
-        rows_of(rank + 1, t, &n);
-        dn_need = band_of(rank + 1).lo - n.lo;  // its top halo = my last rows
-    }
-    if (ht > (first ? 0 : band_of(rank - 1).n()) || hbn > (last ? 0 : band_of(rank + 1).n()) || up_need > band.n() || dn_need > band.n()) {
-        return hb::fail(halide_error_code_constraint_violated,
-                        "local_laplacian_sharded: bands of %d rows are smaller than the input halo (%d above, %d below)", band.n(), ht, hbn);
-    }
+    // rows the rank above needs from my top (its bottom halo) / the rank below needs from my bottom (its top halo)
+    const int up_need = first ? 0 : need[rank - 1].hi - band_of(rank - 1).hi;
+    const int dn_need = last ? 0 : band_of(rank + 1).lo - need[rank + 1].lo;
     if (ht) halo_top = scratch.get<uint16_t>((size_t)C * ht * p.f.in_w);
     if (hbn) halo_bot = scratch.get<uint16_t>((size_t)C * hbn * p.f.in_w);
     if (up_need) send_up = scratch.get<uint16_t>((size_t)C * up_need * p.f.in_w);

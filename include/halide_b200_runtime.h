@@ -270,6 +270,11 @@ int halide_b200_profile_report(char *out, int out_size);
  * joins.  Ranks are ordered top to bottom over the frame's rows. */
 int halide_b200_dist_unique_id(char *out128);
 int halide_b200_dist_init(int rank, int nranks, const char *id128);
+/* In-process loopback group: each of nranks host threads of one process calls this with its rank and from then on
+ * is that rank (a thread-local binding, checked before the NCCL communicator); messages are device-to-device copies
+ * on the one device.  Every host wait is bounded (about 20 s; then the call returns halide_error_code_generic_error).
+ * halide_b200_dist_shutdown on the thread ends its membership. */
+int halide_b200_dist_init_loopback(int rank, int nranks);
 int halide_b200_dist_shutdown(void);
 int halide_b200_dist_rank(void);
 int halide_b200_dist_size(void);
