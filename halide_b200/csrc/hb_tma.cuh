@@ -47,6 +47,11 @@ __device__ __forceinline__ void load_3d(void *dst, const CUtensorMap *map, uint6
                  "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
                  : "memory");
 }
+__device__ __forceinline__ void load_4d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2, int c3) {
+    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(dst)),
+                 "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+                 : "memory");
+}
 
 // ---- host side ---------------------------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,

@@ -42,19 +42,33 @@ const halide_filter_argument_t kArgs[5] = {
     {"beta", halide_argument_kind_input_scalar, 0, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, &sv_beta, nullptr},
     {"output", halide_argument_kind_output_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
+// halide_b200_local_laplacian_batch: the same buffers with a fourth dimension, the frame index n.
+const halide_filter_argument_t kBatchArgs[2] = {
+    {"input", halide_argument_kind_input_buffer, 4, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+    {"output", halide_argument_kind_output_buffer, 4, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+};
 
-// Everything one call needs on the device: frame description + per-level buffers.
+// Everything one call needs on the device: frame description + per-level buffers, for N frames of one geometry.
 struct Plan {
     LLFrame f;
     LevelSet ls;
     ll::Geom geom;
     int J, K;
+    int N;  // frames (1 but for a batch)
+    FrameStrides fs;  // all zero when N == 1
     float alpha;
     float *lut;
 };
 
-// The checks local_laplacian and its sharded variant share, on args = {input, output}.  *done: return r now (an error,
-// a bounds query or an empty output).
+// Grids index frames by blockIdx.z; batches beyond its limit launch in groups of frames [n0, n0 + count).
+constexpr int kMaxGridZ = 65535;
+template<typename F>
+void for_frame_groups(const Plan &p, F launch) {
+    for (int n0 = 0; n0 < p.N; n0 += kMaxGridZ) launch(n0, std::min(kMaxGridZ, p.N - n0));
+}
+
+// The checks local_laplacian and its sharded and batch variants share, on args = {input, output}.  *done: return r now
+// (an error, a bounds query or an empty output).
 int check_and_query(hb::Arg *args, int levels, bool *done) {
     int r;
     *done = true;
@@ -70,7 +84,9 @@ int check_and_query(hb::Arg *args, int levels, bool *done) {
         return hb::fail(levels < 2 ? halide_error_code_param_too_small : halide_error_code_param_too_large,
                         "Parameter levels is %d but must be in [2, 32]", levels);
     }
-    if (output->dim[0].extent <= 0 || output->dim[1].extent <= 0 || output->dim[2].extent <= 0) return 0;
+    for (int d = 0; d < output->dimensions; d++) {
+        if (output->dim[d].extent <= 0) return 0;
+    }
     *done = false;
     return 0;
 }
@@ -90,6 +106,18 @@ void fill_frame(Plan &p, const hb::Arg *args, int levels, float alpha, float bet
     f.out_x0 = output->dim[0].min; f.out_y0 = output->dim[1].min; f.out_c0 = output->dim[2].min;
     f.W = output->dim[0].extent; f.H = output->dim[1].extent; f.C = output->dim[2].extent;
     f.row0 = f.out_y0; f.nrows = f.H;
+    p.fs = FrameStrides{};
+    p.N = 1;
+    if (output->dimensions == 4) {
+        // output frame n reads input frame n: the output's first frame is (out n min - in n min) input frames past the
+        // input's mins
+        f.in += (int64_t)(output->dim[3].min - input->dim[3].min) * input->dim[3].stride;
+        p.N = output->dim[3].extent;
+        if (p.N > 1) {  // (one frame keeps stride 0: the same layout checks, hence kernels, as the 3-D call)
+            p.fs.in = input->dim[3].stride;
+            p.fs.out = output->dim[3].stride;
+        }
+    }
     f.levels = levels;
     f.beta = beta;
     f.flm1 = (float)(levels - 1);
@@ -157,11 +185,16 @@ int alloc_levels(Plan &p, hb::Scratch &scratch) {
         b.xo = lv.xo; b.nq = nq;
         b.gpitch = lv.gpitch; b.opitch = lv.opitch;
         b.has_pair = 0;
-        size_t gpix = (size_t)lv.sy.n() * lv.gpitch;
-        b.gp = scratch.get<float>(gpix * nq * 2);
-        b.ing = scratch.get<float>(gpix);
-        b.pair = p.K == 8 ? scratch.get<float>(gpix * 2) : b.ing;
-        b.outg = scratch.get<float>((size_t)lv.oy.n() * lv.opitch);
+        // one allocation per array for all N frames; a frame's slice starts on 256 bytes, like an allocation of its own
+        auto slice = [](size_t floats) { return (int64_t)((floats + 63) & ~size_t(63)); };
+        const size_t gpix = (size_t)lv.sy.n() * lv.gpitch;
+        const int64_t gp_sn = slice(gpix * nq * 2), ing_sn = slice(gpix), pair_sn = p.K == 8 ? slice(gpix * 2) : ing_sn;
+        const int64_t outg_sn = slice((size_t)lv.oy.n() * lv.opitch);
+        b.gp = scratch.get<float>((size_t)gp_sn * p.N);
+        b.ing = scratch.get<float>((size_t)ing_sn * p.N);
+        b.pair = p.K == 8 ? scratch.get<float>((size_t)pair_sn * p.N) : b.ing;
+        b.outg = scratch.get<float>((size_t)outg_sn * p.N);
+        if (p.N > 1) p.fs.gp[j] = gp_sn, p.fs.ing[j] = ing_sn, p.fs.pair[j] = pair_sn, p.fs.outg[j] = outg_sn;
         if (!b.gp || !b.ing || !b.pair || !b.outg) {
             return hb::fail(halide_error_code_device_malloc_failed, "local_laplacian: scratch allocation failed");
         }
@@ -208,14 +241,14 @@ int resident_slots(Kern kern, int threads, size_t smem) {
 
 // Levels 1 and 2 from the frame (K == 8): stores level-1 rows cy1 and level-2 rows cy2, reading the frame through f
 // (the row-sharded path narrows both spans, and hides the halo rows from the launch that runs before they arrive).
-template<bool BETA1>
+template<bool BETA1, bool FRAMES>
 void launch_level12_kernel(Plan &p, const LLFrame &f, Span cy1, Span cy2, cudaStream_t s) {
     LevelBuf d1 = p.ls.lv[1], d2 = p.ls.lv[2];
     d1.cy = cy1;
     d2.cy = cy2;
     // one pair table and kDWarps warp stages: one block per SM
     const size_t smem = kPairLutN * sizeof(float2) + kDWarps * sizeof(DownStage);
-    const int slots = resident_slots(ll_level1_kernel<BETA1>, kDWarps * 32, smem);
+    const int slots = resident_slots(ll_level1_kernel<BETA1, FRAMES>, kDWarps * 32, smem);
     // strips of 28 level-1 columns from xbase == xo (mod 4), far enough left that their level-2 columns (xbase/2 + 14k ..)
     // reach level 2's first column; chunks of 8 level-1 rows from an odd ybase, over the rows stored and the taps of
     // the level-2 rows stored
@@ -228,26 +261,31 @@ void launch_level12_kernel(Plan &p, const LLFrame &f, Span cy1, Span cy2, cudaSt
     const int ybase = lo - ((lo & 1) ^ 1);
     const int nc = (hi - ybase) / kDR + 1;
     // nr chunk ranges per strip: the fewest step-equivalents per warp over the rounds of runs (a lead-in computes 2 of a
-    // chunk's 8 rows: a quarter chunk)
-    const long long nw = (long long)slots * kDWarps;
+    // chunk's 8 rows: a quarter chunk), over the N * ns strips of the batch
+    const long long nw = (long long)slots * kDWarps, strips = (long long)p.N * ns;
     int nr = 1;
     long long best = -1;
     for (int r = 1; r <= nc; r++) {
-        const long long cost = ((long long)ns * r + nw - 1) / nw * (4ll * ((nc + r - 1) / r) + 1);
+        const long long cost = (strips * r + nw - 1) / nw * (4ll * ((nc + r - 1) / r) + 1);
         if (best < 0 || cost < best) best = cost, nr = r;
     }
-    const long long runs = (long long)ns * nr;
+    const long long runs = strips * nr;
     const int g = (int)std::min<long long>(slots, (runs + kDWarps - 1) / kDWarps);
-    // aligned 32-bit loads of a column pair / 32-bit element offsets from the buffer's first element
-    const int wide = ((uintptr_t)f.in & 3) == 0 && (f.in_sy & 1) == 0 && (f.in_sc & 1) == 0 && (f.in_x0 & 1) == 0 &&
-                     ((uintptr_t)f.halo_top & 3) == 0 && ((uintptr_t)f.halo_bot & 3) == 0 && (f.halo_pitch & 1) == 0;
+    // aligned 32-bit loads of a column pair / 32-bit element offsets from the frame's first element
+    const int wide = ((uintptr_t)f.in & 3) == 0 && (f.in_sy & 1) == 0 && (f.in_sc & 1) == 0 && (p.fs.in & 1) == 0 &&
+                     (f.in_x0 & 1) == 0 && ((uintptr_t)f.halo_top & 3) == 0 && ((uintptr_t)f.halo_bot & 3) == 0 &&
+                     (f.halo_pitch & 1) == 0;
     const int idx32 = f.in_sy > 0 && f.in_sc > 0 && (int64_t)f.in_h * f.in_sy + (int64_t)f.in_c * f.in_sc < (1ll << 31);
-    HB_LAUNCH("ll_level1", (ll_level1_kernel<BETA1>), g, kDWarps * 32, smem, s, f, d1, d2, xbase, ybase, ns, nc, nr, wide, idx32);
+    HB_LAUNCH("ll_level1", (ll_level1_kernel<BETA1, FRAMES>), g, kDWarps * 32, smem, s, f, d1, d2, xbase, ybase, ns, nc, nr, wide, idx32,
+              p.N, p.fs);
 }
 
 void launch_level12(Plan &p, const LLFrame &f, Span cy1, Span cy2, cudaStream_t s) {
-    if (p.f.beta == 1.0f) launch_level12_kernel<true>(p, f, cy1, cy2, s);
-    else launch_level12_kernel<false>(p, f, cy1, cy2, s);
+    const bool beta1 = p.f.beta == 1.0f, frames = p.N > 1;
+    if (beta1 && frames) launch_level12_kernel<true, true>(p, f, cy1, cy2, s);
+    else if (beta1) launch_level12_kernel<true, false>(p, f, cy1, cy2, s);
+    else if (frames) launch_level12_kernel<false, true>(p, f, cy1, cy2, s);
+    else launch_level12_kernel<false, false>(p, f, cy1, cy2, s);
     p.ls.lv[1].has_pair = 1;
 }
 
@@ -263,37 +301,53 @@ void launch_down(Plan &p, int j, cudaStream_t s) {  // produce level j (j >= 1) 
             // stored levels: load-bound row-group kernel; no pair plane (the up-sweep of these small levels picks its two
             // planes out of the level itself)
             const int ns = (lb[j].sx.n() + kRCols - 1) / kRCols, ng = (lb[j].cy.n() + kRG - 1) / kRG;
-            const long long tasks = (long long)ns * ng * 5;
-            const int slots = resident_slots(ll_down_rows_kernel, 256, 0);
+            const long long tasks = (long long)ns * ng * 5 * p.N;
+            auto kern = p.N > 1 ? ll_down_rows_kernel<true> : ll_down_rows_kernel<false>;
+            const int slots = resident_slots(kern, 256, 0);
             long long g = (tasks + 7) / 8;
             if (g > slots) g = slots;
-            HB_LAUNCH("ll_down_rows", ll_down_rows_kernel, (int)g, 256, 0, s, lb[j - 1], lb[j], ns, ng);
+            HB_LAUNCH("ll_down_rows", kern, (int)g, 256, 0, s, lb[j - 1], lb[j], ns, ng, p.N, j, p.fs);
         }
     } else if (lb[j].cy.n() <= 0) {
         return;
     } else if (j == 1) {
-        HB_LAUNCH("ll_level1_generic", ll_level1_naive_kernel, grid_for(lb[1].sx.n(), lb[1].cy.n()), kBlk, 0, s, p.f, lb[1]);
+        for_frame_groups(p, [&](int n0, int nf) {
+            dim3 g = grid_for(lb[1].sx.n(), lb[1].cy.n());
+            g.z = nf;
+            HB_LAUNCH("ll_level1_generic", ll_level1_naive_kernel, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), p.fs);
+        });
     } else {
-        HB_LAUNCH("ll_down", ll_down_naive_kernel, grid_for(lb[j].sx.n(), lb[j].cy.n()), kBlk, 0, s, lb[j - 1], lb[j], p.K);
+        for_frame_groups(p, [&](int n0, int nf) {
+            dim3 g = grid_for(lb[j].sx.n(), lb[j].cy.n());
+            g.z = nf;
+            HB_LAUNCH("ll_down", ll_down_naive_kernel, g, kBlk, 0, s, at_frame(lb[j - 1], j - 1, p.fs, n0), at_frame(lb[j], j, p.fs, n0), p.K, j,
+                      p.fs);
+        });
     }
 }
 
-dim3 up_grid(int x_lo, int x_hi, int y_lo, int y_hi) {  // tiles on even absolute origins
-    return dim3((x_hi - (x_lo & ~1) + kUpTW) / kUpTW, (y_hi - (y_lo & ~1) + kUpTH) / kUpTH);
+dim3 up_grid(int x_lo, int x_hi, int y_lo, int y_hi, int nf) {  // tiles on even absolute origins; z = frames
+    return dim3((x_hi - (x_lo & ~1) + kUpTW) / kUpTW, (y_hi - (y_lo & ~1) + kUpTH) / kUpTH, nf);
 }
 
 void launch_up(Plan &p, int j, cudaStream_t s) {  // produce outGPyramid[j] (1 <= j <= J-1) rows coy
     LevelBuf *lb = p.ls.lv;
     if (lb[j].coy.n() <= 0) return;
     const bool fast_up = (p.K == 8) && !(g_force_naive & 2);
-    if (fast_up && j < p.J - 1) {
-        static const CUtensorMap no_map = {};
-        HB_LAUNCH("ll_up2", (ll_up2_kernel<false, false, true>), up_grid(lb[j].ox.lo, lb[j].ox.hi, lb[j].coy.lo, lb[j].coy.hi), 256,
-                  up2_smem_bytes(false, false), s, p.f, lb[j], lb[j + 1], no_map);
-    } else {
-        HB_LAUNCH("ll_up", ll_up_naive_kernel, grid_for(lb[j].ox.n(), lb[j].coy.n()), kBlk, 0, s, lb[j],
-                  lb[j == p.J - 1 ? j : j + 1], p.f.flm1, p.f.levels, j == p.J - 1 ? 1 : 0);
-    }
+    for_frame_groups(p, [&](int n0, int nf) {
+        if (fast_up && j < p.J - 1) {
+            static const CUtensorMap no_map = {};
+            HB_LAUNCH("ll_up2", (nf > 1 ? ll_up2_kernel<false, false, true, false, true> : ll_up2_kernel<false, false, true, false, false>), up_grid(lb[j].ox.lo, lb[j].ox.hi, lb[j].coy.lo, lb[j].coy.hi, nf),
+                      256, up2_smem_bytes(false, false), s, at_frame(p.f, p.fs, n0), at_frame(lb[j], j, p.fs, n0),
+                      at_frame(lb[j + 1], j + 1, p.fs, n0), no_map, j, p.fs);
+        } else {
+            dim3 g = grid_for(lb[j].ox.n(), lb[j].coy.n());
+            g.z = nf;
+            const int jc = j == p.J - 1 ? j : j + 1;
+            HB_LAUNCH("ll_up", ll_up_naive_kernel, g, kBlk, 0, s, at_frame(lb[j], j, p.fs, n0), at_frame(lb[jc], jc, p.fs, n0),
+                      p.f.flm1, p.f.levels, j == p.J - 1 ? 1 : 0, j, p.fs);
+        }
+    });
 }
 
 void launch_final(Plan &p, cudaStream_t s) {
@@ -306,36 +360,53 @@ void launch_final(Plan &p, cudaStream_t s) {
         const bool aligned = f.C == 3 && f.in_c0 == 0 && f.out_c0 == 0 && f.in_c >= 3 && (f.W & 1) == 0 && (f.out_x0 & 1) == 0 &&
                              (f.in_x0 & 1) == 0 && ((uintptr_t)f.in & 3) == 0 && ((uintptr_t)f.out & 3) == 0 &&
                              (f.in_sy & 1) == 0 && (f.in_sc & 1) == 0 && (f.out_sy & 1) == 0 && (f.out_sc & 1) == 0 &&
-                             f.in_sy > 0 && f.in_sc > 0 && f.out_sy > 0 && f.out_sc > 0 && in_span < (1ll << 31) &&
-                             out_span < (1ll << 31) && !(g_force_naive & 16);
+                             (p.fs.in & 1) == 0 && (p.fs.out & 1) == 0 && f.in_sy > 0 && f.in_sc > 0 && f.out_sy > 0 &&
+                             f.out_sc > 0 && in_span < (1ll << 31) && out_span < (1ll << 31) && !(g_force_naive & 16);
         const bool beta1 = f.beta == 1.0f;
-        // frame tile by TMA when the buffer meets TMA's rules (16-byte aligned base and strides); the map describes the
-        // input buffer itself (x, y, c), so a tile reaching past it reads zeros for pixels that are never stored
-        CUtensorMap in_map = {};
-        bool use_tma = false;
-        if (aligned && !(g_force_naive & 64)) {
-            const int64_t strides[2] = {f.in_sy * 2, f.in_sc * 2};
-            // (every tile's first column must also start on a 16-byte boundary: crops at other even offsets take the load path)
-            if (tma::strides_ok(f.in, strides, 2) && (((f.out_x0 & ~1) - f.in_x0) & 7) == 0) {
-                const uint64_t dims[3] = {(uint64_t)f.in_w, (uint64_t)f.in_h, (uint64_t)f.in_c};
-                const uint32_t box[3] = {kUpInW, kUpTH, 3};
-                use_tma = tma::encode(&in_map, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, (void *)f.in, dims, strides, box);
+        for_frame_groups(p, [&](int n0, int nf) {
+            const LLFrame fg = at_frame(f, p.fs, n0);
+            // frame tile by TMA when the buffer meets TMA's rules (16-byte aligned base and strides); the map describes
+            // the input buffer itself (x, y, c), and the group's frames as a fourth dimension when there are several, so a
+            // tile reaching past it reads zeros for pixels that are never stored
+            CUtensorMap in_map = {};
+            bool use_tma = false;
+            if (aligned && !(g_force_naive & 64)) {
+                const int rank = nf > 1 ? 4 : 3;
+                const int64_t strides[3] = {f.in_sy * 2, f.in_sc * 2, p.fs.in * 2};
+                // (every tile's first column must also start on a 16-byte boundary: crops at other even offsets take the
+                // load path; so do frame strides that are no 16-byte multiple)
+                if (tma::strides_ok(fg.in, strides, rank - 1) && (((f.out_x0 & ~1) - f.in_x0) & 7) == 0) {
+                    const uint64_t dims[4] = {(uint64_t)f.in_w, (uint64_t)f.in_h, (uint64_t)f.in_c, (uint64_t)nf};
+                    const uint32_t box[4] = {kUpInW, kUpTH, 3, 1};
+                    use_tma = tma::encode(&in_map, CU_TENSOR_MAP_DATA_TYPE_UINT16, rank, (void *)fg.in, dims, strides, box);
+                }
             }
-        }
-        auto launch = [&](auto kern, bool tma_on) {
-            const int smem = up2_smem_bytes(true, tma_on);
-            const dim3 g = up_grid(f.out_x0, f.out_x0 + f.W - 1, f.row0, f.row0 + f.nrows - 1);
-            (void)resident_slots(kern, 256, smem);  // (sets the > 48 KB shared-memory attribute once per kernel and device)
-            HB_LAUNCH("ll_final2", kern, g, 256, smem, s, p.f, lb[1], lb[1], in_map);
-        };
-        if (use_tma && beta1) launch(ll_up2_kernel<true, true, true, true>, true);
-        else if (use_tma) launch(ll_up2_kernel<true, true, false, true>, true);
-        else if (aligned && beta1) launch(ll_up2_kernel<true, true, true, false>, false);
-        else if (aligned) launch(ll_up2_kernel<true, true, false, false>, false);
-        else if (beta1) launch(ll_up2_kernel<true, false, true, false>, false);
-        else launch(ll_up2_kernel<true, false, false, false>, false);
+            auto launch = [&](auto kern, bool tma_on) {
+                const int smem = up2_smem_bytes(true, tma_on);
+                const dim3 g = up_grid(f.out_x0, f.out_x0 + f.W - 1, f.row0, f.row0 + f.nrows - 1, nf);
+                (void)resident_slots(kern, 256, smem);  // (sets the > 48 KB shared-memory attribute once per kernel and device)
+                HB_LAUNCH("ll_final2", kern, g, 256, smem, s, fg, at_frame(lb[1], 1, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), in_map, 1,
+                          p.fs);
+            };
+            auto pick = [&](auto frames) {
+                constexpr bool F = decltype(frames)::value;
+                if (use_tma && beta1) launch(ll_up2_kernel<true, true, true, true, F>, true);
+                else if (use_tma) launch(ll_up2_kernel<true, true, false, true, F>, true);
+                else if (aligned && beta1) launch(ll_up2_kernel<true, true, true, false, F>, false);
+                else if (aligned) launch(ll_up2_kernel<true, true, false, false, F>, false);
+                else if (beta1) launch(ll_up2_kernel<true, false, true, false, F>, false);
+                else launch(ll_up2_kernel<true, false, false, false, F>, false);
+            };
+            if (nf > 1) pick(std::true_type{});
+            else pick(std::false_type{});
+        });
     } else {
-        HB_LAUNCH("ll_final", ll_final_naive_kernel, grid_for(p.f.W, p.f.nrows), kBlk, 0, s, p.f, lb[1], p.J > 1 ? 1 : 0);
+        for_frame_groups(p, [&](int n0, int nf) {
+            dim3 g = grid_for(p.f.W, p.f.nrows);
+            g.z = nf;
+            HB_LAUNCH("ll_final", ll_final_naive_kernel, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), p.J > 1 ? 1 : 0,
+                      p.fs);
+        });
     }
 }
 
@@ -354,16 +425,17 @@ bool launch_coarse_fused(Plan &p, int j0, cudaStream_t s) {
             coop = it->second;
         }
     }
-    const int slots = resident_slots(ll_coarse_fused_kernel, 256, 0);  // sms * blocks per SM
+    auto kern = p.N > 1 ? ll_coarse_fused_kernel<true> : ll_coarse_fused_kernel<false>;
+    const int slots = resident_slots(kern, 256, 0);  // sms * blocks per SM
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int max_blocks = coop ? (slots > 2 * sms ? 2 * sms : slots) : 0;
     if (max_blocks <= 0) return false;
-    int J = p.J, K = p.K, levels = p.f.levels, jd = fast_down(p) && j0 < 2 ? 2 : j0;
+    int J = p.J, K = p.K, levels = p.f.levels, jd = fast_down(p) && j0 < 2 ? 2 : j0, nf = p.N;
     float flm1 = p.f.flm1;
-    void *args[] = {&p.ls, &J, &j0, &jd, &K, &flm1, &levels};
+    void *args[] = {&p.ls, &J, &j0, &jd, &K, &flm1, &levels, &nf, &p.fs};
     hb::count_launch("ll_coarse_fused", s);
-    cudaError_t e = cudaLaunchCooperativeKernel((void *)ll_coarse_fused_kernel, dim3(max_blocks), dim3(256), args, 0, s);
+    cudaError_t e = cudaLaunchCooperativeKernel((void *)kern, dim3(max_blocks), dim3(256), args, 0, s);
     hb::after_launch(s);
     if (e != cudaSuccess) {
         cudaGetLastError();
@@ -378,9 +450,10 @@ void run_coarse_sweep(Plan &p, int from_level, cudaStream_t s) {
     int j0 = p.J - 1;
     if (!(g_force_naive & 8)) {
         // (level 1 always has its own launch: it is built from the frame, not from a stored level; on the fast path that
-        // launch also builds level 2, and the fused tail's down-sweep starts after it)
+        // launch also builds level 2, and the fused tail's down-sweep starts after it).  The size is the batch's: all N
+        // frames' pixels of the level.
         const int j_min = from_level < 1 ? 1 : from_level;
-        while (j0 > j_min && (int64_t)p.ls.lv[j0].sx.n() * p.ls.lv[j0].sy.n() <= 40 * 1024) j0--;
+        while (j0 > j_min && (int64_t)p.ls.lv[j0].sx.n() * p.ls.lv[j0].sy.n() * p.N <= 40 * 1024) j0--;
     }
     // j0 = last level produced by its own launch; levels j0+1.. are fused (if any)
     bool fused = false;
@@ -393,12 +466,10 @@ void run_coarse_sweep(Plan &p, int from_level, cudaStream_t s) {
     for (int j = j0; j > from_level; j--) launch_up(p, j, s);
 }
 
-}  // namespace
-
-extern "C" int local_laplacian(halide_buffer_t *input, int32_t levels, float alpha, float beta, halide_buffer_t *output) {
+// One GPU, args = {input, output} of 3 dimensions (one frame) or 4 (a batch of frames along dimension 3).
+int run_local_laplacian(hb::Arg *args, int levels, float alpha, float beta, const char *what) {
     int r;
     bool done;
-    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[4]}};
     if ((r = check_and_query(args, levels, &done)) || done) return r;
     if ((r = hb::acquire(args, 2))) return r;
 
@@ -418,9 +489,23 @@ extern "C" int local_laplacian(halide_buffer_t *input, int32_t levels, float alp
         run_coarse_sweep(p, 0, s);
         launch_final(p, s);
     }
-    return hb::finish(args, 2, "local_laplacian launch");
+    return hb::finish(args, 2, what);
+}
+
+}  // namespace
+
+extern "C" int local_laplacian(halide_buffer_t *input, int32_t levels, float alpha, float beta, halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[4]}};
+    return run_local_laplacian(args, levels, alpha, beta, "local_laplacian launch");
 }
 HB_EXPORT_FILTER(local_laplacian, kArgs)
+
+// Batch entry point (library extension): every frame of a 4-D (x, y, c, n) buffer through one launch sequence.
+extern "C" int halide_b200_local_laplacian_batch(halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                                 halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kBatchArgs[0]}, {output, kBatchArgs[1]}};
+    return run_local_laplacian(args, levels, alpha, beta, "local_laplacian_batch launch");
+}
 // The harness's second AOT variant (apps/local_laplacian/process.cpp:44-48): same implementation.
 HB_EXPORT_AUTO_SCHEDULE(local_laplacian, kArgs)
 

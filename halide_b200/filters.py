@@ -22,6 +22,13 @@ def local_laplacian(input, levels, alpha, beta, output):
                                      ctypes.c_float(beta), output.ptr))
 
 
+def local_laplacian_batch(input, levels, alpha, beta, output):
+    """local_laplacian on every frame of 4-D (x, y, c, n) buffers, e.g. an (N, 3, H, W) uint16 torch tensor or numpy
+    array: output frame n = local_laplacian(input frame n), bit for bit, in one launch sequence for the whole batch."""
+    return check(lib.halide_b200_local_laplacian_batch(input.ptr, ctypes.c_int32(levels), ctypes.c_float(alpha),
+                                                       ctypes.c_float(beta), output.ptr))
+
+
 def stencil_chain(input, output):
     """apps/stencil_chain/stencil_chain_generator.cpp: 32 chained 5x5 uint16 stencils."""
     return check(lib.stencil_chain(input.ptr, output.ptr))

@@ -287,6 +287,14 @@ int halide_b200_dist_size(void);
 int halide_b200_local_laplacian_sharded(struct halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                         struct halide_buffer_t *output, int32_t frame_y_min, int32_t frame_y_extent);
 
+/* local_laplacian on every frame of a 4-D (x, y, c, n) uint16 buffer: output frame n = local_laplacian(input frame n,
+ * levels, alpha, beta), bit for bit, with repeat_edge acting on x, y, c of the input per frame.  The input must cover
+ * the output's region in all four dimensions (else halide_error_code_access_out_of_bounds); a bounds query answers
+ * with the output's region.  All frames share one launch sequence: every kernel spreads the batch's work over the
+ * whole GPU, and the coarse pyramid levels of all frames run in one cooperative launch. */
+int halide_b200_local_laplacian_batch(struct halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                      struct halide_buffer_t *output);
+
 /* Host-only probe of the band geometry for tests: with level jr gathered, out[j*8..j*8+7] = {own.lo, own.hi, d.lo, d.hi,
  * u.lo, u.hi, S.lo, S.hi} per pyramid level j = 0..7 (rows owned in the gather partition / Gaussian-side rows computed and
  * held / outGPyramid rows needed / the level's rows on the whole frame), out[64..65] = input rows read; out[66]. */
