@@ -25,9 +25,9 @@ __host__ __device__ inline int fdiv2(int a) { return a >> 1; }  // Euclidean /2 
 
 struct Level {
     Span sx, sy;   // stored region of the Gaussian-side planes (gPyramid[j] K planes + inGPyramid[j])
-    Span ox, oy;   // region of outGPyramid[j] (stored)
-    Span cy, coy;  // rows this device COMPUTES (== sy / oy on one GPU; the owned band when row-sharded)
-    Span gy, goy;  // rows of the whole frame's S_j / O_j (== sy / oy on one GPU): the clamp range
+    Span ox, oy;   // region of outGPyramid[j], stored and computed here (oy: the rank's rows when row-sharded)
+    Span cy;       // Gaussian-side rows this device COMPUTES (== sy on one GPU; the owned band when row-sharded)
+    Span gy;       // rows of the whole frame's S_j (== sy on one GPU): the clamp range
     int xo;        // even column origin of the Gaussian-side arrays: column x lives at index x - xo
     int gpitch;    // pixels per row of the Gaussian-side planes
     int opitch;    // pixels per row of the outG plane
@@ -71,8 +71,7 @@ inline Geom make_geom(Span outx, Span outy, Span inx, Span iny, int J) {
     for (int j = 0; j < J; j++) {
         g.lv[j].sx = SX[j]; g.lv[j].sy = SY[j];
         g.lv[j].ox = OX[j]; g.lv[j].oy = OY[j];
-        g.lv[j].cy = SY[j]; g.lv[j].coy = OY[j];
-        g.lv[j].gy = SY[j]; g.lv[j].goy = OY[j];
+        g.lv[j].cy = SY[j]; g.lv[j].gy = SY[j];
         g.lv[j].xo = SX[j].lo & ~1;  // (two's complement: rounds toward -inf, also for negative lows)
         g.lv[j].gpitch = (SX[j].hi - g.lv[j].xo + 1 + 3) & ~3;
         g.lv[j].opitch = (OX[j].n() + 3) & ~3;
@@ -150,7 +149,6 @@ inline void compute_shard_rows(const Geom &whole, Span frame_y, Span band, bool 
 inline Geom make_shard_geom(const Geom &whole, const ShardLevel *sl, int jr) {
     Geom g = whole;
     for (int j = 1; j < whole.J; j++) {
-        g.lv[j].gy = whole.lv[j].sy; g.lv[j].goy = whole.lv[j].oy;
         if (j >= jr) {
             // held for the whole frame; level jr is produced band by band (cy = own) and completed by the gather
             g.lv[j].cy = j == jr ? sl[j].own : whole.lv[j].sy;
@@ -161,7 +159,7 @@ inline Geom make_shard_geom(const Geom &whole, const ShardLevel *sl, int jr) {
         Span o = sl[j].u;
         if (o.lo < whole.lv[j].oy.lo) o.lo = whole.lv[j].oy.lo;
         if (o.hi > whole.lv[j].oy.hi) o.hi = whole.lv[j].oy.hi;
-        g.lv[j].oy = o; g.lv[j].coy = o;
+        g.lv[j].oy = o;
     }
     return g;
 }

@@ -1,18 +1,8 @@
 // local_laplacian.cu — host side of local_laplacian(input, levels, alpha, beta, output) for sm_90a:
 // the C-ABI entry points (reference: apps/local_laplacian/local_laplacian_generator.cpp:12-16,287 and
 // the harness apps/local_laplacian/process.cpp:31), argument validation, pyramid geometry, scratch
-// allocation, the launch sequence, and the row-sharded multi-GPU variant.  Kernels: ll_kernels.cuh.
-//
-// Data layout in HBM (all f32, callee-owned scratch):
-//   lut      [2*256*(levels-1)+1]            remap(i), i in [-256(levels-1), 256(levels-1)]
-//   gp[j]    [sy_j][gpitch_j][K]  j=1..J-1   gPyramid[j], the K=levels planes interleaved per
-//                                            pixel (K=8 -> one 32-byte sector per pixel, so the
-//                                            data-dependent (li, li+1) plane pick costs one sector)
-//   ing[j]   [sy_j][gpitch_j]     j=1..J-1   inGPyramid[j]
-//   outg[j]  [oy_j][opitch_j]     j=1..J-1   outGPyramid[j]
-// gray / gPyramid[0] / lPyramid / outLPyramid / outGPyramid[0] are never materialised: they are
-// recomputed from the uint16 input where needed (8 f32 planes at full resolution would be
-// 32 B/px of traffic against 12 B/px of compulsory I/O).
+// allocation, the launch sequence, and the row-sharded multi-GPU variant.  Kernels and the HBM layout of the
+// callee-owned scratch: ll_kernels.cuh.
 #include <stdlib.h>
 #include <string.h>
 
@@ -51,13 +41,10 @@ const halide_filter_argument_t kBatchArgs[2] = {
 // Everything one call needs on the device: frame description + per-level buffers, for N frames of one geometry.
 struct Plan {
     LLFrame f;
-    LevelSet ls;
-    ll::Geom geom;
-    int J, K;
+    LevelSet ls{};  // (level 0 is never stored: its slot stays zero)
     int N;  // frames (1 but for a batch)
     FrameStrides fs;  // all zero when N == 1
     float alpha;
-    float *lut;
 };
 
 // Grids index frames by blockIdx.z; batches beyond its limit launch in groups of frames [n0, n0 + count).
@@ -105,7 +92,6 @@ void fill_frame(Plan &p, const hb::Arg *args, int levels, float alpha, float bet
     f.out_sy = output->dim[1].stride; f.out_sc = output->dim[2].stride;
     f.out_x0 = output->dim[0].min; f.out_y0 = output->dim[1].min; f.out_c0 = output->dim[2].min;
     f.W = output->dim[0].extent; f.H = output->dim[1].extent; f.C = output->dim[2].extent;
-    f.row0 = f.out_y0; f.nrows = f.H;
     p.fs = FrameStrides{};
     p.N = 1;
     if (output->dimensions == 4) {
@@ -123,8 +109,6 @@ void fill_frame(Plan &p, const hb::Arg *args, int levels, float alpha, float bet
     f.flm1 = (float)(levels - 1);
     f.inv_lm1 = 1.0f / (float)(levels - 1);
     f.lut_half = 256 * (levels - 1);
-    p.K = levels;
-    p.J = ll::kMaxJ;
     p.alpha = alpha;
 }
 
@@ -147,7 +131,6 @@ int get_lut(Plan &p, cudaStream_t s) {
     std::lock_guard<std::mutex> lock(g_lut_mu);
     for (const LutEntry &e : g_luts) {
         if (e.device == dev && e.levels == p.f.levels && memcmp(&e.alpha, &p.alpha, sizeof(float)) == 0) {
-            p.lut = e.lut;
             p.f.lut = e.lut;
             return 0;
         }
@@ -170,36 +153,37 @@ int get_lut(Plan &p, cudaStream_t s) {
         return hb::fail(halide_error_code_device_run_failed, "local_laplacian: remap table kernel failed");
     }
     g_luts.push_back({dev, p.f.levels, p.alpha, lut});
-    p.lut = lut;
     p.f.lut = lut;
     return 0;
 }
 
-int alloc_levels(Plan &p, hb::Scratch &scratch) {
-    const int nq = (p.K + 1) / 2;
-    for (int j = 1; j < p.J; j++) {
-        const ll::Level &lv = p.geom.lv[j];
+// the fast level-1 kernel also produces level 2
+bool fast_down(const Plan &p) { return p.f.levels == 8 && !(g_force_naive & 1); }
+
+int alloc_levels(Plan &p, const ll::Geom &geom, hb::Scratch &scratch) {
+    const int nq = (p.f.levels + 1) / 2;
+    for (int j = 1; j < ll::kMaxJ; j++) {
+        const ll::Level &lv = geom.lv[j];
         LevelBuf &b = p.ls.lv[j];
         b.sx = lv.sx; b.sy = lv.sy; b.ox = lv.ox; b.oy = lv.oy;
-        b.cy = lv.cy; b.coy = lv.coy; b.gy = lv.gy;
+        b.cy = lv.cy; b.coy = lv.oy; b.gy = lv.gy;
         b.xo = lv.xo; b.nq = nq;
         b.gpitch = lv.gpitch; b.opitch = lv.opitch;
-        b.has_pair = 0;
         // one allocation per array for all N frames; a frame's slice starts on 256 bytes, like an allocation of its own
         auto slice = [](size_t floats) { return (int64_t)((floats + 63) & ~size_t(63)); };
-        const size_t gpix = (size_t)lv.sy.n() * lv.gpitch;
-        const int64_t gp_sn = slice(gpix * nq * 2), ing_sn = slice(gpix), pair_sn = p.K == 8 ? slice(gpix * 2) : ing_sn;
-        const int64_t outg_sn = slice((size_t)lv.oy.n() * lv.opitch);
+        const size_t gpix = (size_t)b.sy.n() * b.gpitch;
+        const bool with_pair = j == 1 && fast_down(p);  // (written by the level-1 kernel only)
+        const int64_t gp_sn = slice(gpix * nq * 2), ing_sn = slice(gpix), pair_sn = with_pair ? slice(gpix * 2) : 0;
+        const int64_t outg_sn = slice((size_t)b.oy.n() * b.opitch);
         b.gp = scratch.get<float>((size_t)gp_sn * p.N);
         b.ing = scratch.get<float>((size_t)ing_sn * p.N);
-        b.pair = p.K == 8 ? scratch.get<float>((size_t)pair_sn * p.N) : b.ing;
+        if (with_pair) b.pair = scratch.get<float>((size_t)pair_sn * p.N);
         b.outg = scratch.get<float>((size_t)outg_sn * p.N);
         if (p.N > 1) p.fs.gp[j] = gp_sn, p.fs.ing[j] = ing_sn, p.fs.pair[j] = pair_sn, p.fs.outg[j] = outg_sn;
-        if (!b.gp || !b.ing || !b.pair || !b.outg) {
+        if (!b.gp || !b.ing || (with_pair && !b.pair) || !b.outg) {
             return hb::fail(halide_error_code_device_malloc_failed, "local_laplacian: scratch allocation failed");
         }
     }
-    p.ls.lv[0] = p.ls.lv[1];  // level 0 is never stored; keep the slot initialised
     return 0;
 }
 
@@ -286,11 +270,7 @@ void launch_level12(Plan &p, const LLFrame &f, Span cy1, Span cy2, cudaStream_t 
     else if (beta1) launch_level12_kernel<true, false>(p, f, cy1, cy2, s);
     else if (frames) launch_level12_kernel<false, true>(p, f, cy1, cy2, s);
     else launch_level12_kernel<false, false>(p, f, cy1, cy2, s);
-    p.ls.lv[1].has_pair = 1;
 }
-
-// the fast level-1 kernel also produces level 2
-bool fast_down(const Plan &p) { return p.K == 8 && !(g_force_naive & 1); }
 
 void launch_down(Plan &p, int j, cudaStream_t s) {  // produce level j (j >= 1) rows cy
     LevelBuf *lb = p.ls.lv;
@@ -320,7 +300,7 @@ void launch_down(Plan &p, int j, cudaStream_t s) {  // produce level j (j >= 1) 
         for_frame_groups(p, [&](int n0, int nf) {
             dim3 g = grid_for(lb[j].sx.n(), lb[j].cy.n());
             g.z = nf;
-            HB_LAUNCH("ll_down", ll_down_naive_kernel, g, kBlk, 0, s, at_frame(lb[j - 1], j - 1, p.fs, n0), at_frame(lb[j], j, p.fs, n0), p.K, j,
+            HB_LAUNCH("ll_down", ll_down_naive_kernel, g, kBlk, 0, s, at_frame(lb[j - 1], j - 1, p.fs, n0), at_frame(lb[j], j, p.fs, n0), p.f.levels, j,
                       p.fs);
         });
     }
@@ -333,9 +313,9 @@ dim3 up_grid(int x_lo, int x_hi, int y_lo, int y_hi, int nf) {  // tiles on even
 void launch_up(Plan &p, int j, cudaStream_t s) {  // produce outGPyramid[j] (1 <= j <= J-1) rows coy
     LevelBuf *lb = p.ls.lv;
     if (lb[j].coy.n() <= 0) return;
-    const bool fast_up = (p.K == 8) && !(g_force_naive & 2);
+    const bool fast_up = p.f.levels == 8 && !(g_force_naive & 2);
     for_frame_groups(p, [&](int n0, int nf) {
-        if (fast_up && j < p.J - 1) {
+        if (fast_up && j < ll::kMaxJ - 1) {
             static const CUtensorMap no_map = {};
             HB_LAUNCH("ll_up2", (nf > 1 ? ll_up2_kernel<false, false, true, false, true> : ll_up2_kernel<false, false, true, false, false>), up_grid(lb[j].ox.lo, lb[j].ox.hi, lb[j].coy.lo, lb[j].coy.hi, nf),
                       256, up2_smem_bytes(false, false), s, at_frame(p.f, p.fs, n0), at_frame(lb[j], j, p.fs, n0),
@@ -343,17 +323,16 @@ void launch_up(Plan &p, int j, cudaStream_t s) {  // produce outGPyramid[j] (1 <
         } else {
             dim3 g = grid_for(lb[j].ox.n(), lb[j].coy.n());
             g.z = nf;
-            const int jc = j == p.J - 1 ? j : j + 1;
+            const int jc = j == ll::kMaxJ - 1 ? j : j + 1;
             HB_LAUNCH("ll_up", ll_up_naive_kernel, g, kBlk, 0, s, at_frame(lb[j], j, p.fs, n0), at_frame(lb[jc], jc, p.fs, n0),
-                      p.f.flm1, p.f.levels, j == p.J - 1 ? 1 : 0, j, p.fs);
+                      p.f.flm1, p.f.levels, j == ll::kMaxJ - 1 ? 1 : 0, j, p.fs);
         }
     });
 }
 
 void launch_final(Plan &p, cudaStream_t s) {
     LevelBuf *lb = p.ls.lv;
-    if (p.f.nrows <= 0) return;
-    if (p.J > 1 && p.K == 8 && !(g_force_naive & 4) && p.f.C <= 3) {
+    if (p.f.levels == 8 && !(g_force_naive & 4) && p.f.C <= 3) {
         const LLFrame &f = p.f;
         // the common layout takes the kernel's ALIGNED path (32-bit addressing, one aligned word per thread and channel)
         const int64_t in_span = (int64_t)f.in_h * f.in_sy + 3 * f.in_sc, out_span = (int64_t)f.H * f.out_sy + 3 * f.out_sc;
@@ -383,7 +362,7 @@ void launch_final(Plan &p, cudaStream_t s) {
             }
             auto launch = [&](auto kern, bool tma_on) {
                 const int smem = up2_smem_bytes(true, tma_on);
-                const dim3 g = up_grid(f.out_x0, f.out_x0 + f.W - 1, f.row0, f.row0 + f.nrows - 1, nf);
+                const dim3 g = up_grid(f.out_x0, f.out_x0 + f.W - 1, f.out_y0, f.out_y0 + f.H - 1, nf);
                 (void)resident_slots(kern, 256, smem);  // (sets the > 48 KB shared-memory attribute once per kernel and device)
                 HB_LAUNCH("ll_final2", kern, g, 256, smem, s, fg, at_frame(lb[1], 1, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), in_map, 1,
                           p.fs);
@@ -402,10 +381,9 @@ void launch_final(Plan &p, cudaStream_t s) {
         });
     } else {
         for_frame_groups(p, [&](int n0, int nf) {
-            dim3 g = grid_for(p.f.W, p.f.nrows);
+            dim3 g = grid_for(p.f.W, p.f.H);
             g.z = nf;
-            HB_LAUNCH("ll_final", ll_final_naive_kernel, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), p.J > 1 ? 1 : 0,
-                      p.fs);
+            HB_LAUNCH("ll_final", ll_final_naive_kernel, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), 1, p.fs);
         });
     }
 }
@@ -431,7 +409,7 @@ bool launch_coarse_fused(Plan &p, int j0, cudaStream_t s) {
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int max_blocks = coop ? (slots > 2 * sms ? 2 * sms : slots) : 0;
     if (max_blocks <= 0) return false;
-    int J = p.J, K = p.K, levels = p.f.levels, jd = fast_down(p) && j0 < 2 ? 2 : j0, nf = p.N;
+    int J = ll::kMaxJ, K = p.f.levels, levels = p.f.levels, jd = fast_down(p) && j0 < 2 ? 2 : j0, nf = p.N;
     float flm1 = p.f.flm1;
     void *args[] = {&p.ls, &J, &j0, &jd, &K, &flm1, &levels, &nf, &p.fs};
     hb::count_launch("ll_coarse_fused", s);
@@ -447,7 +425,7 @@ bool launch_coarse_fused(Plan &p, int j0, cudaStream_t s) {
 // Levels from_level+1 .. J-1 down, then J-1 .. from_level+1 up: the part of the sweep that runs on whole levels
 // (everything on one GPU; the replicated coarse levels when row-sharded).  Small levels share one cooperative launch.
 void run_coarse_sweep(Plan &p, int from_level, cudaStream_t s) {
-    int j0 = p.J - 1;
+    int j0 = ll::kMaxJ - 1;
     if (!(g_force_naive & 8)) {
         // (level 1 always has its own launch: it is built from the frame, not from a stored level; on the fast path that
         // launch also builds level 2, and the fused tail's down-sweep starts after it).  The size is the batch's: all N
@@ -458,10 +436,10 @@ void run_coarse_sweep(Plan &p, int from_level, cudaStream_t s) {
     // j0 = last level produced by its own launch; levels j0+1.. are fused (if any)
     bool fused = false;
     for (int j = from_level + 1; j <= j0; j++) launch_down(p, j, s);
-    if (j0 < p.J - 1) fused = launch_coarse_fused(p, j0, s);
+    if (j0 < ll::kMaxJ - 1) fused = launch_coarse_fused(p, j0, s);
     if (!fused) {
-        for (int j = j0 + 1; j < p.J; j++) launch_down(p, j, s);
-        for (int j = p.J - 1; j > j0; j--) launch_up(p, j, s);
+        for (int j = j0 + 1; j < ll::kMaxJ; j++) launch_down(p, j, s);
+        for (int j = ll::kMaxJ - 1; j > j0; j--) launch_up(p, j, s);
     }
     for (int j = j0; j > from_level; j--) launch_up(p, j, s);
 }
@@ -478,9 +456,8 @@ int run_local_laplacian(hb::Arg *args, int levels, float alpha, float beta, cons
     const int W = p.f.W, H = p.f.H;
     Span outx = {p.f.out_x0, p.f.out_x0 + W - 1}, outy = {p.f.out_y0, p.f.out_y0 + H - 1};
     Span inx = {p.f.in_x0, p.f.in_x0 + p.f.in_w - 1}, iny = {p.f.in_y0, p.f.in_y0 + p.f.in_h - 1};
-    p.geom = ll::make_geom(outx, outy, inx, iny, p.J);
     hb::Scratch scratch;
-    if ((r = alloc_levels(p, scratch))) return r;
+    if ((r = alloc_levels(p, ll::make_geom(outx, outy, inx, iny, ll::kMaxJ), scratch))) return r;
 
     cudaStream_t s = hb::stream();
     if ((r = get_lut(p, s))) return r;
@@ -581,8 +558,8 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
     const int W = p.f.W, C = p.f.in_c;
     Span outx = {p.f.out_x0, p.f.out_x0 + W - 1};
     Span inx = {p.f.in_x0, p.f.in_x0 + p.f.in_w - 1};
-    const ll::Geom whole = ll::make_geom(outx, frame_y, inx, frame_y, p.J);
-    const int jr = choose_coarse_level(whole, nranks, p.J, p.K);
+    const ll::Geom whole = ll::make_geom(outx, frame_y, inx, frame_y, ll::kMaxJ);
+    const int jr = choose_coarse_level(whole, nranks, ll::kMaxJ, p.f.levels);
 
     // every rank's band: gathered once per geometry (collective on first use / change) and per communicator (a rank
     // that kept its plan from an earlier group would skip the gather its new peers enter)
@@ -612,7 +589,7 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
     for (int q = 0; q < nranks; q++) {
         ll::ShardLevel t[ll::kMaxJ];
         rows_of(q, t, &need[q]);
-        for (int j = 1; j <= jr && j < p.J; j++) {
+        for (int j = 1; j <= jr && j < ll::kMaxJ; j++) {
             if (t[j].own.n() < 1) {
                 return hb::fail(halide_error_code_constraint_violated,
                                 "local_laplacian_sharded: rank %d's band of %d rows is too small for %d ranks (level %d owns no row)", q,
@@ -629,11 +606,10 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
     ll::ShardLevel sl[ll::kMaxJ];
     Span in_need;
     rows_of(rank, sl, &in_need);
-    p.geom = ll::make_shard_geom(whole, sl, jr);
     p.f.clamp_y0 = frame_y.lo;
     p.f.clamp_h = frame_y.n();
     hb::Scratch scratch;
-    if ((r = alloc_levels(p, scratch))) return r;
+    if ((r = alloc_levels(p, ll::make_shard_geom(whole, sl, jr), scratch))) return r;
 
     // ---- input halo: rows [in_need.lo, band.lo) from the rank above, (band.hi, in_need.hi] from the rank below ----
     const int ht = band.lo - in_need.lo, hbn = in_need.hi - band.hi;
@@ -758,8 +734,7 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
                 if (r) return r;
             }
         }
-        lb[jr].cy = lb[jr].sy;   // from here on level jr is complete (its pair plane is not: the up-sweep gathers from gp)
-        lb[jr].has_pair = 0;
+        lb[jr].cy = lb[jr].sy;   // from here on level jr is complete
         run_coarse_sweep(p, jr, s);          // levels jr+1.. down, ..jr+1 up, whole frame, on every rank
         launch_up(p, jr, s);
         for (int j = jr - 1; j >= 1; j--) launch_up(p, j, s);

@@ -297,7 +297,7 @@ int halide_b200_local_laplacian_batch(struct halide_buffer_t *input, int32_t lev
 
 /* Host-only probe of the band geometry for tests: with level jr gathered, out[j*8..j*8+7] = {own.lo, own.hi, d.lo, d.hi,
  * u.lo, u.hi, S.lo, S.hi} per pyramid level j = 0..7 (rows owned in the gather partition / Gaussian-side rows computed and
- * held / outGPyramid rows needed / the level's rows on the whole frame), out[64..65] = input rows read; out[66]. */
+ * held / outGPyramid rows needed / the level's rows on the whole frame), out[64..65] = input rows read. */
 int halide_b200_ll_band_geometry(int32_t frame_w, int32_t frame_h, int32_t band_lo, int32_t band_hi, int32_t first,
                                  int32_t last, int32_t jr, int32_t *out);
 /* Row-sharded local_laplacian: pyramid level gathered all-to-all so that the coarser levels are computed

@@ -159,7 +159,7 @@ def test_beta_not_one_takes_the_general_kernels(hb, oracle):
 
 
 def test_wide_frame_many_strips(hb, oracle):
-    """A frame wide enough for several 30-column strips and 64-column tiles per row, odd sizes."""
+    """A frame wide enough for several 28-column level-1 strips and 60-column tiles per row, odd sizes."""
     _check(hb, oracle, u16_frame((3, 77, 1031), 8), 8, 1.0 / 7.0, 1.0)
 
 
@@ -171,19 +171,19 @@ def test_final_kernel_simple_and_general_layout_paths(hb, oracle, shape):
     img = u16_frame(shape, 77)
     want = oracle.local_laplacian(img, 8, 1.0 / 7.0, 1.0)
     l = hb.load_library()
-    got_simple = run_local_laplacian(hb, img, 8, 1.0 / 7.0, 1.0)
+    got_aligned = run_local_laplacian(hb, img, 8, 1.0 / 7.0, 1.0)
     try:
         l.halide_b200_ll_force_generic(16)
         got_general = run_local_laplacian(hb, img, 8, 1.0 / 7.0, 1.0)
     finally:
         l.halide_b200_ll_force_generic(0)
-    assert np.array_equal(got_simple, want) and np.array_equal(got_general, want)
+    assert np.array_equal(got_aligned, want) and np.array_equal(got_general, want)
     c, h, w = shape
     out_shape = (3, h - 9, w - 12)  # even width, output columns start at an odd input column
     want_crop = oracle.local_laplacian(img, 8, 1.0 / 7.0, 1.0, out_shape=out_shape, in_mins=(0, 0, 0), out_mins=(5, 4, 0))
     got_crop = run_local_laplacian(hb, img, 8, 1.0 / 7.0, 1.0, out_shape=out_shape, in_mins=(0, 0, 0), out_mins=(5, 4, 0))
     assert np.array_equal(got_crop, want_crop)
-    out_shape = (3, h - 8, w - 12)  # even offsets: SIMPLE path on a crop (row pointer no longer at the buffer start)
+    out_shape = (3, h - 8, w - 12)  # even offsets: aligned path on a crop (row pointer no longer at the buffer start)
     want_crop = oracle.local_laplacian(img, 8, 1.0 / 7.0, 1.0, out_shape=out_shape, in_mins=(0, 0, 0), out_mins=(6, 4, 0))
     got_crop = run_local_laplacian(hb, img, 8, 1.0 / 7.0, 1.0, out_shape=out_shape, in_mins=(0, 0, 0), out_mins=(6, 4, 0))
     assert np.array_equal(got_crop, want_crop)
