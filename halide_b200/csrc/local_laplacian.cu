@@ -159,6 +159,10 @@ int get_lut(Plan &p, cudaStream_t s) {
 
 // the fast level-1 kernel also produces level 2
 bool fast_down(const Plan &p) { return p.f.levels == 8 && !(g_force_naive & 1); }
+// the fast final kernel also produces outGPyramid[1] (for its own tile), so no up-sweep launch runs for level 1
+bool fast_final(const Plan &p) { return p.f.levels == 8 && !(g_force_naive & 4) && p.f.C <= 3; }
+// lowest level the up-sweep launches produce
+int first_up_level(const Plan &p) { return fast_final(p) ? 2 : 1; }
 
 int alloc_levels(Plan &p, const ll::Geom &geom, hb::Scratch &scratch) {
     const int nq = (p.f.levels + 1) / 2;
@@ -172,15 +176,13 @@ int alloc_levels(Plan &p, const ll::Geom &geom, hb::Scratch &scratch) {
         // one allocation per array for all N frames; a frame's slice starts on 256 bytes, like an allocation of its own
         auto slice = [](size_t floats) { return (int64_t)((floats + 63) & ~size_t(63)); };
         const size_t gpix = (size_t)b.sy.n() * b.gpitch;
-        const bool with_pair = j == 1 && fast_down(p);  // (written by the level-1 kernel only)
-        const int64_t gp_sn = slice(gpix * nq * 2), ing_sn = slice(gpix), pair_sn = with_pair ? slice(gpix * 2) : 0;
-        const int64_t outg_sn = slice((size_t)b.oy.n() * b.opitch);
+        const bool with_outg = j >= first_up_level(p);  // (level 1's is computed inside the fast final kernel)
+        const int64_t gp_sn = slice(gpix * nq * 2), ing_sn = slice(gpix), outg_sn = with_outg ? slice((size_t)b.oy.n() * b.opitch) : 0;
         b.gp = scratch.get<float>((size_t)gp_sn * p.N);
         b.ing = scratch.get<float>((size_t)ing_sn * p.N);
-        if (with_pair) b.pair = scratch.get<float>((size_t)pair_sn * p.N);
-        b.outg = scratch.get<float>((size_t)outg_sn * p.N);
-        if (p.N > 1) p.fs.gp[j] = gp_sn, p.fs.ing[j] = ing_sn, p.fs.pair[j] = pair_sn, p.fs.outg[j] = outg_sn;
-        if (!b.gp || !b.ing || (with_pair && !b.pair) || !b.outg) {
+        b.outg = with_outg ? scratch.get<float>((size_t)outg_sn * p.N) : nullptr;
+        if (p.N > 1) p.fs.gp[j] = gp_sn, p.fs.ing[j] = ing_sn, p.fs.outg[j] = outg_sn;
+        if (!b.gp || !b.ing || (with_outg && !b.outg)) {
             return hb::fail(halide_error_code_device_malloc_failed, "local_laplacian: scratch allocation failed");
         }
     }
@@ -278,8 +280,7 @@ void launch_down(Plan &p, int j, cudaStream_t s) {  // produce level j (j >= 1) 
         if (j == 1) {
             launch_level12(p, p.f, lb[1].cy, lb[2].cy, s);
         } else if (j > 2 && lb[j].cy.n() > 0) {
-            // stored levels: load-bound row-group kernel; no pair plane (the up-sweep of these small levels picks its two
-            // planes out of the level itself)
+            // stored levels: load-bound row-group kernel
             const int ns = (lb[j].sx.n() + kRCols - 1) / kRCols, ng = (lb[j].cy.n() + kRG - 1) / kRG;
             const long long tasks = (long long)ns * ng * 5 * p.N;
             auto kern = p.N > 1 ? ll_down_rows_kernel<true> : ll_down_rows_kernel<false>;
@@ -332,7 +333,7 @@ void launch_up(Plan &p, int j, cudaStream_t s) {  // produce outGPyramid[j] (1 <
 
 void launch_final(Plan &p, cudaStream_t s) {
     LevelBuf *lb = p.ls.lv;
-    if (p.f.levels == 8 && !(g_force_naive & 4) && p.f.C <= 3) {
+    if (fast_final(p)) {
         const LLFrame &f = p.f;
         // the common layout takes the kernel's ALIGNED path (32-bit addressing, one aligned word per thread and channel)
         const int64_t in_span = (int64_t)f.in_h * f.in_sy + 3 * f.in_sc, out_span = (int64_t)f.H * f.out_sy + 3 * f.out_sc;
@@ -364,7 +365,7 @@ void launch_final(Plan &p, cudaStream_t s) {
                 const int smem = up2_smem_bytes(true, tma_on);
                 const dim3 g = up_grid(f.out_x0, f.out_x0 + f.W - 1, f.out_y0, f.out_y0 + f.H - 1, nf);
                 (void)resident_slots(kern, 256, smem);  // (sets the > 48 KB shared-memory attribute once per kernel and device)
-                HB_LAUNCH("ll_final2", kern, g, 256, smem, s, fg, at_frame(lb[1], 1, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), in_map, 1,
+                HB_LAUNCH("ll_final2", kern, g, 256, smem, s, fg, at_frame(lb[1], 1, p.fs, n0), at_frame(lb[2], 2, p.fs, n0), in_map, 1,
                           p.fs);
             };
             auto pick = [&](auto frames) {
@@ -441,7 +442,7 @@ void run_coarse_sweep(Plan &p, int from_level, cudaStream_t s) {
         for (int j = j0 + 1; j < ll::kMaxJ; j++) launch_down(p, j, s);
         for (int j = ll::kMaxJ - 1; j > j0; j--) launch_up(p, j, s);
     }
-    for (int j = j0; j > from_level; j--) launch_up(p, j, s);
+    for (int j = j0; j > from_level && j >= first_up_level(p); j--) launch_up(p, j, s);
 }
 
 // One GPU, args = {input, output} of 3 dimensions (one frame) or 4 (a batch of frames along dimension 3).
@@ -737,7 +738,7 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
         lb[jr].cy = lb[jr].sy;   // from here on level jr is complete
         run_coarse_sweep(p, jr, s);          // levels jr+1.. down, ..jr+1 up, whole frame, on every rank
         launch_up(p, jr, s);
-        for (int j = jr - 1; j >= 1; j--) launch_up(p, j, s);
+        for (int j = jr - 1; j >= first_up_level(p); j--) launch_up(p, j, s);
         launch_final(p, s);
     }
     return hb::finish(args, 2, "local_laplacian_sharded launch");
