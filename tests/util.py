@@ -3,6 +3,7 @@ reference produced."""
 import hashlib
 import json
 import os
+from contextlib import contextmanager
 
 import numpy as np
 
@@ -49,6 +50,21 @@ def smooth_u16_frame(shape, seed):
 def f32_frame(shape, seed):
     rng = np.random.default_rng(seed)
     return rng.random(shape, dtype=np.float32)
+
+
+@contextmanager
+def kernels_run(hb):
+    """Collects {kernel name: (launches, ms)} of the launches made inside the block (the library's profile mode), so a
+    test can assert which kernel variant a call took."""
+    report = {}
+    hb.lib.profile_reset()
+    hb.lib.profile(True)
+    try:
+        yield report
+        report.update(hb.lib.profile_report())
+    finally:
+        hb.lib.profile(False)
+        hb.lib.profile_reset()
 
 
 def run_blur(hb, inp, out_shape, in_mins=None, out_mins=None):
