@@ -37,20 +37,46 @@ const halide_filter_argument_t kBatchArgs[2] = {
     {"input", halide_argument_kind_input_buffer, 4, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
     {"output", halide_argument_kind_output_buffer, 4, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
 };
+// halide_b200_local_laplacian_u8 / _u8_batch: uint8 buffers of 3 / 4 dimensions.
+const halide_filter_argument_t kU8Args[2] = {
+    {"input", halide_argument_kind_input_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+    {"output", halide_argument_kind_output_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+};
+const halide_filter_argument_t kU8BatchArgs[2] = {
+    {"input", halide_argument_kind_input_buffer, 4, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+    {"output", halide_argument_kind_output_buffer, 4, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+};
 
 // Everything one call needs on the device: frame description + per-level buffers, for N frames of one geometry.
-struct Plan {
-    LLFrame f;
+// T = the frame's element type (uint16_t, or uint8_t for the 8-bit entry points).
+template<typename T>
+struct PlanT {
+    LLFrameT<T> f;
     LevelSet ls{};  // (level 0 is never stored: its slot stays zero)
     int N;  // frames (1 but for a batch)
     FrameStrides fs;  // all zero when N == 1
     float alpha;
 };
+using Plan = PlanT<uint16_t>;
+
+// The non-final up-sweep launches read only the frame's scalars (levels, remap table), never a sample, so one
+// instantiation of them serves every element type: they get the frame description retyped to uint16_t.
+template<typename T>
+LLFrame scalars_frame(const LLFrameT<T> &f) {
+    if constexpr (std::is_same<T, uint16_t>::value) {
+        return f;
+    } else {
+        static_assert(sizeof(LLFrame) == sizeof(LLFrameT<T>), "frame descriptions differ only in their pointer types");
+        LLFrame g;
+        memcpy(&g, &f, sizeof g);
+        return g;
+    }
+}
 
 // Grids index frames by blockIdx.z; batches beyond its limit launch in groups of frames [n0, n0 + count).
 constexpr int kMaxGridZ = 65535;
-template<typename F>
-void for_frame_groups(const Plan &p, F launch) {
+template<typename P, typename F>
+void for_frame_groups(const P &p, F launch) {
     for (int n0 = 0; n0 < p.N; n0 += kMaxGridZ) launch(n0, std::min(kMaxGridZ, p.N - n0));
 }
 
@@ -78,17 +104,18 @@ int check_and_query(hb::Arg *args, int levels, bool *done) {
     return 0;
 }
 
-void fill_frame(Plan &p, const hb::Arg *args, int levels, float alpha, float beta) {
+template<typename T>
+void fill_frame(PlanT<T> &p, const hb::Arg *args, int levels, float alpha, float beta) {
     const halide_buffer_t *input = args[0].b, *output = args[1].b;
-    LLFrame &f = p.f;
-    f.in = (const uint16_t *)args[0].dev;
+    LLFrameT<T> &f = p.f;
+    f.in = (const T *)args[0].dev;
     f.in_sy = input->dim[1].stride; f.in_sc = input->dim[2].stride;
     f.in_x0 = input->dim[0].min; f.in_y0 = input->dim[1].min; f.in_c0 = input->dim[2].min;
     f.in_w = input->dim[0].extent; f.in_h = input->dim[1].extent; f.in_c = input->dim[2].extent;
     f.clamp_y0 = f.in_y0; f.clamp_h = f.in_h;
     f.halo_top = f.halo_bot = nullptr;
     f.halo_top_rows = f.halo_bot_rows = f.halo_pitch = 0;
-    f.out = (uint16_t *)args[1].dev;
+    f.out = (T *)args[1].dev;
     f.out_sy = output->dim[1].stride; f.out_sc = output->dim[2].stride;
     f.out_x0 = output->dim[0].min; f.out_y0 = output->dim[1].min; f.out_c0 = output->dim[2].min;
     f.W = output->dim[0].extent; f.H = output->dim[1].extent; f.C = output->dim[2].extent;
@@ -125,7 +152,8 @@ struct LutEntry {
 std::mutex g_lut_mu;
 std::vector<LutEntry> g_luts;
 
-int get_lut(Plan &p, cudaStream_t s) {
+template<typename T>
+int get_lut(PlanT<T> &p, cudaStream_t s) {
     int dev = 0;
     cudaGetDevice(&dev);
     std::lock_guard<std::mutex> lock(g_lut_mu);
@@ -158,13 +186,17 @@ int get_lut(Plan &p, cudaStream_t s) {
 }
 
 // the fast level-1 kernel also produces level 2
-bool fast_down(const Plan &p) { return p.f.levels == 8 && !(g_force_naive & 1); }
+template<typename P>
+bool fast_down(const P &p) { return p.f.levels == 8 && !(g_force_naive & 1); }
 // the fast final kernel also produces outGPyramid[1] (for its own tile), so no up-sweep launch runs for level 1
-bool fast_final(const Plan &p) { return p.f.levels == 8 && !(g_force_naive & 4) && p.f.C <= 3; }
+template<typename P>
+bool fast_final(const P &p) { return p.f.levels == 8 && !(g_force_naive & 4) && p.f.C <= 3; }
 // lowest level the up-sweep launches produce
-int first_up_level(const Plan &p) { return fast_final(p) ? 2 : 1; }
+template<typename P>
+int first_up_level(const P &p) { return fast_final(p) ? 2 : 1; }
 
-int alloc_levels(Plan &p, const ll::Geom &geom, hb::Scratch &scratch) {
+template<typename P>
+int alloc_levels(P &p, const ll::Geom &geom, hb::Scratch &scratch) {
     const int nq = (p.f.levels + 1) / 2;
     for (int j = 1; j < ll::kMaxJ; j++) {
         const ll::Level &lv = geom.lv[j];
@@ -227,14 +259,14 @@ int resident_slots(Kern kern, int threads, size_t smem) {
 
 // Levels 1 and 2 from the frame (K == 8): stores level-1 rows cy1 and level-2 rows cy2, reading the frame through f
 // (the row-sharded path narrows both spans, and hides the halo rows from the launch that runs before they arrive).
-template<bool BETA1, bool FRAMES>
-void launch_level12_kernel(Plan &p, const LLFrame &f, Span cy1, Span cy2, cudaStream_t s) {
+template<bool BETA1, bool FRAMES, typename T>
+void launch_level12_kernel(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2, cudaStream_t s) {
     LevelBuf d1 = p.ls.lv[1], d2 = p.ls.lv[2];
     d1.cy = cy1;
     d2.cy = cy2;
     // one pair table and kDWarps warp stages: one block per SM
     const size_t smem = kPairLutN * sizeof(float2) + kDWarps * sizeof(DownStage);
-    const int slots = resident_slots(ll_level1_kernel<BETA1, FRAMES>, kDWarps * 32, smem);
+    const int slots = resident_slots(ll_level1_kernel<BETA1, FRAMES, T>, kDWarps * 32, smem);
     // strips of 28 level-1 columns from xbase == xo (mod 4), far enough left that their level-2 columns (xbase/2 + 14k ..)
     // reach level 2's first column; chunks of 8 level-1 rows from an odd ybase, over the rows stored and the taps of
     // the level-2 rows stored
@@ -257,16 +289,19 @@ void launch_level12_kernel(Plan &p, const LLFrame &f, Span cy1, Span cy2, cudaSt
     }
     const long long runs = strips * nr;
     const int g = (int)std::min<long long>(slots, (runs + kDWarps - 1) / kDWarps);
-    // aligned 32-bit loads of a column pair / 32-bit element offsets from the frame's first element
-    const int wide = ((uintptr_t)f.in & 3) == 0 && (f.in_sy & 1) == 0 && (f.in_sc & 1) == 0 && (p.fs.in & 1) == 0 &&
-                     (f.in_x0 & 1) == 0 && ((uintptr_t)f.halo_top & 3) == 0 && ((uintptr_t)f.halo_bot & 3) == 0 &&
-                     (f.halo_pitch & 1) == 0;
+    // aligned 4-byte words (a column pair of uint16, the pairs of two lanes of uint8): every byte offset between the
+    // frame's first element and a staged word is a multiple of 4; 32-bit element offsets from the frame's first element
+    const int64_t eb = sizeof(T);
+    auto w4 = [](int64_t bytes) { return (bytes & 3) == 0; };
+    const int wide = w4((int64_t)(uintptr_t)f.in) && w4(f.in_sy * eb) && w4(f.in_sc * eb) && w4(p.fs.in * eb) && w4(f.in_x0 * eb) &&
+                     w4((int64_t)(uintptr_t)f.halo_top) && w4((int64_t)(uintptr_t)f.halo_bot) && w4(f.halo_pitch * eb);
     const int idx32 = f.in_sy > 0 && f.in_sc > 0 && (int64_t)f.in_h * f.in_sy + (int64_t)f.in_c * f.in_sc < (1ll << 31);
-    HB_LAUNCH("ll_level1", (ll_level1_kernel<BETA1, FRAMES>), g, kDWarps * 32, smem, s, f, d1, d2, xbase, ybase, ns, nc, nr, wide, idx32,
+    HB_LAUNCH("ll_level1", (ll_level1_kernel<BETA1, FRAMES, T>), g, kDWarps * 32, smem, s, f, d1, d2, xbase, ybase, ns, nc, nr, wide, idx32,
               p.N, p.fs);
 }
 
-void launch_level12(Plan &p, const LLFrame &f, Span cy1, Span cy2, cudaStream_t s) {
+template<typename T>
+void launch_level12(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2, cudaStream_t s) {
     const bool beta1 = p.f.beta == 1.0f, frames = p.N > 1;
     if (beta1 && frames) launch_level12_kernel<true, true>(p, f, cy1, cy2, s);
     else if (beta1) launch_level12_kernel<true, false>(p, f, cy1, cy2, s);
@@ -274,7 +309,8 @@ void launch_level12(Plan &p, const LLFrame &f, Span cy1, Span cy2, cudaStream_t 
     else launch_level12_kernel<false, false>(p, f, cy1, cy2, s);
 }
 
-void launch_down(Plan &p, int j, cudaStream_t s) {  // produce level j (j >= 1) rows cy
+template<typename T>
+void launch_down(PlanT<T> &p, int j, cudaStream_t s) {  // produce level j (j >= 1) rows cy
     LevelBuf *lb = p.ls.lv;
     if (fast_down(p)) {
         if (j == 1) {
@@ -295,7 +331,7 @@ void launch_down(Plan &p, int j, cudaStream_t s) {  // produce level j (j >= 1) 
         for_frame_groups(p, [&](int n0, int nf) {
             dim3 g = grid_for(lb[1].sx.n(), lb[1].cy.n());
             g.z = nf;
-            HB_LAUNCH("ll_level1_generic", ll_level1_naive_kernel, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), p.fs);
+            HB_LAUNCH("ll_level1_generic", ll_level1_naive_kernel<T>, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), p.fs);
         });
     } else {
         for_frame_groups(p, [&](int n0, int nf) {
@@ -311,7 +347,8 @@ dim3 up_grid(int x_lo, int x_hi, int y_lo, int y_hi, int nf) {  // tiles on even
     return dim3((x_hi - (x_lo & ~1) + kUpTW) / kUpTW, (y_hi - (y_lo & ~1) + kUpTH) / kUpTH, nf);
 }
 
-void launch_up(Plan &p, int j, cudaStream_t s) {  // produce outGPyramid[j] (1 <= j <= J-1) rows coy
+template<typename P>
+void launch_up(P &p, int j, cudaStream_t s) {  // produce outGPyramid[j] (1 <= j <= J-1) rows coy
     LevelBuf *lb = p.ls.lv;
     if (lb[j].coy.n() <= 0) return;
     const bool fast_up = p.f.levels == 8 && !(g_force_naive & 2);
@@ -319,7 +356,7 @@ void launch_up(Plan &p, int j, cudaStream_t s) {  // produce outGPyramid[j] (1 <
         if (fast_up && j < ll::kMaxJ - 1) {
             static const CUtensorMap no_map = {};
             HB_LAUNCH("ll_up2", (nf > 1 ? ll_up2_kernel<false, false, true, false, true> : ll_up2_kernel<false, false, true, false, false>), up_grid(lb[j].ox.lo, lb[j].ox.hi, lb[j].coy.lo, lb[j].coy.hi, nf),
-                      256, up2_smem_bytes(false, false), s, at_frame(p.f, p.fs, n0), at_frame(lb[j], j, p.fs, n0),
+                      256, up2_smem_bytes(false, false), s, scalars_frame(at_frame(p.f, p.fs, n0)), at_frame(lb[j], j, p.fs, n0),
                       at_frame(lb[j + 1], j + 1, p.fs, n0), no_map, j, p.fs);
         } else {
             dim3 g = grid_for(lb[j].ox.n(), lb[j].coy.n());
@@ -331,20 +368,24 @@ void launch_up(Plan &p, int j, cudaStream_t s) {  // produce outGPyramid[j] (1 <
     });
 }
 
-void launch_final(Plan &p, cudaStream_t s) {
+template<typename T>
+void launch_final(PlanT<T> &p, cudaStream_t s) {
     LevelBuf *lb = p.ls.lv;
     if (fast_final(p)) {
-        const LLFrame &f = p.f;
-        // the common layout takes the kernel's ALIGNED path (32-bit addressing, one aligned word per thread and channel)
+        const LLFrameT<T> &f = p.f;
+        // the common layout takes the kernel's ALIGNED path (32-bit addressing, one aligned word of two pixels per thread
+        // and channel: wb bytes, so every pointer and element offset to such a word is a multiple of wb bytes)
+        const int64_t eb = sizeof(T), wb = 2 * eb;
+        auto aw = [&](int64_t bytes) { return bytes % wb == 0; };
         const int64_t in_span = (int64_t)f.in_h * f.in_sy + 3 * f.in_sc, out_span = (int64_t)f.H * f.out_sy + 3 * f.out_sc;
-        const bool aligned = f.C == 3 && f.in_c0 == 0 && f.out_c0 == 0 && f.in_c >= 3 && (f.W & 1) == 0 && (f.out_x0 & 1) == 0 &&
-                             (f.in_x0 & 1) == 0 && ((uintptr_t)f.in & 3) == 0 && ((uintptr_t)f.out & 3) == 0 &&
-                             (f.in_sy & 1) == 0 && (f.in_sc & 1) == 0 && (f.out_sy & 1) == 0 && (f.out_sc & 1) == 0 &&
-                             (p.fs.in & 1) == 0 && (p.fs.out & 1) == 0 && f.in_sy > 0 && f.in_sc > 0 && f.out_sy > 0 &&
+        const bool aligned = f.C == 3 && f.in_c0 == 0 && f.out_c0 == 0 && f.in_c >= 3 && aw(f.W * eb) && aw(f.out_x0 * eb) &&
+                             aw(f.in_x0 * eb) && aw((int64_t)(uintptr_t)f.in) && aw((int64_t)(uintptr_t)f.out) &&
+                             aw(f.in_sy * eb) && aw(f.in_sc * eb) && aw(f.out_sy * eb) && aw(f.out_sc * eb) &&
+                             aw(p.fs.in * eb) && aw(p.fs.out * eb) && f.in_sy > 0 && f.in_sc > 0 && f.out_sy > 0 &&
                              f.out_sc > 0 && in_span < (1ll << 31) && out_span < (1ll << 31) && !(g_force_naive & 16);
         const bool beta1 = f.beta == 1.0f;
         for_frame_groups(p, [&](int n0, int nf) {
-            const LLFrame fg = at_frame(f, p.fs, n0);
+            const LLFrameT<T> fg = at_frame(f, p.fs, n0);
             // frame tile by TMA when the buffer meets TMA's rules (16-byte aligned base and strides); the map describes
             // the input buffer itself (x, y, c), and the group's frames as a fourth dimension when there are several, so a
             // tile reaching past it reads zeros for pixels that are never stored
@@ -352,17 +393,18 @@ void launch_final(Plan &p, cudaStream_t s) {
             bool use_tma = false;
             if (aligned && !(g_force_naive & 64)) {
                 const int rank = nf > 1 ? 4 : 3;
-                const int64_t strides[3] = {f.in_sy * 2, f.in_sc * 2, p.fs.in * 2};
+                const int64_t strides[3] = {f.in_sy * eb, f.in_sc * eb, p.fs.in * eb};
                 // (every tile's first column must also start on a 16-byte boundary: crops at other even offsets take the
                 // load path; so do frame strides that are no 16-byte multiple)
-                if (tma::strides_ok(fg.in, strides, rank - 1) && (((f.out_x0 & ~1) - f.in_x0) & 7) == 0) {
+                if (tma::strides_ok(fg.in, strides, rank - 1) && (((f.out_x0 & ~1) - f.in_x0) * eb) % 16 == 0) {
                     const uint64_t dims[4] = {(uint64_t)f.in_w, (uint64_t)f.in_h, (uint64_t)f.in_c, (uint64_t)nf};
-                    const uint32_t box[4] = {kUpInW, kUpTH, 3, 1};
-                    use_tma = tma::encode(&in_map, CU_TENSOR_MAP_DATA_TYPE_UINT16, rank, (void *)fg.in, dims, strides, box);
+                    const uint32_t box[4] = {(uint32_t)up_in_w<T>(), kUpTH, 3, 1};
+                    use_tma = tma::encode(&in_map, sizeof(T) == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16, rank,
+                                          (void *)fg.in, dims, strides, box);
                 }
             }
             auto launch = [&](auto kern, bool tma_on) {
-                const int smem = up2_smem_bytes(true, tma_on);
+                const int smem = up2_smem_bytes(true, tma_on, (int)sizeof(T));
                 const dim3 g = up_grid(f.out_x0, f.out_x0 + f.W - 1, f.out_y0, f.out_y0 + f.H - 1, nf);
                 (void)resident_slots(kern, 256, smem);  // (sets the > 48 KB shared-memory attribute once per kernel and device)
                 HB_LAUNCH("ll_final2", kern, g, 256, smem, s, fg, at_frame(lb[1], 1, p.fs, n0), at_frame(lb[2], 2, p.fs, n0), in_map, 1,
@@ -370,12 +412,12 @@ void launch_final(Plan &p, cudaStream_t s) {
             };
             auto pick = [&](auto frames) {
                 constexpr bool F = decltype(frames)::value;
-                if (use_tma && beta1) launch(ll_up2_kernel<true, true, true, true, F>, true);
-                else if (use_tma) launch(ll_up2_kernel<true, true, false, true, F>, true);
-                else if (aligned && beta1) launch(ll_up2_kernel<true, true, true, false, F>, false);
-                else if (aligned) launch(ll_up2_kernel<true, true, false, false, F>, false);
-                else if (beta1) launch(ll_up2_kernel<true, false, true, false, F>, false);
-                else launch(ll_up2_kernel<true, false, false, false, F>, false);
+                if (use_tma && beta1) launch(ll_up2_kernel<true, true, true, true, F, T>, true);
+                else if (use_tma) launch(ll_up2_kernel<true, true, false, true, F, T>, true);
+                else if (aligned && beta1) launch(ll_up2_kernel<true, true, true, false, F, T>, false);
+                else if (aligned) launch(ll_up2_kernel<true, true, false, false, F, T>, false);
+                else if (beta1) launch(ll_up2_kernel<true, false, true, false, F, T>, false);
+                else launch(ll_up2_kernel<true, false, false, false, F, T>, false);
             };
             if (nf > 1) pick(std::true_type{});
             else pick(std::false_type{});
@@ -384,13 +426,14 @@ void launch_final(Plan &p, cudaStream_t s) {
         for_frame_groups(p, [&](int n0, int nf) {
             dim3 g = grid_for(p.f.W, p.f.H);
             g.z = nf;
-            HB_LAUNCH("ll_final", ll_final_naive_kernel, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), 1, p.fs);
+            HB_LAUNCH("ll_final", ll_final_naive_kernel<T>, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), 1, p.fs);
         });
     }
 }
 
 // Coarse tail in one cooperative launch: levels j0+1 .. J-1 down and up (see ll_coarse_fused_kernel).
-bool launch_coarse_fused(Plan &p, int j0, cudaStream_t s) {
+template<typename P>
+bool launch_coarse_fused(P &p, int j0, cudaStream_t s) {
     int dev = 0, coop = 0;
     cudaGetDevice(&dev);
     static std::map<int, int> coop_ok;  // per device (guarded by g_slots_mu)
@@ -425,7 +468,8 @@ bool launch_coarse_fused(Plan &p, int j0, cudaStream_t s) {
 
 // Levels from_level+1 .. J-1 down, then J-1 .. from_level+1 up: the part of the sweep that runs on whole levels
 // (everything on one GPU; the replicated coarse levels when row-sharded).  Small levels share one cooperative launch.
-void run_coarse_sweep(Plan &p, int from_level, cudaStream_t s) {
+template<typename P>
+void run_coarse_sweep(P &p, int from_level, cudaStream_t s) {
     int j0 = ll::kMaxJ - 1;
     if (!(g_force_naive & 8)) {
         // (level 1 always has its own launch: it is built from the frame, not from a stored level; on the fast path that
@@ -445,14 +489,15 @@ void run_coarse_sweep(Plan &p, int from_level, cudaStream_t s) {
     for (int j = j0; j > from_level && j >= first_up_level(p); j--) launch_up(p, j, s);
 }
 
-// One GPU, args = {input, output} of 3 dimensions (one frame) or 4 (a batch of frames along dimension 3).
+// One GPU, args = {input, output} of 3 dimensions (one frame) or 4 (a batch of frames along dimension 3), elements T.
+template<typename T>
 int run_local_laplacian(hb::Arg *args, int levels, float alpha, float beta, const char *what) {
     int r;
     bool done;
     if ((r = check_and_query(args, levels, &done)) || done) return r;
     if ((r = hb::acquire(args, 2))) return r;
 
-    Plan p;
+    PlanT<T> p;
     fill_frame(p, args, levels, alpha, beta);
     const int W = p.f.W, H = p.f.H;
     Span outx = {p.f.out_x0, p.f.out_x0 + W - 1}, outy = {p.f.out_y0, p.f.out_y0 + H - 1};
@@ -474,7 +519,7 @@ int run_local_laplacian(hb::Arg *args, int levels, float alpha, float beta, cons
 
 extern "C" int local_laplacian(halide_buffer_t *input, int32_t levels, float alpha, float beta, halide_buffer_t *output) {
     hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[4]}};
-    return run_local_laplacian(args, levels, alpha, beta, "local_laplacian launch");
+    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, "local_laplacian launch");
 }
 HB_EXPORT_FILTER(local_laplacian, kArgs)
 
@@ -482,7 +527,20 @@ HB_EXPORT_FILTER(local_laplacian, kArgs)
 extern "C" int halide_b200_local_laplacian_batch(halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                                  halide_buffer_t *output) {
     hb::Arg args[2] = {{input, kBatchArgs[0]}, {output, kBatchArgs[1]}};
-    return run_local_laplacian(args, levels, alpha, beta, "local_laplacian_batch launch");
+    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, "local_laplacian_batch launch");
+}
+
+// 8-bit entry points (library extensions): out8 = to_u8(local_laplacian(to_u16(in8))) with the reference's element
+// conversions, computed in one pass — the conversions happen inside the kernels that read and write the frame.
+extern "C" int halide_b200_local_laplacian_u8(halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                              halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kU8Args[0]}, {output, kU8Args[1]}};
+    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, "local_laplacian_u8 launch");
+}
+extern "C" int halide_b200_local_laplacian_u8_batch(halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                                    halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kU8BatchArgs[0]}, {output, kU8BatchArgs[1]}};
+    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, "local_laplacian_u8_batch launch");
 }
 // The harness's second AOT variant (apps/local_laplacian/process.cpp:44-48): same implementation.
 HB_EXPORT_AUTO_SCHEDULE(local_laplacian, kArgs)

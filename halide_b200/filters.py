@@ -29,6 +29,21 @@ def local_laplacian_batch(input, levels, alpha, beta, output):
                                                        ctypes.c_float(beta), output.ptr))
 
 
+def local_laplacian_u8(input, levels, alpha, beta, output):
+    """local_laplacian on 3-D (x, y, c) uint8 buffers: output = to_u8(local_laplacian(to_u16(input))) bit for bit, with the
+    reference's element conversions (image_io.convert: to_u16(v) = v * 257, to_u8(w) = ((w + 128) * 255 + 255) >> 16),
+    done inside the kernels: no uint16 copy of either frame is made."""
+    return check(lib.halide_b200_local_laplacian_u8(input.ptr, ctypes.c_int32(levels), ctypes.c_float(alpha),
+                                                    ctypes.c_float(beta), output.ptr))
+
+
+def local_laplacian_u8_batch(input, levels, alpha, beta, output):
+    """local_laplacian_u8 on every frame of 4-D (x, y, c, n) uint8 buffers, e.g. an (N, 3, H, W) uint8 torch tensor (a
+    decoded clip): output frame n = local_laplacian_u8(input frame n), in one launch sequence for the whole batch."""
+    return check(lib.halide_b200_local_laplacian_u8_batch(input.ptr, ctypes.c_int32(levels), ctypes.c_float(alpha),
+                                                          ctypes.c_float(beta), output.ptr))
+
+
 def stencil_chain(input, output):
     """apps/stencil_chain/stencil_chain_generator.cpp: 32 chained 5x5 uint16 stencils."""
     return check(lib.stencil_chain(input.ptr, output.ptr))

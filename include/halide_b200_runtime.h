@@ -295,6 +295,19 @@ int halide_b200_local_laplacian_sharded(struct halide_buffer_t *input, int32_t l
 int halide_b200_local_laplacian_batch(struct halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                       struct halide_buffer_t *output);
 
+/* local_laplacian on 3-D (x, y, c) uint8 buffers: output = to_u8(local_laplacian(to_u16(input), levels, alpha, beta)),
+ * bit for bit, with the element conversions of the reference's image I/O (tools/halide_image_io.h, Internal::convert):
+ * to_u16(v) = v * 257 and to_u8(w) = ((w + 128) * 255 + 255) >> 16 in 32-bit arithmetic.  Both happen inside the kernels
+ * that read and write the frame, so no uint16 copy of either frame exists.  Bounds, repeat_edge, channel crops, error
+ * codes and the bounds query are those of local_laplacian; both buffers must be uint8 (else halide_error_code_bad_type). */
+int halide_b200_local_laplacian_u8(struct halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                   struct halide_buffer_t *output);
+
+/* halide_b200_local_laplacian_u8 on every frame of a 4-D (x, y, c, n) uint8 buffer, with the frame rules of
+ * halide_b200_local_laplacian_batch: output frame n = halide_b200_local_laplacian_u8(input frame n), bit for bit. */
+int halide_b200_local_laplacian_u8_batch(struct halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                         struct halide_buffer_t *output);
+
 /* Host-only probe of the band geometry for tests: with level jr gathered, out[j*8..j*8+7] = {own.lo, own.hi, d.lo, d.hi,
  * u.lo, u.hi, S.lo, S.hi} per pyramid level j = 0..7 (rows owned in the gather partition / Gaussian-side rows computed and
  * held / outGPyramid rows needed / the level's rows on the whole frame), out[64..65] = input rows read. */
