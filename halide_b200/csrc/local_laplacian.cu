@@ -264,8 +264,9 @@ void launch_level12_kernel(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2
     LevelBuf d1 = p.ls.lv[1], d2 = p.ls.lv[2];
     d1.cy = cy1;
     d2.cy = cy2;
-    // one pair table and kDWarps warp stages: one block per SM
-    const size_t smem = kPairLutN * sizeof(float2) + kDWarps * sizeof(DownStage);
+    // one pair table and a stage per strip walker (warp pair or warp): one block per SM
+    constexpr int pairs = kL1Walkers<FRAMES, T>;
+    const size_t smem = kPairLutN * sizeof(float2) + pairs * sizeof(DownStage);
     const int slots = resident_slots(ll_level1_kernel<BETA1, FRAMES, T>, kDWarps * 32, smem);
     // strips of 28 level-1 columns from xbase == xo (mod 4), far enough left that their level-2 columns (xbase/2 + 14k ..)
     // reach level 2's first column; chunks of 8 level-1 rows from an odd ybase, over the rows stored and the taps of
@@ -278,17 +279,23 @@ void launch_level12_kernel(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2
     if (lo > hi) return;
     const int ybase = lo - ((lo & 1) ^ 1);
     const int nc = (hi - ybase) / kDR + 1;
-    // nr chunk ranges per strip: the fewest step-equivalents per warp over the rounds of runs (a lead-in computes 2 of a
-    // chunk's 8 rows: a quarter chunk), over the N * ns strips of the batch
-    const long long nw = (long long)slots * kDWarps, strips = (long long)p.N * ns;
+    // nr chunk ranges per strip: the fewest step-equivalents per walker over the rounds of runs (a lead-in computes 2 of
+    // a chunk's 8 rows: a quarter chunk), over the N * ns strips of the batch.  Warp pairs take, of the counts within 1 %
+    // of the fewest, the most ranges (the shortest runs): counts the cost puts within 1 % of each other ran up to 5 %
+    // apart, the shorter runs faster (16K on an H100, DESIGN §9).
+    const long long np = (long long)slots * pairs, strips = (long long)p.N * ns;
+    std::vector<long long> cost(nc + 1);
     int nr = 1;
-    long long best = -1;
     for (int r = 1; r <= nc; r++) {
-        const long long cost = (strips * r + nw - 1) / nw * (4ll * ((nc + r - 1) / r) + 1);
-        if (best < 0 || cost < best) best = cost, nr = r;
+        cost[r] = (strips * r + np - 1) / np * (4ll * ((nc + r - 1) / r) + 1);
+        if (cost[r] < cost[nr]) nr = r;
+    }
+    if (kL1Pairs<FRAMES, T>) {
+        const long long best = cost[nr];
+        for (nr = nc; cost[nr] * 100 > best * 101;) nr--;
     }
     const long long runs = strips * nr;
-    const int g = (int)std::min<long long>(slots, (runs + kDWarps - 1) / kDWarps);
+    const int g = (int)std::min<long long>(slots, (runs + pairs - 1) / pairs);
     // aligned 4-byte words (a column pair of uint16, the pairs of two lanes of uint8): every byte offset between the
     // frame's first element and a staged word is a multiple of 4; 32-bit element offsets from the frame's first element
     const int64_t eb = sizeof(T);
