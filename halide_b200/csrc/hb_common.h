@@ -83,10 +83,14 @@ constexpr const char *kTarget = "x86-64-linux-cuda-cuda_capability_90-h100_nativ
 
 // One buffer argument: the caller's buffer, its record in the filter's metadata (name, type,
 // dimensions, input or output) and, once acquired, the device address of its element at the mins.
+// interleaved: the buffer holds pixel-interleaved channels (dim[2].stride == 1, dim[0].stride = the pixel pitch, at
+// least the channel extent) instead of the dense-x layout every filter argument has otherwise (set per argument by the
+// entry points that read or write such buffers).
 struct Arg {
     halide_buffer_t *b;
     const halide_filter_argument_t &meta;
     void *dev = nullptr;
+    bool interleaved = false;
 };
 
 // The part of a buffer a call touches: proposed by a bounds query, and required of the caller's
@@ -100,9 +104,11 @@ Region region_of(const halide_buffer_t *b, bool must_cover);  // the buffer's ow
 // null → -12, type → -3, dimensions → -43, buffer by buffer in argument order.
 int check_args(const Arg *a, int n);
 // Bounds-query mode (HalideRuntime.h:1851-1853): every buffer with neither host nor device memory
-// gets need[i] with dense strides (src/AddImageChecks.cpp:386-436,477-496).  True if any did.
+// gets need[i] with dense strides (src/AddImageChecks.cpp:386-436,477-496); interleaved ones get dense interleaved
+// strides (C, W*C, 1[, W*H*C]).  True if any did.
 bool answer_bounds_query(Arg *a, const Region *need, int n);
-// negative extent → -28, |extent*stride| and extent product limits → -5/-6, stride[0] != 1 → -8.
+// negative extent → -28, |extent*stride| and extent product limits → -5/-6, stride[0] != 1 → -8 (interleaved
+// arguments instead: stride[2] != 1, stride[0] < extent[2], stride[1] or stride[3] not positive → -8).
 int check_shapes(const Arg *a, int n);
 // every must_cover region must lie inside its buffer, dimension by dimension → else -4.
 int check_required(const Arg *a, const Region *need, int n);

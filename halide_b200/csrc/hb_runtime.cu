@@ -564,7 +564,10 @@ bool answer_bounds_query(Arg *a, const Region *need, int n) {
         halide_buffer_t *b = a[i].b;
         if (b->host != nullptr || b->device != 0) continue;
         int64_t stride = 1;
-        for (int d = 0; d < b->dimensions; d++) {
+        // (interleaved: the channel dimension is the innermost one, then x, y and the rest)
+        const bool il = a[i].interleaved && b->dimensions >= 3;
+        for (int k = 0; k < b->dimensions; k++) {
+            const int d = il ? (k == 0 ? 2 : (k <= 2 ? k - 1 : k)) : k;
             b->dim[d].min = need[i].min[d];
             b->dim[d].extent = need[i].extent[d];
             b->dim[d].stride = (int32_t)stride;
@@ -599,6 +602,26 @@ int check_shapes(const Arg *a, int n) {
                             "Product of extents for buffer %s is %lld, which exceeds the maximum size of 2147483647",
                             name, (long long)total);
             }
+        }
+        if (a[i].interleaved) {
+            const halide_dimension_t *dm = b->dim;
+            if (b->dimensions < 3 || dm[2].stride != 1) {
+                return fail(halide_error_code_constraint_violated,
+                            "Constraint violated: %s.stride.2 (%d) == 1 (1): an interleaved buffer's channels must be adjacent",
+                            name, b->dimensions < 3 ? 0 : dm[2].stride);
+            }
+            if (dm[0].stride < dm[2].extent) {
+                return fail(halide_error_code_constraint_violated,
+                            "Constraint violated: %s.stride.0 (%d) >= %s.extent.2 (%d): an interleaved buffer's pixel pitch must hold its channels",
+                            name, dm[0].stride, name, dm[2].extent);
+            }
+            for (int d = 1; d < b->dimensions; d += 2) {  // dimensions 1 (y) and 3 (n)
+                if (dm[d].stride <= 0) {
+                    return fail(halide_error_code_constraint_violated, "Constraint violated: %s.stride.%d (%d) > 0 (0) for an interleaved buffer",
+                                name, d, dm[d].stride);
+                }
+            }
+            continue;
         }
         if (b->dimensions > 0 && b->dim[0].stride != 1) {
             return fail(halide_error_code_constraint_violated, "Constraint violated: %s.stride.0 (%d) == 1 (1)",

@@ -54,8 +54,9 @@ struct PlanT {
     LLFrameT<T> f;
     LevelSet ls{};  // (level 0 is never stored: its slot stays zero)
     int N;  // frames (1 but for a batch)
-    FrameStrides fs;  // all zero when N == 1
+    FrameStrides fs;  // all zero when N == 1 (but the pixel pitches)
     float alpha;
+    bool il = false;  // interleaved frames (the kernels' IL instantiations)
 };
 using Plan = PlanT<uint16_t>;
 
@@ -120,6 +121,10 @@ void fill_frame(PlanT<T> &p, const hb::Arg *args, int levels, float alpha, float
     f.out_x0 = output->dim[0].min; f.out_y0 = output->dim[1].min; f.out_c0 = output->dim[2].min;
     f.W = output->dim[0].extent; f.H = output->dim[1].extent; f.C = output->dim[2].extent;
     p.fs = FrameStrides{};
+    // interleaved buffers: channel stride 1 (in_sc / out_sc above), pixel pitch dim[0].stride
+    p.il = args[0].interleaved;
+    p.fs.px_in = p.il ? input->dim[0].stride : 1;
+    p.fs.px_out = p.il ? output->dim[0].stride : 1;
     p.N = 1;
     if (output->dimensions == 4) {
         // output frame n reads input frame n: the output's first frame is (out n min - in n min) input frames past the
@@ -259,7 +264,7 @@ int resident_slots(Kern kern, int threads, size_t smem) {
 
 // Levels 1 and 2 from the frame (K == 8): stores level-1 rows cy1 and level-2 rows cy2, reading the frame through f
 // (the row-sharded path narrows both spans, and hides the halo rows from the launch that runs before they arrive).
-template<bool BETA1, bool FRAMES, typename T>
+template<bool BETA1, bool FRAMES, bool IL, typename T>
 void launch_level12_kernel(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2, cudaStream_t s) {
     LevelBuf d1 = p.ls.lv[1], d2 = p.ls.lv[2];
     d1.cy = cy1;
@@ -267,7 +272,7 @@ void launch_level12_kernel(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2
     // one pair table and a stage per strip walker (warp pair or warp): one block per SM
     constexpr int pairs = kL1Walkers<FRAMES, T>;
     const size_t smem = kPairLutN * sizeof(float2) + pairs * sizeof(DownStage);
-    const int slots = resident_slots(ll_level1_kernel<BETA1, FRAMES, T>, kDWarps * 32, smem);
+    const int slots = resident_slots(ll_level1_kernel<BETA1, FRAMES, T, IL>, kDWarps * 32, smem);
     // strips of 28 level-1 columns from xbase == xo (mod 4), far enough left that their level-2 columns (xbase/2 + 14k ..)
     // reach level 2's first column; chunks of 8 level-1 rows from an odd ybase, over the rows stored and the taps of
     // the level-2 rows stored
@@ -302,18 +307,26 @@ void launch_level12_kernel(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2
     auto w4 = [](int64_t bytes) { return (bytes & 3) == 0; };
     const int wide = w4((int64_t)(uintptr_t)f.in) && w4(f.in_sy * eb) && w4(f.in_sc * eb) && w4(p.fs.in * eb) && w4(f.in_x0 * eb) &&
                      w4((int64_t)(uintptr_t)f.halo_top) && w4((int64_t)(uintptr_t)f.halo_bot) && w4(f.halo_pitch * eb);
-    const int idx32 = f.in_sy > 0 && f.in_sc > 0 && (int64_t)f.in_h * f.in_sy + (int64_t)f.in_c * f.in_sc < (1ll << 31);
-    HB_LAUNCH("ll_level1", (ll_level1_kernel<BETA1, FRAMES, T>), g, kDWarps * 32, smem, s, f, d1, d2, xbase, ybase, ns, nc, nr, wide, idx32,
+    // (an interleaved frame's columns are px_in elements apart: its last sample is up to in_w * px_in further)
+    const int idx32 = f.in_sy > 0 && f.in_sc > 0 &&
+                      (int64_t)f.in_h * f.in_sy + (int64_t)f.in_c * f.in_sc + (IL ? (int64_t)f.in_w * p.fs.px_in : 0) < (1ll << 31);
+    HB_LAUNCH("ll_level1", (ll_level1_kernel<BETA1, FRAMES, T, IL>), g, kDWarps * 32, smem, s, f, d1, d2, xbase, ybase, ns, nc, nr, wide, idx32,
               p.N, p.fs);
+}
+
+template<bool IL, typename T>
+void launch_level12_il(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2, cudaStream_t s) {
+    const bool beta1 = p.f.beta == 1.0f, frames = p.N > 1;
+    if (beta1 && frames) launch_level12_kernel<true, true, IL>(p, f, cy1, cy2, s);
+    else if (beta1) launch_level12_kernel<true, false, IL>(p, f, cy1, cy2, s);
+    else if (frames) launch_level12_kernel<false, true, IL>(p, f, cy1, cy2, s);
+    else launch_level12_kernel<false, false, IL>(p, f, cy1, cy2, s);
 }
 
 template<typename T>
 void launch_level12(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2, cudaStream_t s) {
-    const bool beta1 = p.f.beta == 1.0f, frames = p.N > 1;
-    if (beta1 && frames) launch_level12_kernel<true, true>(p, f, cy1, cy2, s);
-    else if (beta1) launch_level12_kernel<true, false>(p, f, cy1, cy2, s);
-    else if (frames) launch_level12_kernel<false, true>(p, f, cy1, cy2, s);
-    else launch_level12_kernel<false, false>(p, f, cy1, cy2, s);
+    if (p.il) launch_level12_il<true>(p, f, cy1, cy2, s);
+    else launch_level12_il<false>(p, f, cy1, cy2, s);
 }
 
 template<typename T>
@@ -338,7 +351,8 @@ void launch_down(PlanT<T> &p, int j, cudaStream_t s) {  // produce level j (j >=
         for_frame_groups(p, [&](int n0, int nf) {
             dim3 g = grid_for(lb[1].sx.n(), lb[1].cy.n());
             g.z = nf;
-            HB_LAUNCH("ll_level1_generic", ll_level1_naive_kernel<T>, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), p.fs);
+            HB_LAUNCH("ll_level1_generic", (p.il ? ll_level1_naive_kernel<T, true> : ll_level1_naive_kernel<T, false>), g, kBlk, 0, s,
+                      at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), p.fs);
         });
     } else {
         for_frame_groups(p, [&](int n0, int nf) {
@@ -385,11 +399,22 @@ void launch_final(PlanT<T> &p, cudaStream_t s) {
         const int64_t eb = sizeof(T), wb = 2 * eb;
         auto aw = [&](int64_t bytes) { return bytes % wb == 0; };
         const int64_t in_span = (int64_t)f.in_h * f.in_sy + 3 * f.in_sc, out_span = (int64_t)f.H * f.out_sy + 3 * f.out_sc;
-        const bool aligned = f.C == 3 && f.in_c0 == 0 && f.out_c0 == 0 && f.in_c >= 3 && aw(f.W * eb) && aw(f.out_x0 * eb) &&
+        // (interleaved frames always take the general-layout path)
+        const bool aligned = !p.il && f.C == 3 && f.in_c0 == 0 && f.out_c0 == 0 && f.in_c >= 3 && aw(f.W * eb) && aw(f.out_x0 * eb) &&
                              aw(f.in_x0 * eb) && aw((int64_t)(uintptr_t)f.in) && aw((int64_t)(uintptr_t)f.out) &&
                              aw(f.in_sy * eb) && aw(f.in_sc * eb) && aw(f.out_sy * eb) && aw(f.out_sc * eb) &&
                              aw(p.fs.in * eb) && aw(p.fs.out * eb) && f.in_sy > 0 && f.in_sc > 0 && f.out_sy > 0 &&
                              f.out_sc > 0 && in_span < (1ll << 31) && out_span < (1ll << 31) && !(g_force_naive & 16);
+        // Interleaved RGB / RGBA frames of channels [0, 3) (RGB -> RGB, RGBA -> RGB, RGBA -> RGBA's channels [0, 3)) take
+        // the kernel's aligned form with fixed pitches: the frame tile by TMA (an RGBA input must describe its fourth
+        // channel: the tile reads whole pixels), a pixel pair's output samples stored together as wb-byte words (so the
+        // output's base, row and frame strides in bytes are multiples of wb, and both its columns and the input's start
+        // even).  Everything else interleaved takes the general-layout path.
+        const int pin = p.fs.px_in, pout = p.fs.px_out;
+        const bool il_fast = p.il && f.C == 3 && f.in_c0 == 0 && f.out_c0 == 0 && f.in_c == pin &&
+                             ((pin == 3 && pout == 3) || (pin == 4 && (pout == 3 || pout == 4))) && f.W % 2 == 0 &&
+                             f.out_x0 % 2 == 0 && f.in_x0 % 2 == 0 && aw((int64_t)(uintptr_t)f.out) && aw(f.out_sy * eb) &&
+                             aw(p.fs.out * eb) && f.out_sy > 0 && !(g_force_naive & 16) && !(g_force_naive & 64);
         const bool beta1 = f.beta == 1.0f;
         for_frame_groups(p, [&](int n0, int nf) {
             const LLFrameT<T> fg = at_frame(f, p.fs, n0);
@@ -410,8 +435,20 @@ void launch_final(PlanT<T> &p, cudaStream_t s) {
                                           (void *)fg.in, dims, strides, box);
                 }
             }
-            auto launch = [&](auto kern, bool tma_on) {
-                const int smem = up2_smem_bytes(true, tma_on, (int)sizeof(T));
+            if (il_fast) {
+                const int rank = nf > 1 ? 3 : 2;
+                const int64_t strides[2] = {f.in_sy * eb, p.fs.in * eb};
+                if (tma::strides_ok(fg.in, strides, rank - 1) && (((f.out_x0 & ~1) - f.in_x0) * eb) % 16 == 0) {
+                    // RGB: x runs over samples (a box of 3 * up_in_w samples); RGBA: over pixels, one 4-sample element each
+                    const uint64_t dims[3] = {(uint64_t)(pin == 3 ? 3 * f.in_w : f.in_w), (uint64_t)f.in_h, (uint64_t)nf};
+                    const uint32_t box[3] = {(uint32_t)(pin == 3 ? 3 * up_in_w<T>() : up_in_w<T>()), kUpTH, 1};
+                    const CUtensorMapDataType dt = pin == 3 ? (sizeof(T) == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16)
+                                                            : (sizeof(T) == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_UINT64);
+                    use_tma = tma::encode(&in_map, dt, rank, (void *)fg.in, dims, strides, box);
+                }
+            }
+            auto launch = [&](auto kern, bool tma_on, int samples = 3) {
+                const int smem = up2_smem_bytes(true, tma_on, (int)sizeof(T), samples);
                 const dim3 g = up_grid(f.out_x0, f.out_x0 + f.W - 1, f.out_y0, f.out_y0 + f.H - 1, nf);
                 (void)resident_slots(kern, 256, smem);  // (sets the > 48 KB shared-memory attribute once per kernel and device)
                 HB_LAUNCH("ll_final2", kern, g, 256, smem, s, fg, at_frame(lb[1], 1, p.fs, n0), at_frame(lb[2], 2, p.fs, n0), in_map, 1,
@@ -419,10 +456,19 @@ void launch_final(PlanT<T> &p, cudaStream_t s) {
             };
             auto pick = [&](auto frames) {
                 constexpr bool F = decltype(frames)::value;
-                if (use_tma && beta1) launch(ll_up2_kernel<true, true, true, true, F, T>, true);
+                if (p.il && use_tma) {
+                    if (pin == 3 && beta1) launch(ll_up2_kernel<true, true, true, true, F, T, 3, 3>, true, 3);
+                    else if (pin == 3) launch(ll_up2_kernel<true, true, false, true, F, T, 3, 3>, true, 3);
+                    else if (pout == 3 && beta1) launch(ll_up2_kernel<true, true, true, true, F, T, 4, 3>, true, 4);
+                    else if (pout == 3) launch(ll_up2_kernel<true, true, false, true, F, T, 4, 3>, true, 4);
+                    else if (beta1) launch(ll_up2_kernel<true, true, true, true, F, T, 4, 4>, true, 4);
+                    else launch(ll_up2_kernel<true, true, false, true, F, T, 4, 4>, true, 4);
+                } else if (use_tma && beta1) launch(ll_up2_kernel<true, true, true, true, F, T>, true);
                 else if (use_tma) launch(ll_up2_kernel<true, true, false, true, F, T>, true);
                 else if (aligned && beta1) launch(ll_up2_kernel<true, true, true, false, F, T>, false);
                 else if (aligned) launch(ll_up2_kernel<true, true, false, false, F, T>, false);
+                else if (p.il && beta1) launch(ll_up2_kernel<true, false, true, false, F, T, 0, 0>, false);
+                else if (p.il) launch(ll_up2_kernel<true, false, false, false, F, T, 0, 0>, false);
                 else if (beta1) launch(ll_up2_kernel<true, false, true, false, F, T>, false);
                 else launch(ll_up2_kernel<true, false, false, false, F, T>, false);
             };
@@ -433,7 +479,8 @@ void launch_final(PlanT<T> &p, cudaStream_t s) {
         for_frame_groups(p, [&](int n0, int nf) {
             dim3 g = grid_for(p.f.W, p.f.H);
             g.z = nf;
-            HB_LAUNCH("ll_final", ll_final_naive_kernel<T>, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), 1, p.fs);
+            HB_LAUNCH("ll_final", (p.il ? ll_final_naive_kernel<T, true> : ll_final_naive_kernel<T, false>), g, kBlk, 0, s, at_frame(p.f, p.fs, n0),
+                      at_frame(lb[1], 1, p.fs, n0), 1, p.fs);
         });
     }
 }
@@ -548,6 +595,30 @@ extern "C" int halide_b200_local_laplacian_u8_batch(halide_buffer_t *input, int3
                                                     halide_buffer_t *output) {
     hb::Arg args[2] = {{input, kU8BatchArgs[0]}, {output, kU8BatchArgs[1]}};
     return run_local_laplacian<uint8_t>(args, levels, alpha, beta, "local_laplacian_u8_batch launch");
+}
+
+// Interleaved entry points (library extensions): the four above on pixel-interleaved buffers (RGBRGB..., RGBA...:
+// dim[2].stride == 1, dim[0].stride = the pixel pitch, at least the channel extent), bit for bit what they give on planar
+// copies of the same buffers.  The argument records are the planar ones; only the layout rule checked differs.
+extern "C" int halide_b200_local_laplacian_interleaved(halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                                       halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kArgs[0], nullptr, true}, {output, kArgs[4], nullptr, true}};
+    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, "local_laplacian_interleaved launch");
+}
+extern "C" int halide_b200_local_laplacian_interleaved_batch(halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                                             halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kBatchArgs[0], nullptr, true}, {output, kBatchArgs[1], nullptr, true}};
+    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, "local_laplacian_interleaved_batch launch");
+}
+extern "C" int halide_b200_local_laplacian_u8_interleaved(halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                                          halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kU8Args[0], nullptr, true}, {output, kU8Args[1], nullptr, true}};
+    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, "local_laplacian_u8_interleaved launch");
+}
+extern "C" int halide_b200_local_laplacian_u8_interleaved_batch(halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                                                halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kU8BatchArgs[0], nullptr, true}, {output, kU8BatchArgs[1], nullptr, true}};
+    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, "local_laplacian_u8_interleaved_batch launch");
 }
 // The harness's second AOT variant (apps/local_laplacian/process.cpp:44-48): same implementation.
 HB_EXPORT_AUTO_SCHEDULE(local_laplacian, kArgs)

@@ -44,6 +44,47 @@ def local_laplacian_u8_batch(input, levels, alpha, beta, output):
                                                           ctypes.c_float(beta), output.ptr))
 
 
+_INTERLEAVED_LAYOUT = """
+    Both buffers are pixel-interleaved (RGBRGB..., RGBA...): ``dim[2].stride == 1`` and ``dim[0].stride`` is the pixel
+    pitch, at least the channel extent; ``dim[1].stride`` (and ``dim[3].stride``) positive.  Anything else, a planar
+    buffer included, is refused with -8.  The result is, bit for bit, what the planar entry point gives on planar copies
+    of the same buffers.  An output whose pitch exceeds its channel extent (channels [0, 3) of an RGBA frame) leaves the
+    samples it does not cover untouched.  The common sources:
+
+    - a torch tensor in ``torch.channels_last`` memory format: ``HalideBuffer.from_torch(t)`` already describes it as
+      ``(x: C, y: W*C, c: 1, n: H*W*C)``;
+    - a numpy ``(H, W, C)`` array (PIL, OpenCV): ``HalideBuffer.from_numpy(arr.transpose(2, 0, 1))``.
+    """
+
+
+def local_laplacian_interleaved(input, levels, alpha, beta, output):
+    return check(lib.halide_b200_local_laplacian_interleaved(input.ptr, ctypes.c_int32(levels), ctypes.c_float(alpha),
+                                                             ctypes.c_float(beta), output.ptr))
+
+
+def local_laplacian_interleaved_batch(input, levels, alpha, beta, output):
+    return check(lib.halide_b200_local_laplacian_interleaved_batch(input.ptr, ctypes.c_int32(levels), ctypes.c_float(alpha),
+                                                                   ctypes.c_float(beta), output.ptr))
+
+
+def local_laplacian_u8_interleaved(input, levels, alpha, beta, output):
+    return check(lib.halide_b200_local_laplacian_u8_interleaved(input.ptr, ctypes.c_int32(levels), ctypes.c_float(alpha),
+                                                                ctypes.c_float(beta), output.ptr))
+
+
+def local_laplacian_u8_interleaved_batch(input, levels, alpha, beta, output):
+    return check(lib.halide_b200_local_laplacian_u8_interleaved_batch(input.ptr, ctypes.c_int32(levels), ctypes.c_float(alpha),
+                                                                      ctypes.c_float(beta), output.ptr))
+
+
+local_laplacian_interleaved.__doc__ = "local_laplacian on 3-D (x, y, c) uint16 interleaved buffers.\n" + _INTERLEAVED_LAYOUT
+local_laplacian_interleaved_batch.__doc__ = ("local_laplacian_batch on 4-D (x, y, c, n) uint16 interleaved buffers, e.g. an "
+                                             "(N, 3, H, W) channels_last tensor.\n" + _INTERLEAVED_LAYOUT)
+local_laplacian_u8_interleaved.__doc__ = "local_laplacian_u8 on 3-D (x, y, c) uint8 interleaved buffers.\n" + _INTERLEAVED_LAYOUT
+local_laplacian_u8_interleaved_batch.__doc__ = ("local_laplacian_u8_batch on 4-D (x, y, c, n) uint8 interleaved buffers, e.g. a "
+                                                "decoded (N, 3, H, W) channels_last clip.\n" + _INTERLEAVED_LAYOUT)
+
+
 def stencil_chain(input, output):
     """apps/stencil_chain/stencil_chain_generator.cpp: 32 chained 5x5 uint16 stencils."""
     return check(lib.stencil_chain(input.ptr, output.ptr))

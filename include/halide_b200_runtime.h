@@ -308,6 +308,21 @@ int halide_b200_local_laplacian_u8(struct halide_buffer_t *input, int32_t levels
 int halide_b200_local_laplacian_u8_batch(struct halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                          struct halide_buffer_t *output);
 
+/* The four local_laplacian entry points above (uint16 / uint8, one frame / batch) on pixel-interleaved buffers (RGBRGB...,
+ * RGBA...): every buffer must have dim[2].stride == 1, dim[0].stride (the pixel pitch) >= dim[2].extent, and positive
+ * dim[1].stride (and dim[3].stride), else halide_error_code_constraint_violated — a planar buffer included.  The result
+ * is, bit for bit, what the matching planar entry point gives on planar copies of the same buffers; output samples the
+ * buffer's channels do not cover (an RGBA frame's alpha under an output of channels [0, 3)) are left untouched.  A
+ * bounds query proposes dense interleaved strides (C, W*C, 1[, W*H*C]). */
+int halide_b200_local_laplacian_interleaved(struct halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                            struct halide_buffer_t *output);
+int halide_b200_local_laplacian_interleaved_batch(struct halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                                  struct halide_buffer_t *output);
+int halide_b200_local_laplacian_u8_interleaved(struct halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                               struct halide_buffer_t *output);
+int halide_b200_local_laplacian_u8_interleaved_batch(struct halide_buffer_t *input, int32_t levels, float alpha, float beta,
+                                                     struct halide_buffer_t *output);
+
 /* Host-only probe of the band geometry for tests: with level jr gathered, out[j*8..j*8+7] = {own.lo, own.hi, d.lo, d.hi,
  * u.lo, u.hi, S.lo, S.hi} per pyramid level j = 0..7 (rows owned in the gather partition / Gaussian-side rows computed and
  * held / outGPyramid rows needed / the level's rows on the whole frame), out[64..65] = input rows read. */

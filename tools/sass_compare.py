@@ -1,0 +1,62 @@
+"""Compare the SASS of every kernel in one object file against another, instruction by instruction (no GPU needed).
+
+    python tools/sass_compare.py OLD.o NEW.o
+
+For example, to check that a change leaves the planar local_laplacian kernels alone: build the parent commit's
+halide_b200/csrc/local_laplacian.o in a scratch checkout, build this tree's, and compare the two.
+
+Kernels are matched by demangled name.  A template parameter that a change appends with a default value changes the
+mangled name of every existing instantiation without changing its code, so the new object's names are also tried with
+such trailing defaults removed: the interleaved-layout parameters `bool IL = false` (ll_level1_kernel, the generic
+kernels) and `int PI = 1, int PO = 1` (ll_up2_kernel).  Instruction addresses are dropped before comparing; opcodes,
+operands and encodings must match.  Prints each old kernel that is missing or differs, then a count; exits 1 if any.
+"""
+import re
+import subprocess
+import sys
+
+CUOBJDUMP = "/usr/local/cuda/bin/cuobjdump"
+# trailing template arguments that stand for the defaults of appended parameters
+DEFAULT_TAILS = [", 1, 1>(", ", false>("]
+
+
+def kernels(obj):
+    out = subprocess.run([CUOBJDUMP, "-sass", obj], capture_output=True, text=True, check=True).stdout
+    res, name, body = {}, None, []
+    for line in out.splitlines():
+        m = re.match(r"\s*Function : (\S+)", line)
+        if m:
+            if name:
+                res[name] = body
+            name, body = m.group(1), []
+        elif name and "/*" in line:
+            body.append(re.sub(r"/\*[0-9a-f]{4,}\*/", "", line).strip())
+    if name:
+        res[name] = body
+    names = list(res)
+    demangled = subprocess.run(["c++filt"], input="\n".join(names), capture_output=True, text=True, check=True).stdout.split("\n")
+    return {d: res[m] for m, d in zip(names, demangled)}
+
+
+def main():
+    if len(sys.argv) != 3:
+        sys.exit(__doc__)
+    old, new = kernels(sys.argv[1]), kernels(sys.argv[2])
+    by_name = {}
+    for k, v in new.items():
+        by_name.setdefault(k, []).append(v)
+        for tail in DEFAULT_TAILS:
+            if tail in k:
+                by_name.setdefault(k.replace(tail, ">("), []).append(v)
+    bad = 0
+    for k, v in old.items():
+        cands = by_name.get(k, [])
+        if not any(c == v for c in cands):
+            print(("DIFFERS " if cands else "MISSING ") + k)
+            bad += 1
+    print(f"{len(old) - bad} of {len(old)} kernels of {sys.argv[1]} have identical SASS in {sys.argv[2]} ({len(new)} kernels there)")
+    sys.exit(1 if bad else 0)
+
+
+if __name__ == "__main__":
+    main()
