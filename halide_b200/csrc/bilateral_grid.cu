@@ -1,4 +1,5 @@
-// bilateral_grid.cu — bilateral_grid(input, r_sigma, output) for sm_90a (s_sigma = 8).
+// bilateral_grid.cu — bilateral_grid(input, r_sigma, output) for sm_90a (s_sigma = 8), and
+// halide_b200_bilateral_grid_s_sigma for any cell size (its kernels follow bg_slice below).
 //
 // Reference algorithm: apps/bilateral_grid/bilateral_grid_generator.cpp:17-67
 //   histogram(x,y,zi,c) += mux(c,{val,1}) over the 8x8 pixels of cell (x,y) (offset -4), zi = int(val/r_sigma + 0.5)
@@ -18,6 +19,8 @@
 //                   4 pixels per thread (float4 in / float4 out), 8 shared 8-byte corner loads per pixel.
 // Grid layout in HBM: [cell_y][cell_x][z][2] f32 — the (z, z+1) x (value, weight) quad a pixel
 // needs at one corner is 16 contiguous bytes.
+#include <algorithm>
+
 #include "hb_common.h"
 #include "hl_math.cuh"
 
@@ -209,6 +212,241 @@ __global__ void __launch_bounds__(256) bg_slice_kernel(BGParams p) {
     }
 }
 
+// ==== any cell size: halide_b200_bilateral_grid_s_sigma ==============================================================
+// bg_blur_xy only sees the grid and runs unchanged; the histogram and slice kernels below take S at run time.
+
+// floor(n / S) = (n * mag) >> kMagShift with mag = ceil(2^kMagShift / S), exact for 0 <= n and n * S < 2^kMagShift:
+// n * mag / 2^k = n / S + n * e / (S * 2^k) with 0 <= e < S, and that error stays below 1 / S (the least distance from
+// n / S up to the next integer) when n * e < 2^k.  The slice applies it to offsets n < S + 1024 <= 1152 (its tallest
+// tile is 4 passes of 256 rows, its widest 128 columns) and the histogram to column offsets n < kHistCols = 4096, with
+// S <= 128: n * S <= 2^19, and n * mag < 4096 * 2^20 fits in 32 bits.
+constexpr int kMagShift = 20;
+
+struct BGSParams {
+    int S;          // cell size in pixels, 1..128
+    float inv_s;    // fold(1 / S): the reciprocal in double rounded to float (hl::recip_const of the oracle)
+    uint32_t mag;   // ceil(2^kMagShift / S)
+    int cpb, cslots;  // histogram: cells per block, cell slots (nb threads each; a slot takes every cslots-th cell)
+    int rows_chunk;   // histogram: rows staged at a time
+    int cell_stride;  // histogram: float2 per staged cell (odd)
+    int tx, th;     // slice tile: tx threads (4 px each) across, th pixel rows
+    int ncx, ncy;   // slice tile: staged cells per row, staged cell rows
+    int plane;      // slice tile: float2 entries per staged plane (odd)
+};
+
+__device__ __forceinline__ int floor_div_dev(int a, int b) {  // b > 0; per block, never per pixel
+    const int q = a / b;
+    return (a % b != 0 && a < 0) ? q - 1 : q;
+}
+
+// ---- histogram + blurz for any S ---------------------------------------------------------------------------------
+// Bin b of a cell is the sequential float sum, in the generator's order (rows, then columns: the RDom's r.x innermost),
+// of the cell's pixels that fall into b; pixels of other bins never touch it.  So a thread per (cell, bin) that walks the
+// cell's pixels in that order and adds those of its bin forms exactly the generator's sum, and a cell's S x S pixels are
+// shared out over nb threads.  (The weight channel adds 1.0f per pixel: exact integers, in any order.)
+// Block = 256 threads over cpb = cslots * k horizontally adjacent cells of one cell row: thread t < cslots * nb owns bin
+// t % nb of cells t / nb + j * cslots.  Rows are staged rows_chunk at a time, all cpb * S columns of the block read with
+// coalesced loads, each pixel as (clamped value, bin) in one float2, cell-major with an odd cell stride: lanes of one cell
+// read one address, lanes of adjacent cells different banks.  Running sums live in shared memory as [cell][bin], each
+// entry owned by one thread.  blurz then runs over (cell, z) items, so consecutive threads store consecutive float2 of the
+// grid (the block's cells are contiguous there).  (The minimum-blocks hint: without it ptxas held this kernel to 32
+// registers and spilled.)
+__global__ void __launch_bounds__(256, 1) bg_hist_blurz_s_kernel(BGParams p, BGSParams q) {
+    extern __shared__ float2 s_hist[];  // [cpb][nb] running sums, then [cpb][cell_stride] staged pixels
+    const int tid = threadIdx.x, S = q.S, nb = p.zmax + 1, cpb = q.cpb;
+    float2 *s_pix = s_hist + cpb * nb;
+    for (int i = tid; i < cpb * nb; i += 256) s_hist[i] = make_float2(0.f, 0.f);
+    const int cell_row = blockIdx.x, c0 = blockIdx.y * cpb;
+    const int ncell = min(cpb, p.gw - c0);  // stored cells of this block
+    const int gy = p.gy0 + cell_row;
+    const int xb = (p.gx0 + c0) * S - S / 2;  // absolute x of the block's first pixel column
+    const int xlo = p.in_x0, xhi = p.in_x0 + p.in_w - 1;
+    const int cols = ncell * S, cs = q.cell_stride;
+    const int b = tid % nb, slot = tid / nb;
+    for (int r0 = 0; r0 < S; r0 += q.rows_chunk) {
+        const int nr = min(q.rows_chunk, S - r0);
+        __syncthreads();  // the previous chunk is consumed (first chunk: the sums are cleared)
+        for (int r = 0; r < nr; r++) {
+            const int y = hl::clampi(gy * S + r0 + r - S / 2, p.in_y0, p.in_y0 + p.in_h - 1) - p.in_y0;
+            const float *row = p.in + (int64_t)y * p.in_sy;
+            for (int c = tid; c < cols; c += 256) {
+                const float val = hl::clampf(__ldg(row + (hl::clampi(xb + c, xlo, xhi) - xlo)), 0.0f, 1.0f);
+                int zi = (int)__fadd_rn(__fmul_rn(val, p.inv_r), 0.5f);
+                zi = min(zi, p.zmax);
+                const int cell = (int)(((uint32_t)c * q.mag) >> kMagShift);
+                s_pix[cell * cs + r * S + (c - cell * S)] = make_float2(val, __int_as_float(zi));
+            }
+        }
+        __syncthreads();
+        if (slot < q.cslots) {
+            for (int cell = slot; cell < ncell; cell += q.cslots) {
+                const float2 *px = s_pix + cell * cs;
+                float2 acc = s_hist[cell * nb + b];
+                for (int i = 0; i < nr * S; i++) {
+                    const float2 e = px[i];
+                    if (__float_as_int(e.y) == b) {
+                        acc.x += e.x;
+                        acc.y += 1.0f;
+                    }
+                }
+                s_hist[cell * nb + b] = acc;
+            }
+        }
+    }
+    __syncthreads();
+    float2 *g = reinterpret_cast<float2 *>(p.grid_a) + ((size_t)cell_row * p.gw + c0) * p.nz;
+    for (int it = tid; it < ncell * p.nz; it += 256) {
+        const int cell = it / p.nz, z = it - cell * p.nz;
+        const float2 *hc = s_hist + cell * nb;
+        float2 t[5];  // h(z-2) .. h(z+2), zero outside the bins
+#pragma unroll
+        for (int d = 0; d < 5; d++) {
+            const int zz = z - 2 + d;
+            t[d] = (zz < 0 || zz > p.zmax) ? make_float2(0.f, 0.f) : hc[zz];
+        }
+        const float2 hm2 = t[0], hm1 = t[1], h0 = t[2], h1 = t[3], h2 = t[4];
+        // blurz = h(z-2) + 4 h(z-1) + 6 h(z) + 4 h(z+1) + h(z+2) (generator :33-37)
+        g[it] = make_float2((((hm2.x + hm1.x * 4.0f) + h0.x * 6.0f) + h1.x * 4.0f) + h2.x,
+                            (((hm2.y + hm1.y * 4.0f) + h0.y * 6.0f) + h1.y * 4.0f) + h2.y);
+    }
+}
+
+// Histogram block shape for cell size S, nb bins and a grid of gw x gh cells: as many cell slots as 256 threads hold
+// (at most 4096 / S columns' worth), k cells per slot so a block reads at least 256 columns, running sums within 64 KB,
+// and fewer slots when the frame would not give two blocks per SM; staged rows fill up to 4096 pixels.
+constexpr int kHistCols = 4096;
+
+void choose_hist_block(BGSParams &q, int nb, int gw, int gh) {
+    const int S = q.S;
+    int cslots = std::max(1, std::min(256 / nb, kHistCols / S));
+    while (cslots > 1 && (int64_t)gh * ((gw + cslots - 1) / cslots) < 2 * 132) cslots = (cslots + 1) / 2;
+    int k = std::max(1, (256 + cslots * S - 1) / (cslots * S));
+    while (k > 1 && (cslots * k * S > kHistCols || (size_t)cslots * k * nb * sizeof(float2) > 64 * 1024)) k--;
+    q.cslots = cslots;
+    q.cpb = cslots * k;
+    q.rows_chunk = std::max(1, std::min(S, kHistCols / (q.cpb * S)));
+    q.cell_stride = (q.rows_chunk * S) | 1;
+}
+
+size_t hist_s_bytes(const BGSParams &q, int nb) {
+    return ((size_t)q.cpb * nb + (size_t)q.cpb * q.cell_stride) * sizeof(float2);
+}
+
+// ---- trilinear slice + normalise for any S -----------------------------------------------------------------------
+// One block = 256 threads over a tile of 4 * tx x th pixels; the ncx x ncy cells (x nz planes x 2 channels) its pixels
+// interpolate between are staged once in shared memory as [z][cell row][cell column] float2.  Thread (c, r) owns the 4
+// pixels at tile column 4c and rows r, r + 256 / tx, ...: float4 in / float4 out where aligned.  Cell index and
+// fraction come from the offset within the tile (floor division by S via a magic multiplier, see kMagShift), never from
+// a per-pixel division.  Bank conflicts: lanes whose corners fall in one cell read one address when their planes agree
+// (a broadcast) and, with an odd plane stride, different banks when the planes differ by less than 16; lanes in
+// different cells can still collide when the data puts them on different planes.
+__global__ void __launch_bounds__(256) bg_slice_s_kernel(BGParams p, BGSParams q) {
+    extern __shared__ float2 s_cells[];  // [nz][plane], plane >= ncy * ncx
+    const int tid = threadIdx.x, S = q.S;
+    const int X0 = (p.out_x0 & ~3) + blockIdx.y * (4 * q.tx), Y0 = p.out_y0 + blockIdx.x * q.th;
+    const int cxl = floor_div_dev(X0, S), cyl = floor_div_dev(Y0, S);  // first cell of the tile (absolute)
+    const int rx0 = X0 - cxl * S, ry0 = Y0 - cyl * S;                   // tile origin within that cell, [0, S)
+    {
+        const float2 *g = reinterpret_cast<const float2 *>(p.grid_b);
+        const int ncells = q.ncx * q.ncy;
+        // plane fastest: a cell's planes are contiguous in HBM, and an odd plane stride spreads them over the banks
+        for (int it = tid; it < ncells * p.nz; it += 256) {
+            const int cell = it / p.nz, z = it - cell * p.nz;
+            const int cr = cell / q.ncx, cc = cell - cr * q.ncx;
+            const int cx = min(max(cxl + cc - p.gx0, 0), p.gw - 1), cy = min(max(cyl + cr - p.gy0, 0), p.gh - 1);
+            s_cells[z * q.plane + cell] = __ldg(g + ((size_t)cy * p.gw + cx) * p.nz + z);
+        }
+    }
+    __syncthreads();
+    const int c = tid % q.tx, rows_pass = 256 / q.tx;
+    const int x = X0 + 4 * c;
+    if (x + 3 < p.out_x0 || x >= p.out_x0 + p.W) return;
+    int xi[4];
+    float xf[4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const uint32_t n = (uint32_t)(rx0 + 4 * c + i);
+        xi[i] = (int)((n * q.mag) >> kMagShift);  // cell column within the tile
+        xf[i] = __fmul_rn((float)((int)n - xi[i] * S), q.inv_s);
+    }
+    for (int r = tid / q.tx; r < q.th; r += rows_pass) {
+        const int y = Y0 + r;
+        if (y >= p.out_y0 + p.H) break;
+        const uint32_t n = (uint32_t)(ry0 + r);
+        const int yi = (int)((n * q.mag) >> kMagShift);
+        const float yf = __fmul_rn((float)((int)n - yi * S), q.inv_s);
+        const float2 *crow = s_cells + yi * q.ncx;  // cell row yi of plane 0
+        const float *ip = p.in + (int64_t)(y - p.in_y0) * p.in_sy + (x - p.in_x0);
+        float *op = p.out + (int64_t)(y - p.out_y0) * p.out_sy + (x - p.out_x0);
+        auto px = [&](float raw, int i) -> float {
+            const float val = hl::clampf(raw, 0.0f, 1.0f);
+            const float zv = __fmul_rn(val, p.inv_r);
+            int zi = (int)zv;
+            const float zf = __fsub_rn(zv, (float)zi);
+            zi = min(zi, p.nz - 2);
+            const float2 *e = crow + zi * q.plane + xi[i];
+            const int P = q.plane, R = q.ncx;
+            const float2 a0 = e[0], b0 = e[1], d0 = e[R], e0 = e[R + 1];
+            const float2 a1 = e[P], b1 = e[P + 1], d1 = e[P + R], e1 = e[P + R + 1];
+            // lerp nest x -> y -> z exactly as generator :59-64
+            const float v0 = hl::lerpf(hl::lerpf(hl::lerpf(a0.x, b0.x, xf[i]), hl::lerpf(d0.x, e0.x, xf[i]), yf),
+                                       hl::lerpf(hl::lerpf(a1.x, b1.x, xf[i]), hl::lerpf(d1.x, e1.x, xf[i]), yf), zf);
+            const float v1 = hl::lerpf(hl::lerpf(hl::lerpf(a0.y, b0.y, xf[i]), hl::lerpf(d0.y, e0.y, xf[i]), yf),
+                                       hl::lerpf(hl::lerpf(a1.y, b1.y, xf[i]), hl::lerpf(d1.y, e1.y, xf[i]), yf), zf);
+            return __fdiv_rn(v0, v1);
+        };
+        const bool full = x >= p.out_x0 && x + 3 < p.out_x0 + p.W;
+        if (full && ((reinterpret_cast<uintptr_t>(ip) | reinterpret_cast<uintptr_t>(op)) & 15) == 0) {
+            const float4 v = __ldg(reinterpret_cast<const float4 *>(ip));
+            float4 o;
+            o.x = px(v.x, 0);
+            o.y = px(v.y, 1);
+            o.z = px(v.z, 2);
+            o.w = px(v.w, 3);
+            *reinterpret_cast<float4 *>(op) = o;
+        } else {
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                if (x + i >= p.out_x0 && x + i < p.out_x0 + p.W) op[i] = px(__ldg(ip + i), i);
+            }
+        }
+    }
+}
+
+// Slice tile for cell size S and nz planes: the widest, tallest tile (up to four row passes) whose staged cells fit
+// kSliceBudget bytes, so that two blocks share an SM; failing that, the single-pass tile with the most pixels (busy
+// threads) that fits the opt-in maximum (S = 1 with 200 bins).  A tile of 4 x 1 pixels (5 x 2 cells) always fits.
+constexpr int kSliceBudget = 112 * 1024, kSliceMaxSmem = 227 * 1024;
+
+size_t slice_s_bytes(const BGSParams &q, int nz) {
+    return (size_t)q.plane * nz * sizeof(float2);
+}
+
+void choose_slice_tile(BGSParams &q, int nz) {
+    auto set = [&](int tx, int th) {
+        q.tx = tx; q.th = th;
+        q.ncx = (4 * tx - 1 + q.S - 1) / q.S + 2;  // floor((X0 + 4tx - 1) / S) - floor(X0 / S) + 2 at most
+        q.ncy = (th - 1 + q.S - 1) / q.S + 2;
+        q.plane = (q.ncx * q.ncy) | 1;
+        return slice_s_bytes(q, nz);
+    };
+    for (int passes = 4; passes >= 1; passes >>= 1) {
+        for (int tx = 32; tx >= 1; tx >>= 1) {
+            if (set(tx, passes * (256 / tx)) <= (size_t)kSliceBudget) return;
+        }
+    }
+    int best_tx = 1, best_th = 1;  // else the single-pass tile covering the most pixels within the opt-in maximum
+    for (int tx = 32; tx >= 1; tx >>= 1) {
+        for (int th = 256 / tx; th >= 1; th--) {
+            if (set(tx, th) <= (size_t)kSliceMaxSmem) {
+                if (tx * th > best_tx * best_th) best_tx = tx, best_th = th;
+                break;
+            }
+        }
+    }
+    set(best_tx, best_th);
+}
+
 int64_t est_i[2][2] = {{0, 1536}, {0, 2560}};
 const int64_t *const est_ptrs[4] = {&est_i[0][0], &est_i[0][1], &est_i[1][0], &est_i[1][1]};
 const halide_scalar_value_t sv_rsigma = hb::scalar_f32(0.1f);
@@ -294,3 +532,90 @@ extern "C" int bilateral_grid(halide_buffer_t *input, float r_sigma, halide_buff
 }
 HB_EXPORT_FILTER(bilateral_grid, kArgs)
 HB_EXPORT_AUTO_SCHEDULE(bilateral_grid, kArgs)
+
+// bilateral_grid with the s_sigma GeneratorParam as a run-time argument: what the generator built with s_sigma = S
+// computes.  S = 8 is bilateral_grid itself (its kernels, bit for bit); every other S runs bg_hist_blurz_s, bg_blur_xy
+// and bg_slice_s.  Buffer rules, error codes and the bounds query are bilateral_grid's.
+extern "C" int halide_b200_bilateral_grid_s_sigma(halide_buffer_t *input, int32_t s_sigma, float r_sigma,
+                                                  halide_buffer_t *output) {
+    int r;
+    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[2]}};
+    if ((r = hb::check_args(args, 2))) return r;
+    const hb::Region need[2] = {hb::region_of(output, true), hb::region_of(output, false)};
+    if (hb::answer_bounds_query(args, need, 2)) return 0;
+    if ((r = hb::check_shapes(args, 2)) || (r = hb::check_required(args, need, 2))) return r;
+    const int W = output->dim[0].extent, H = output->dim[1].extent;
+    if (W <= 0 || H <= 0) return 0;
+    if (s_sigma < 1 || s_sigma > 128) {
+        return hb::fail(s_sigma < 1 ? halide_error_code_param_too_small : halide_error_code_param_too_large,
+                        "Parameter s_sigma is %d but must be in [1, 128]", (int)s_sigma);
+    }
+    if (s_sigma == S) return bilateral_grid(input, r_sigma, output);
+    if (!(r_sigma > 0.0f)) {
+        return hb::fail(halide_error_code_param_too_small, "Parameter r_sigma is %g but must be positive", (double)r_sigma);
+    }
+    BGParams p;
+    p.inv_r = 1.0f / r_sigma;
+    p.zmax = (int)(1.0f * p.inv_r + 0.5f);
+    p.nz = p.zmax + 2;
+    // the same bin limit as bilateral_grid: one 128-thread block of lane-private bins
+    const size_t bins_bytes = (size_t)(p.zmax + 1) * 2 * 128 * sizeof(float);
+    if (bins_bytes > 200 * 1024) {
+        return hb::fail(halide_error_code_param_too_small,
+                        "Parameter r_sigma is %g: more than %d intensity bins are not supported by this build",
+                        (double)r_sigma, (int)(200 * 1024 / (2 * 128 * sizeof(float))));
+    }
+    const int Ss = s_sigma;
+    BGSParams q;
+    q.S = Ss;
+    q.inv_s = (float)(1.0 / (double)Ss);
+    q.mag = (uint32_t)(((1u << kMagShift) + Ss - 1) / Ss);
+    choose_slice_tile(q, p.nz);
+    if ((r = hb::acquire(args, 2))) return r;
+
+    const int ox = output->dim[0].min, oy = output->dim[1].min;
+    p.in = (const float *)args[0].dev;
+    p.in_sy = input->dim[1].stride;
+    p.in_x0 = input->dim[0].min; p.in_y0 = input->dim[1].min;
+    p.in_w = input->dim[0].extent; p.in_h = input->dim[1].extent;
+    p.out = (float *)args[1].dev;
+    p.out_sy = output->dim[1].stride;
+    p.out_x0 = ox; p.out_y0 = oy; p.W = W; p.H = H;
+    // cells the slice touches are xi..xi+1; blury/blurx add 2 cells on every side
+    p.gx0 = fdiv(ox, Ss) - 2;
+    p.gy0 = fdiv(oy, Ss) - 2;
+    p.gw = fdiv(ox + W - 1, Ss) + 1 + 2 - p.gx0 + 1;
+    p.gh = fdiv(oy + H - 1, Ss) + 1 + 2 - p.gy0 + 1;
+    choose_hist_block(q, p.zmax + 1, p.gw, p.gh);
+    hb::Scratch scratch;
+    const size_t gelems = (size_t)p.gw * p.gh * p.nz * 2;
+    p.grid_a = scratch.get<float>(gelems);
+    p.grid_b = scratch.get<float>(gelems);
+    if (!p.grid_a || !p.grid_b) return hb::fail(halide_error_code_device_malloc_failed, "bilateral_grid: scratch allocation failed");
+
+    cudaStream_t s = hb::stream();
+    {
+        hb::CallTimer timer(s);
+        static hb::PerDeviceOnce hist_attr, slice_attr;
+        const size_t hist_bytes = hist_s_bytes(q, p.zmax + 1);
+        if (hist_bytes > 48 * 1024) {
+            hist_attr.run([] { cudaFuncSetAttribute(bg_hist_blurz_s_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024); });
+        }
+        dim3 g1(p.gh, (p.gw + q.cpb - 1) / q.cpb);
+        HB_LAUNCH("bg_hist_blurz_s", bg_hist_blurz_s_kernel, g1, 256, hist_bytes, s, p, q);
+        const int V = p.nz * 2;
+        const int cols = (p.gw - 4) * V;
+        int rows = 16;
+        while (rows > 2 && (int64_t)((cols + 255) / 256) * ((p.gh - 4 + rows - 1) / rows) < 132 * 4) rows >>= 1;
+        dim3 g2((cols + 255) / 256, (p.gh - 4 + rows - 1) / rows);
+        HB_LAUNCH("bg_blur_xy", bg_blur_xy_kernel, g2, 256, 0, s, p, rows);
+        const int tw = 4 * q.tx, tx0 = ox & ~3;
+        dim3 g3((H + q.th - 1) / q.th, (ox + W - tx0 + tw - 1) / tw);
+        const size_t slice_smem = slice_s_bytes(q, p.nz);
+        if (slice_smem > 48 * 1024) {
+            slice_attr.run([] { cudaFuncSetAttribute(bg_slice_s_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSliceMaxSmem); });
+        }
+        HB_LAUNCH("bg_slice_s", bg_slice_s_kernel, g3, 256, slice_smem, s, p, q);
+    }
+    return hb::finish(args, 2, "bilateral_grid launch");
+}

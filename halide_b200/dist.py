@@ -122,8 +122,10 @@ def halo_rows(name, **params):
     if name == "stencil_chain":
         return 2 * params.get("stencils", 32), 2 * params.get("stencils", 32)   # 5x5 stencil per stage
     if name == "bilateral_grid":
-        # grid cells yi-2 .. yi+3 (blury +-2, slice yi / yi+1) of 8 rows each, cell origin offset by -4: <= 27 rows
-        return 32, 32
+        # grid cells yi-2 .. yi+3 (blury +-2, slice yi / yi+1) of S rows each, cell origin offset by -S/2: at most
+        # 3S - 1 + S/2 rows above and 4S - 1 - S/2 below (S = s_sigma, 8 unless given)
+        s = params.get("s_sigma", 8)
+        return 4 * s, 4 * s
     raise ValueError(f"no halo rule for {name}")
 
 
@@ -226,10 +228,13 @@ class InputHaloSharder:
         from . import filters
         return self._run("stencil_chain", lambda bi, bo: filters.stencil_chain(bi, bo), in_band, frame_h, out_band, frame_h)
 
-    def bilateral_grid(self, in_band, r_sigma, out_band, frame_h):
+    def bilateral_grid(self, in_band, r_sigma, out_band, frame_h, s_sigma=8):
         from . import filters
-        return self._run("bilateral_grid", lambda bi, bo: filters.bilateral_grid(bi, r_sigma, bo), in_band, frame_h,
-                         out_band, frame_h)
+        if s_sigma == 8:
+            invoke = lambda bi, bo: filters.bilateral_grid(bi, r_sigma, bo)  # noqa: E731
+        else:
+            invoke = lambda bi, bo: filters.bilateral_grid_s_sigma(bi, s_sigma, r_sigma, bo)  # noqa: E731
+        return self._run("bilateral_grid", invoke, in_band, frame_h, out_band, frame_h, s_sigma=s_sigma)
 
     def camera_pipe(self, raw_band, raw_frame_h, m3200, m7000, color_temp, gamma, contrast, sharpen_strength, black, white,
                     out_band, out_frame_h):

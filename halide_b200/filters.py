@@ -95,6 +95,14 @@ def bilateral_grid(input, r_sigma, output):
     return check(lib.bilateral_grid(input.ptr, ctypes.c_float(r_sigma), output.ptr))
 
 
+def bilateral_grid_s_sigma(input, s_sigma, r_sigma, output):
+    """bilateral_grid with the generator's s_sigma (grid cell size in pixels, the spatial scale of the smoothing) chosen
+    per call, 1 <= s_sigma <= 128: the result is what the generator built with that s_sigma computes.  Buffers, r_sigma
+    and error codes as bilateral_grid; s_sigma = 8 is bilateral_grid itself, bit for bit."""
+    return check(lib.halide_b200_bilateral_grid_s_sigma(input.ptr, ctypes.c_int32(s_sigma), ctypes.c_float(r_sigma),
+                                                        output.ptr))
+
+
 def nl_means(input, patch_size, search_area, sigma, output):
     """apps/nl_means/nl_means_generator.cpp, float32, output has exactly 3 channels."""
     return check(lib.nl_means(input.ptr, ctypes.c_int32(patch_size), ctypes.c_int32(search_area),

@@ -323,6 +323,13 @@ int halide_b200_local_laplacian_u8_interleaved(struct halide_buffer_t *input, in
 int halide_b200_local_laplacian_u8_interleaved_batch(struct halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                                      struct halide_buffer_t *output);
 
+/* bilateral_grid with its s_sigma GeneratorParam (the grid cell size in pixels, 8 in bilateral_grid) as an argument:
+ * the result is what the generator built with s_sigma computes.  s_sigma must be in [1, 128] (else
+ * halide_error_code_param_too_small / _too_large, checked after the buffer checks and the bounds query, before any CUDA
+ * call); r_sigma, buffers, error codes and the bounds query follow bilateral_grid, which s_sigma == 8 runs, bit for bit. */
+int halide_b200_bilateral_grid_s_sigma(struct halide_buffer_t *input, int32_t s_sigma, float r_sigma,
+                                       struct halide_buffer_t *output);
+
 /* Host-only probe of the band geometry for tests: with level jr gathered, out[j*8..j*8+7] = {own.lo, own.hi, d.lo, d.hi,
  * u.lo, u.hi, S.lo, S.hi} per pyramid level j = 0..7 (rows owned in the gather partition / Gaussian-side rows computed and
  * held / outGPyramid rows needed / the level's rows on the whole frame), out[64..65] = input rows read. */
