@@ -162,16 +162,32 @@ def stencil_chain(inp, out_shape=None, in_mins=None, out_mins=None, stencils=32)
 
 
 def camera_pipe(raw, m3200, m7000, color_temp, gamma, contrast, sharpen_strength, black, white, out_shape, in_mins=None,
-                out_mins=None):
-    """raw: uint16 [h, w]; m3200/m7000: float32 [3, 4]; returns uint8 [3, H, W]."""
+                out_mins=None, m3200_mins=None, m7000_mins=None):
+    """raw: uint16 [h, w]; m3200/m7000: float32 [3, 4], or larger arrays whose element (x, y) = (0, 0) sits at the
+    given mins; returns uint8 [3, H, W]."""
     out = np.zeros(out_shape, np.uint8)
-    r = lib().oracle_camera_pipe(ctypes.byref(image(raw, in_mins)), ctypes.byref(image(m3200)), ctypes.byref(image(m7000)),
+    r = lib().oracle_camera_pipe(ctypes.byref(image(raw, in_mins)), ctypes.byref(image(m3200, m3200_mins)),
+                                 ctypes.byref(image(m7000, m7000_mins)),
                                  ctypes.c_float(color_temp), ctypes.c_float(gamma), ctypes.c_float(contrast),
                                  ctypes.c_float(sharpen_strength), ctypes.c_int(black), ctypes.c_int(white),
                                  ctypes.byref(image(out, out_mins)))
     if r != 0:
         raise RuntimeError(f"oracle_camera_pipe returned {r}")
     return out
+
+
+def camera_pipe_tables(m3200, m7000, color_temp, gamma, contrast, sharpen_strength, black, white):
+    """camera_pipe's per-call tables: (Q8.8 colour matrix int16 [3, 4], tone curve uint8 [1024], sharpen_strength_x32).
+    m3200/m7000: float32 [3, 4]."""
+    m32, m70 = (np.ascontiguousarray(m, np.float32) for m in (m3200, m7000))
+    matrix = np.zeros((3, 4), np.int16)
+    curve = np.zeros(1024, np.uint8)
+    s32 = ctypes.c_uint8()
+    f = ctypes.c_void_p
+    lib().oracle_camera_pipe_tables(m32.ctypes.data_as(f), m70.ctypes.data_as(f), ctypes.c_float(color_temp), ctypes.c_float(gamma),
+                                    ctypes.c_float(contrast), ctypes.c_float(sharpen_strength), ctypes.c_int(black),
+                                    ctypes.c_int(white), matrix.ctypes.data_as(f), curve.ctypes.data_as(f), ctypes.byref(s32))
+    return matrix, curve, s32.value
 
 
 def conv_layer(inp, filt, bias):
