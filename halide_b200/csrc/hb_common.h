@@ -60,7 +60,7 @@ void *scratch_alloc(size_t bytes);  // returns nullptr on failure (caller maps t
 void scratch_free(void *p);         // stream-ordered: safe to call right after the last launch
 
 struct Scratch {  // frees everything it handed out when the filter call returns
-    static constexpr int kMax = 48;
+    static constexpr int kMax = 64;  // (local_laplacian at pyramid_levels 20 takes 57: three arrays for each of levels 1 .. 19)
     void *ptrs[kMax];
     int n = 0;
     ~Scratch() {

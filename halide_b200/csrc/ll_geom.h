@@ -14,7 +14,9 @@
 
 namespace ll {
 
-constexpr int kMaxJ = 8;  // pyramid_levels GeneratorParam of the shipped app (generator :10)
+constexpr int kMaxJ = 8;  // pyramid_levels GeneratorParam of the shipped app (generator :10): the level slots of the kernels'
+                          // LevelSet / FrameStrides, and J of every entry point but halide_b200_local_laplacian_pyramid_levels
+constexpr int kMaxLevels = 20;  // the generator's largest pyramid_levels (maxJ, generator :6): sizes the host-side geometry
 
 struct Span {
     int lo, hi;  // inclusive
@@ -35,12 +37,12 @@ struct Level {
 
 struct Geom {
     int J;
-    Level lv[kMaxJ];
+    Level lv[kMaxLevels];
 };
 
 // out_[xy]: output region; in_[xy]: bounds of the input buffer (for the clamp / constant borders).
 inline void compute_axis(Span out, Span in, int J, Span *S, Span *O) {
-    Span G[kMaxJ];
+    Span G[kMaxLevels];
     O[0] = out;
     for (int j = 1; j < J; j++) O[j] = {fdiv2(O[j - 1].lo - 1), fdiv2(O[j - 1].hi + 1)};
     G[J - 1] = O[J - 1];
@@ -65,7 +67,7 @@ inline void compute_axis(Span out, Span in, int J, Span *S, Span *O) {
 inline Geom make_geom(Span outx, Span outy, Span inx, Span iny, int J) {
     Geom g;
     g.J = J;
-    Span SX[kMaxJ], OX[kMaxJ], SY[kMaxJ], OY[kMaxJ];
+    Span SX[kMaxLevels], OX[kMaxLevels], SY[kMaxLevels], OY[kMaxLevels];
     compute_axis(outx, inx, J, SX, OX);
     compute_axis(outy, iny, J, SY, OY);
     for (int j = 0; j < J; j++) {

@@ -52,7 +52,8 @@ const halide_filter_argument_t kU8BatchArgs[2] = {
 template<typename T>
 struct PlanT {
     LLFrameT<T> f;
-    LevelSet ls{};  // (level 0 is never stored: its slot stays zero)
+    LevelSetDeep ls{};  // levels 1 .. J-1 (level 0 is never stored: its slot stays zero)
+    int J = ll::kMaxJ;  // pyramid levels (8 but for halide_b200_local_laplacian_pyramid_levels, whose frames have N == 1)
     int N;  // frames (1 but for a batch)
     FrameStrides fs;  // all zero when N == 1 (but the pixel pitches)
     float alpha;
@@ -82,8 +83,8 @@ void for_frame_groups(const P &p, F launch) {
 }
 
 // The checks local_laplacian and its sharded and batch variants share, on args = {input, output}.  *done: return r now
-// (an error, a bounds query or an empty output).
-int check_and_query(hb::Arg *args, int levels, bool *done) {
+// (an error, a bounds query or an empty output).  J: the pyramid_levels GeneratorParam, checked after levels.
+int check_and_query(hb::Arg *args, int levels, bool *done, int J = ll::kMaxJ) {
     int r;
     *done = true;
     if ((r = hb::check_args(args, 2))) return r;
@@ -97,6 +98,10 @@ int check_and_query(hb::Arg *args, int levels, bool *done) {
         // 1/(levels-1) (generator :41) is meaningless below 2; the reference does not check, we do.
         return hb::fail(levels < 2 ? halide_error_code_param_too_small : halide_error_code_param_too_large,
                         "Parameter levels is %d but must be in [2, 32]", levels);
+    }
+    if (J < 1 || J > ll::kMaxLevels) {
+        return hb::fail(J < 1 ? halide_error_code_param_too_small : halide_error_code_param_too_large,
+                        "Parameter pyramid_levels is %d but must be in [1, %d]", J, ll::kMaxLevels);
     }
     for (int d = 0; d < output->dimensions; d++) {
         if (output->dim[d].extent <= 0) return 0;
@@ -190,12 +195,13 @@ int get_lut(PlanT<T> &p, cudaStream_t s) {
     return 0;
 }
 
-// the fast level-1 kernel also produces level 2
+// the fast level-1 kernel also produces level 2 (so the pyramid must have one: J >= 3)
 template<typename P>
-bool fast_down(const P &p) { return p.f.levels == 8 && !(g_force_naive & 1); }
-// the fast final kernel also produces outGPyramid[1] (for its own tile), so no up-sweep launch runs for level 1
+bool fast_down(const P &p) { return p.f.levels == 8 && p.J >= 3 && !(g_force_naive & 1); }
+// the fast final kernel also produces outGPyramid[1] (for its own tile) from level 2, so no up-sweep launch runs for
+// level 1 (J >= 3 as well)
 template<typename P>
-bool fast_final(const P &p) { return p.f.levels == 8 && !(g_force_naive & 4) && p.f.C <= 3; }
+bool fast_final(const P &p) { return p.f.levels == 8 && p.J >= 3 && !(g_force_naive & 4) && p.f.C <= 3; }
 // lowest level the up-sweep launches produce
 template<typename P>
 int first_up_level(const P &p) { return fast_final(p) ? 2 : 1; }
@@ -203,7 +209,7 @@ int first_up_level(const P &p) { return fast_final(p) ? 2 : 1; }
 template<typename P>
 int alloc_levels(P &p, const ll::Geom &geom, hb::Scratch &scratch) {
     const int nq = (p.f.levels + 1) / 2;
-    for (int j = 1; j < ll::kMaxJ; j++) {
+    for (int j = 1; j < p.J; j++) {
         const ll::Level &lv = geom.lv[j];
         LevelBuf &b = p.ls.lv[j];
         b.sx = lv.sx; b.sy = lv.sy; b.ox = lv.ox; b.oy = lv.oy;
@@ -218,7 +224,7 @@ int alloc_levels(P &p, const ll::Geom &geom, hb::Scratch &scratch) {
         b.gp = scratch.get<float>((size_t)gp_sn * p.N);
         b.ing = scratch.get<float>((size_t)ing_sn * p.N);
         b.outg = with_outg ? scratch.get<float>((size_t)outg_sn * p.N) : nullptr;
-        if (p.N > 1) p.fs.gp[j] = gp_sn, p.fs.ing[j] = ing_sn, p.fs.outg[j] = outg_sn;
+        if (p.N > 1) p.fs.gp[j] = gp_sn, p.fs.ing[j] = ing_sn, p.fs.outg[j] = outg_sn;  // (N > 1: J == 8)
         if (!b.gp || !b.ing || (with_outg && !b.outg)) {
             return hb::fail(halide_error_code_device_malloc_failed, "local_laplacian: scratch allocation failed");
         }
@@ -329,6 +335,13 @@ void launch_level12(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2, cudaS
     else launch_level12_il<false>(p, f, cy1, cy2, s);
 }
 
+// Index of level j's entries in FrameStrides, whose arrays have ll::kMaxJ slots (a kernel reads those of j - 1 .. j + 1).
+// A batch has J == 8: j itself.  A deeper pyramid (J > 8) is a single frame, whose level strides are all zero: its
+// levels from 7 on, whose neighbours could reach slot 8, take slot 6 (neighbours 5 .. 7) — every read stays inside the
+// arrays and still sees a zero stride.
+template<typename P>
+int fs_slot(const P &p, int j) { return p.J <= ll::kMaxJ ? j : std::min(j, ll::kMaxJ - 2); }
+
 template<typename T>
 void launch_down(PlanT<T> &p, int j, cudaStream_t s) {  // produce level j (j >= 1) rows cy
     LevelBuf *lb = p.ls.lv;
@@ -343,7 +356,7 @@ void launch_down(PlanT<T> &p, int j, cudaStream_t s) {  // produce level j (j >=
             const int slots = resident_slots(kern, 256, 0);
             long long g = (tasks + 7) / 8;
             if (g > slots) g = slots;
-            HB_LAUNCH("ll_down_rows", kern, (int)g, 256, 0, s, lb[j - 1], lb[j], ns, ng, p.N, j, p.fs);
+            HB_LAUNCH("ll_down_rows", kern, (int)g, 256, 0, s, lb[j - 1], lb[j], ns, ng, p.N, fs_slot(p, j), p.fs);
         }
     } else if (lb[j].cy.n() <= 0) {
         return;
@@ -355,10 +368,11 @@ void launch_down(PlanT<T> &p, int j, cudaStream_t s) {  // produce level j (j >=
                       at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), p.fs);
         });
     } else {
+        const int js = fs_slot(p, j);
         for_frame_groups(p, [&](int n0, int nf) {
             dim3 g = grid_for(lb[j].sx.n(), lb[j].cy.n());
             g.z = nf;
-            HB_LAUNCH("ll_down", ll_down_naive_kernel, g, kBlk, 0, s, at_frame(lb[j - 1], j - 1, p.fs, n0), at_frame(lb[j], j, p.fs, n0), p.f.levels, j,
+            HB_LAUNCH("ll_down", ll_down_naive_kernel, g, kBlk, 0, s, at_frame(lb[j - 1], js - 1, p.fs, n0), at_frame(lb[j], js, p.fs, n0), p.f.levels, js,
                       p.fs);
         });
     }
@@ -373,18 +387,20 @@ void launch_up(P &p, int j, cudaStream_t s) {  // produce outGPyramid[j] (1 <= j
     LevelBuf *lb = p.ls.lv;
     if (lb[j].coy.n() <= 0) return;
     const bool fast_up = p.f.levels == 8 && !(g_force_naive & 2);
+    const bool top = j == p.J - 1;
+    const int js = fs_slot(p, j);
     for_frame_groups(p, [&](int n0, int nf) {
-        if (fast_up && j < ll::kMaxJ - 1) {
+        if (fast_up && !top) {
             static const CUtensorMap no_map = {};
             HB_LAUNCH("ll_up2", (nf > 1 ? ll_up2_kernel<false, false, true, false, true> : ll_up2_kernel<false, false, true, false, false>), up_grid(lb[j].ox.lo, lb[j].ox.hi, lb[j].coy.lo, lb[j].coy.hi, nf),
-                      256, up2_smem_bytes(false, false), s, scalars_frame(at_frame(p.f, p.fs, n0)), at_frame(lb[j], j, p.fs, n0),
-                      at_frame(lb[j + 1], j + 1, p.fs, n0), no_map, j, p.fs);
+                      256, up2_smem_bytes(false, false), s, scalars_frame(at_frame(p.f, p.fs, n0)), at_frame(lb[j], js, p.fs, n0),
+                      at_frame(lb[j + 1], js + 1, p.fs, n0), no_map, js, p.fs);
         } else {
             dim3 g = grid_for(lb[j].ox.n(), lb[j].coy.n());
             g.z = nf;
-            const int jc = j == ll::kMaxJ - 1 ? j : j + 1;
-            HB_LAUNCH("ll_up", ll_up_naive_kernel, g, kBlk, 0, s, at_frame(lb[j], j, p.fs, n0), at_frame(lb[jc], jc, p.fs, n0),
-                      p.f.flm1, p.f.levels, j == ll::kMaxJ - 1 ? 1 : 0, j, p.fs);
+            const int jc = top ? j : j + 1;
+            HB_LAUNCH("ll_up", ll_up_naive_kernel, g, kBlk, 0, s, at_frame(lb[j], js, p.fs, n0), at_frame(lb[jc], top ? js : js + 1, p.fs, n0),
+                      p.f.flm1, p.f.levels, top ? 1 : 0, js, p.fs);
         }
     });
 }
@@ -501,15 +517,20 @@ bool launch_coarse_fused(P &p, int j0, cudaStream_t s) {
             coop = it->second;
         }
     }
-    auto kern = p.N > 1 ? ll_coarse_fused_kernel<true> : ll_coarse_fused_kernel<false>;
+    // J <= 8: the LevelSet instantiations, on the first 8 slots; a deeper pyramid (one frame) takes all of LevelSetDeep
+    LevelSet ls8;
+    memcpy(ls8.lv, p.ls.lv, sizeof ls8.lv);
+    const bool deep = p.J > ll::kMaxJ;
+    const void *kern = deep ? (const void *)ll_coarse_fused_kernel<false, LevelSetDeep>
+                            : (p.N > 1 ? (const void *)ll_coarse_fused_kernel<true> : (const void *)ll_coarse_fused_kernel<false>);
     const int slots = resident_slots(kern, 256, 0);  // sms * blocks per SM
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int max_blocks = coop ? (slots > 2 * sms ? 2 * sms : slots) : 0;
     if (max_blocks <= 0) return false;
-    int J = ll::kMaxJ, K = p.f.levels, levels = p.f.levels, jd = fast_down(p) && j0 < 2 ? 2 : j0, nf = p.N;
+    int J = p.J, K = p.f.levels, levels = p.f.levels, jd = fast_down(p) && j0 < 2 ? 2 : j0, nf = p.N;
     float flm1 = p.f.flm1;
-    void *args[] = {&p.ls, &J, &j0, &jd, &K, &flm1, &levels, &nf, &p.fs};
+    void *args[] = {deep ? (void *)&p.ls : (void *)&ls8, &J, &j0, &jd, &K, &flm1, &levels, &nf, &p.fs};
     hb::count_launch("ll_coarse_fused", s);
     cudaError_t e = cudaLaunchCooperativeKernel((void *)kern, dim3(max_blocks), dim3(256), args, 0, s);
     hb::after_launch(s);
@@ -520,11 +541,11 @@ bool launch_coarse_fused(P &p, int j0, cudaStream_t s) {
     return true;
 }
 
-// Levels from_level+1 .. J-1 down, then J-1 .. from_level+1 up: the part of the sweep that runs on whole levels
-// (everything on one GPU; the replicated coarse levels when row-sharded).  Small levels share one cooperative launch.
+// Last level of the sweep from from_level that has launches of its own: the levels above it, of at most 40 K pixels each
+// (all N frames'), share the fused tail.
 template<typename P>
-void run_coarse_sweep(P &p, int from_level, cudaStream_t s) {
-    int j0 = ll::kMaxJ - 1;
+int last_own_level(const P &p, int from_level) {
+    int j0 = p.J - 1;
     if (!(g_force_naive & 8)) {
         // (level 1 always has its own launch: it is built from the frame, not from a stored level; on the fast path that
         // launch also builds level 2, and the fused tail's down-sweep starts after it).  The size is the batch's: all N
@@ -532,39 +553,71 @@ void run_coarse_sweep(P &p, int from_level, cudaStream_t s) {
         const int j_min = from_level < 1 ? 1 : from_level;
         while (j0 > j_min && (int64_t)p.ls.lv[j0].sx.n() * p.ls.lv[j0].sy.n() * p.N <= 40 * 1024) j0--;
     }
+    return j0;
+}
+
+// Levels from_level+1 .. J-1 down, then J-1 .. from_level+1 up: the part of the sweep that runs on whole levels
+// (everything on one GPU; the replicated coarse levels when row-sharded).  Small levels share one cooperative launch.
+template<typename P>
+void run_coarse_sweep(P &p, int from_level, cudaStream_t s) {
     // j0 = last level produced by its own launch; levels j0+1.. are fused (if any)
+    const int j0 = last_own_level(p, from_level);
     bool fused = false;
     for (int j = from_level + 1; j <= j0; j++) launch_down(p, j, s);
-    if (j0 < ll::kMaxJ - 1) fused = launch_coarse_fused(p, j0, s);
+    if (j0 < p.J - 1) fused = launch_coarse_fused(p, j0, s);
     if (!fused) {
-        for (int j = j0 + 1; j < ll::kMaxJ; j++) launch_down(p, j, s);
-        for (int j = ll::kMaxJ - 1; j > j0; j--) launch_up(p, j, s);
+        for (int j = j0 + 1; j < p.J; j++) launch_down(p, j, s);
+        for (int j = p.J - 1; j > j0; j--) launch_up(p, j, s);
     }
     for (int j = j0; j > from_level && j >= first_up_level(p); j--) launch_up(p, j, s);
 }
 
-// One GPU, args = {input, output} of 3 dimensions (one frame) or 4 (a batch of frames along dimension 3), elements T.
+// J = 1: the whole filter is the pointwise tone kernel over the output region (ll_tone_kernel).  Its aligned form needs
+// every plane row it reads and writes to start on 16 bytes at the output's first column.
+void launch_tone(Plan &p, cudaStream_t s) {
+    const LLFrame &f = p.f;
+    const int upr = (f.W + kTonePx - 1) / kTonePx;
+    const long long units = (long long)upr * f.H;
+    auto a16 = [](int64_t bytes) { return (bytes & 15) == 0; };
+    const uint16_t *in0 = f.in + (int64_t)(f.out_y0 - f.in_y0) * f.in_sy + (f.out_x0 - f.in_x0);
+    const bool vec = a16((int64_t)(uintptr_t)in0) && a16(f.in_sy * 2) && a16(f.in_sc * 2) && a16((int64_t)(uintptr_t)f.out) &&
+                     a16(f.out_sy * 2) && a16(f.out_sc * 2) && !(g_force_naive & 16);
+    const size_t smem = (size_t)(2 * f.lut_half + 1) * sizeof(float);
+    auto kern = vec ? ll_tone_kernel<true> : ll_tone_kernel<false>;
+    const int slots = resident_slots(kern, 256, smem);  // (also sets the > 48 KB shared-memory attribute: levels > 24)
+    const int g = (int)std::min<long long>(slots, (units + 255) / 256);
+    HB_LAUNCH("ll_tone", kern, g, 256, smem, s, f, upr, units);
+}
+
+// One GPU, args = {input, output} of 3 dimensions (one frame) or 4 (a batch of frames along dimension 3), elements T;
+// J = pyramid levels (8 but for halide_b200_local_laplacian_pyramid_levels: uint16, one frame).
 template<typename T>
-int run_local_laplacian(hb::Arg *args, int levels, float alpha, float beta, const char *what) {
+int run_local_laplacian(hb::Arg *args, int levels, float alpha, float beta, int J, const char *what) {
     int r;
     bool done;
-    if ((r = check_and_query(args, levels, &done)) || done) return r;
+    if ((r = check_and_query(args, levels, &done, J)) || done) return r;
     if ((r = hb::acquire(args, 2))) return r;
 
     PlanT<T> p;
     fill_frame(p, args, levels, alpha, beta);
+    p.J = J;
     const int W = p.f.W, H = p.f.H;
     Span outx = {p.f.out_x0, p.f.out_x0 + W - 1}, outy = {p.f.out_y0, p.f.out_y0 + H - 1};
     Span inx = {p.f.in_x0, p.f.in_x0 + p.f.in_w - 1}, iny = {p.f.in_y0, p.f.in_y0 + p.f.in_h - 1};
     hb::Scratch scratch;
-    if ((r = alloc_levels(p, ll::make_geom(outx, outy, inx, iny, ll::kMaxJ), scratch))) return r;
+    if ((r = alloc_levels(p, ll::make_geom(outx, outy, inx, iny, J), scratch))) return r;
 
     cudaStream_t s = hb::stream();
     if ((r = get_lut(p, s))) return r;
     {
         hb::CallTimer timer(s);
-        run_coarse_sweep(p, 0, s);
-        launch_final(p, s);
+        if constexpr (std::is_same<T, uint16_t>::value) {
+            if (J == 1) launch_tone(p, s);
+        }
+        if (J > 1) {
+            run_coarse_sweep(p, 0, s);
+            launch_final(p, s);
+        }
     }
     return hb::finish(args, 2, what);
 }
@@ -573,7 +626,7 @@ int run_local_laplacian(hb::Arg *args, int levels, float alpha, float beta, cons
 
 extern "C" int local_laplacian(halide_buffer_t *input, int32_t levels, float alpha, float beta, halide_buffer_t *output) {
     hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[4]}};
-    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, "local_laplacian launch");
+    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, ll::kMaxJ, "local_laplacian launch");
 }
 HB_EXPORT_FILTER(local_laplacian, kArgs)
 
@@ -581,7 +634,7 @@ HB_EXPORT_FILTER(local_laplacian, kArgs)
 extern "C" int halide_b200_local_laplacian_batch(halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                                  halide_buffer_t *output) {
     hb::Arg args[2] = {{input, kBatchArgs[0]}, {output, kBatchArgs[1]}};
-    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, "local_laplacian_batch launch");
+    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, ll::kMaxJ, "local_laplacian_batch launch");
 }
 
 // 8-bit entry points (library extensions): out8 = to_u8(local_laplacian(to_u16(in8))) with the reference's element
@@ -589,12 +642,12 @@ extern "C" int halide_b200_local_laplacian_batch(halide_buffer_t *input, int32_t
 extern "C" int halide_b200_local_laplacian_u8(halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                               halide_buffer_t *output) {
     hb::Arg args[2] = {{input, kU8Args[0]}, {output, kU8Args[1]}};
-    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, "local_laplacian_u8 launch");
+    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, ll::kMaxJ, "local_laplacian_u8 launch");
 }
 extern "C" int halide_b200_local_laplacian_u8_batch(halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                                     halide_buffer_t *output) {
     hb::Arg args[2] = {{input, kU8BatchArgs[0]}, {output, kU8BatchArgs[1]}};
-    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, "local_laplacian_u8_batch launch");
+    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, ll::kMaxJ, "local_laplacian_u8_batch launch");
 }
 
 // Interleaved entry points (library extensions): the four above on pixel-interleaved buffers (RGBRGB..., RGBA...:
@@ -603,25 +656,35 @@ extern "C" int halide_b200_local_laplacian_u8_batch(halide_buffer_t *input, int3
 extern "C" int halide_b200_local_laplacian_interleaved(halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                                        halide_buffer_t *output) {
     hb::Arg args[2] = {{input, kArgs[0], nullptr, true}, {output, kArgs[4], nullptr, true}};
-    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, "local_laplacian_interleaved launch");
+    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, ll::kMaxJ, "local_laplacian_interleaved launch");
 }
 extern "C" int halide_b200_local_laplacian_interleaved_batch(halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                                              halide_buffer_t *output) {
     hb::Arg args[2] = {{input, kBatchArgs[0], nullptr, true}, {output, kBatchArgs[1], nullptr, true}};
-    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, "local_laplacian_interleaved_batch launch");
+    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, ll::kMaxJ, "local_laplacian_interleaved_batch launch");
 }
 extern "C" int halide_b200_local_laplacian_u8_interleaved(halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                                           halide_buffer_t *output) {
     hb::Arg args[2] = {{input, kU8Args[0], nullptr, true}, {output, kU8Args[1], nullptr, true}};
-    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, "local_laplacian_u8_interleaved launch");
+    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, ll::kMaxJ, "local_laplacian_u8_interleaved launch");
 }
 extern "C" int halide_b200_local_laplacian_u8_interleaved_batch(halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                                                 halide_buffer_t *output) {
     hb::Arg args[2] = {{input, kU8BatchArgs[0], nullptr, true}, {output, kU8BatchArgs[1], nullptr, true}};
-    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, "local_laplacian_u8_interleaved_batch launch");
+    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, ll::kMaxJ, "local_laplacian_u8_interleaved_batch launch");
 }
 // The harness's second AOT variant (apps/local_laplacian/process.cpp:44-48): same implementation.
 HB_EXPORT_AUTO_SCHEDULE(local_laplacian, kArgs)
+
+// local_laplacian with the pyramid_levels GeneratorParam J (generator :6,10) as a run-time argument, 1 <= J <= 20: what
+// the generator built with pyramid_levels = J computes, on the buffers local_laplacian takes.  J = 8 is local_laplacian
+// itself (the same launches); J >= 3 runs the same kernels over J levels (the fast level-1 and final kernels need level
+// 2), J = 2 the generic ones, and J = 1, where the filter is pointwise, only ll_tone.
+extern "C" int halide_b200_local_laplacian_pyramid_levels(halide_buffer_t *input, int32_t pyramid_levels, int32_t levels, float alpha,
+                                                          float beta, halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[4]}};
+    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, pyramid_levels, "local_laplacian_pyramid_levels launch");
+}
 
 namespace {
 
@@ -898,6 +961,20 @@ extern "C" void halide_b200_ll_shard_coarse_level(int level) {
 extern "C" int halide_b200_ll_shard_plan_level(int32_t frame_w, int32_t frame_h, int32_t nranks) {
     Span fx = {0, frame_w - 1}, fy = {0, frame_h - 1};
     return choose_coarse_level(ll::make_geom(fx, fy, fx, fy, ll::kMaxJ), nranks, ll::kMaxJ, 8);
+}
+
+// Probe for the CPU-side tests (no CUDA calls): the last pyramid level that halide_b200_local_laplacian_pyramid_levels
+// gives launches of its own on a frame_w x frame_h frame (input == output region); the levels above it share the fused
+// coarse tail.
+extern "C" int halide_b200_ll_last_own_level(int32_t frame_w, int32_t frame_h, int32_t pyramid_levels) {
+    if (frame_w < 1 || frame_h < 1 || pyramid_levels < 1 || pyramid_levels > ll::kMaxLevels) return -1;
+    Span fx = {0, frame_w - 1}, fy = {0, frame_h - 1};
+    const ll::Geom g = ll::make_geom(fx, fy, fx, fy, pyramid_levels);
+    Plan p;
+    p.J = pyramid_levels;
+    p.N = 1;
+    for (int j = 0; j < p.J; j++) p.ls.lv[j].sx = g.lv[j].sx, p.ls.lv[j].sy = g.lv[j].sy;
+    return last_own_level(p, 0);
 }
 
 // Row-sharded entry point (library extension; see run_local_laplacian_sharded).

@@ -44,6 +44,15 @@ def local_laplacian_u8_batch(input, levels, alpha, beta, output):
                                                           ctypes.c_float(beta), output.ptr))
 
 
+def local_laplacian_pyramid_levels(input, pyramid_levels, levels, alpha, beta, output):
+    """local_laplacian with the generator's pyramid_levels J (the pyramid depth: the coarsest level's pixels cover 2^(J-1)
+    frame pixels, the spatial scale of the detail the filter manipulates) chosen per call, 1 <= J <= 20: the result is
+    what the generator built with that J computes, bit for bit.  Buffers (3-D uint16), levels, alpha, beta and error
+    codes as local_laplacian; J = 8 is local_laplacian itself."""
+    return check(lib.halide_b200_local_laplacian_pyramid_levels(input.ptr, ctypes.c_int32(pyramid_levels), ctypes.c_int32(levels),
+                                                                ctypes.c_float(alpha), ctypes.c_float(beta), output.ptr))
+
+
 _INTERLEAVED_LAYOUT = """
     Both buffers are pixel-interleaved (RGBRGB..., RGBA...): ``dim[2].stride == 1`` and ``dim[0].stride`` is the pixel
     pitch, at least the channel extent; ``dim[1].stride`` (and ``dim[3].stride``) positive.  Anything else, a planar

@@ -330,6 +330,17 @@ int halide_b200_local_laplacian_u8_interleaved_batch(struct halide_buffer_t *inp
 int halide_b200_bilateral_grid_s_sigma(struct halide_buffer_t *input, int32_t s_sigma, float r_sigma,
                                        struct halide_buffer_t *output);
 
+/* local_laplacian with its pyramid_levels GeneratorParam J (the pyramid depth, 8 in local_laplacian) as an argument: the
+ * result is what the generator built with pyramid_levels = J computes, bit for bit.  J must be in [1, 20] (else
+ * halide_error_code_param_too_small / _too_large, checked after the buffer checks, the bounds query and the levels check,
+ * before any CUDA call); buffers (3-D, planar, uint16), levels, alpha, beta, error codes and the bounds query follow
+ * local_laplacian, which J == 8 runs.  J does not change the input region required: it is the output's. */
+int halide_b200_local_laplacian_pyramid_levels(struct halide_buffer_t *input, int32_t pyramid_levels, int32_t levels, float alpha,
+                                               float beta, struct halide_buffer_t *output);
+/* Host-only probe for tests: the last pyramid level halide_b200_local_laplacian_pyramid_levels gives launches of its own
+ * on a frame_w x frame_h frame (the levels above it share one cooperative launch); -1 for arguments out of range. */
+int halide_b200_ll_last_own_level(int32_t frame_w, int32_t frame_h, int32_t pyramid_levels);
+
 /* Host-only probe of the band geometry for tests: with level jr gathered, out[j*8..j*8+7] = {own.lo, own.hi, d.lo, d.hi,
  * u.lo, u.hi, S.lo, S.hi} per pyramid level j = 0..7 (rows owned in the gather partition / Gaussian-side rows computed and
  * held / outGPyramid rows needed / the level's rows on the whole frame), out[64..65] = input rows read. */

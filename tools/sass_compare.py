@@ -8,7 +8,7 @@ halide_b200/csrc/local_laplacian.o in a scratch checkout, build this tree's, and
 Kernels are matched by demangled name.  A template parameter that a change appends with a default value changes the
 mangled name of every existing instantiation without changing its code, so the new object's names are also tried with
 such trailing defaults removed: the interleaved-layout parameters `bool IL = false` (ll_level1_kernel, the generic
-kernels) and `int PI = 1, int PO = 1` (ll_up2_kernel).  Instruction addresses are dropped before comparing; opcodes,
+kernels), `int PI = 1, int PO = 1` (ll_up2_kernel) and the level set type `typename LS = LevelSet` (ll_coarse_fused_kernel).  Instruction addresses and padding are dropped before comparing; opcodes,
 operands and encodings must match.  Prints each old kernel that is missing or differs, then a count; exits 1 if any.
 """
 import re
@@ -17,7 +17,7 @@ import sys
 
 CUOBJDUMP = "/usr/local/cuda/bin/cuobjdump"
 # trailing template arguments that stand for the defaults of appended parameters
-DEFAULT_TAILS = [", 1, 1>(", ", false>("]
+DEFAULT_TAILS = [", 1, 1>(", ", false>(", ", llk::LevelSet>("]
 
 
 def kernels(obj):
@@ -30,7 +30,8 @@ def kernels(obj):
                 res[name] = body
             name, body = m.group(1), []
         elif name and "/*" in line:
-            body.append(re.sub(r"/\*[0-9a-f]{4,}\*/", "", line).strip())
+            # (runs of blanks collapsed: cuobjdump pads every line to the longest instruction in the file)
+            body.append(" ".join(re.sub(r"/\*[0-9a-f]{4,}\*/", "", line).split()))
     if name:
         res[name] = body
     names = list(res)
