@@ -8,11 +8,10 @@
 // changes the summation order; the harness data are all positive so there is no cancellation).
 //
 // The contraction is the tensor-core implicit GEMM of conv_layer_tc.cu (wgmma + TMA, 3xTF32 split): M = 40 000
-// output pixels, N = 128, K = 1152, 11.8 GFLOP.  This file holds the Halide call boundary and the fixed-shape checks.
+// output pixels, N = 128, K = 1152, 11.8 GFLOP.  This file holds the Halide call boundary and the fixed-shape checks,
+// and halide_b200_conv_layer_any_shape: the same algorithm with the five constants read from the buffers.
+#include "conv_layer_tc.h"  // the wgmma / TMA implementation
 #include "hb_common.h"
-
-// wgmma / TMA implementation (conv_layer_tc.cu)
-int conv_layer_tc_run(const float *din, const float *df, const float *db, float *dout, cudaStream_t s);
 
 namespace {
 
@@ -72,3 +71,44 @@ extern "C" int conv_layer(halide_buffer_t *input, halide_buffer_t *filter, halid
 }
 HB_EXPORT_FILTER(conv_layer, kArgs)
 HB_EXPORT_AUTO_SCHEDULE(conv_layer, kArgs)
+
+// conv_layer with the generator's set_bounds / set_stride constraints removed: CO, W, H, N and the mins (c0, x0, y0, n0)
+// are relu's, CI is filter's last extent (input's first when filter is the buffer of a bounds query).  Nothing is
+// edge-clamped, so input must cover [0,CI) x [x0, x0+W+2) x [y0, y0+H+2) x [n0, n0+N), filter [c0, c0+CO) x 3 x 3 x [0,CI)
+// and bias [c0, c0+CO); buffers may be larger and every stride but the innermost (1) is free.
+extern "C" int halide_b200_conv_layer_any_shape(halide_buffer_t *input, halide_buffer_t *filter, halide_buffer_t *bias,
+                                                halide_buffer_t *relu) {
+    int r;
+    hb::Arg args[4] = {{input, kArgs[0]}, {filter, kArgs[1]}, {bias, kArgs[2]}, {relu, kArgs[3]}};
+    if ((r = hb::check_args(args, 4))) return r;
+    const halide_dimension_t *o = relu->dim;
+    const bool filter_queried = filter->host == nullptr && filter->device == 0;
+    const int co = o[0].extent, w = o[1].extent, h = o[2].extent, n = o[3].extent;
+    const int ci = filter_queried ? input->dim[0].extent : filter->dim[3].extent;
+    const hb::Region need[4] = {{{0, o[1].min, o[2].min, o[3].min}, {ci, w + 2, h + 2, n}, true},
+                                {{o[0].min, 0, 0, 0}, {co, 3, 3, ci}, true},
+                                {{o[0].min}, {co}, true},
+                                hb::region_of(relu, false)};
+    if (hb::answer_bounds_query(args, need, 4)) return 0;
+    if ((r = hb::check_shapes(args, 4))) return r;
+    if (co <= 0 || w <= 0 || h <= 0 || n <= 0) return 0;
+    if ((r = hb::check_required(args, need, 4))) return r;
+    if ((r = hb::acquire(args, 4))) return r;
+    const halide_dimension_t *in = input->dim, *f = filter->dim;
+    ConvProblem p;
+    p.N = n, p.CI = ci, p.CO = co, p.W = w, p.H = h;
+    p.in_sx = in[1].stride, p.in_sy = in[2].stride, p.in_sn = in[3].stride;
+    p.in = (const float *)args[0].dev + (0 - in[0].min) + (o[1].min - in[1].min) * p.in_sx + (o[2].min - in[2].min) * p.in_sy +
+           (o[3].min - in[3].min) * p.in_sn;
+    p.f_skx = f[1].stride, p.f_sky = f[2].stride, p.f_sci = f[3].stride;
+    p.filt = (const float *)args[1].dev + (o[0].min - f[0].min) + (0 - f[1].min) * p.f_skx + (0 - f[2].min) * p.f_sky + (0 - f[3].min) * p.f_sci;
+    p.bias = (const float *)args[2].dev + (o[0].min - bias->dim[0].min);
+    p.out = (float *)args[3].dev;
+    p.out_sx = o[1].stride, p.out_sy = o[2].stride, p.out_sn = o[3].stride;
+    cudaStream_t s = hb::stream();
+    {
+        hb::CallTimer timer(s);
+        if ((r = conv_layer_tc_run_any_shape(p, s))) return r;
+    }
+    return hb::finish(args, 4, "conv_layer_any_shape launch");
+}

@@ -129,3 +129,14 @@ def camera_pipe(input, matrix_3200, matrix_7000, color_temp, gamma, contrast, sh
 def conv_layer(input, filter, bias, relu):
     """apps/conv_layer/conv_layer_generator.cpp: 3x3 conv + bias + relu, fixed shapes (N5 CI128 CO128 100x80), f32."""
     return check(lib.conv_layer(input.ptr, filter.ptr, bias.ptr, relu.ptr))
+
+
+def conv_layer_any_shape(input, filter, bias, relu):
+    """conv_layer (3x3 conv + bias + relu, f32) with N, CI, CO, W and H taken from the buffers instead of the generator's
+    fixed shape: relu (co, x, y, n) gives CO, W, H, N and the mins, filter (co, kx, ky, ci) gives CI; input (ci, x, y, n)
+    must cover the output's region grown by two columns and two rows (the caller pads; nothing is clamped), filter and
+    bias the output's channels, else -4.  Buffers may be larger than required and every stride but the channel one (1,
+    else -8) is free, so crops and padded rows of larger tensors work in place.  In torch terms: an NHWC input
+    ``[N, H + 2, W + 2, CI]``, a filter ``[CI, 3, 3, CO]``, a bias ``[CO]`` and an NHWC output ``[N, H, W, CO]``.  At
+    conv_layer's shape the result is conv_layer's, byte for byte."""
+    return check(lib.halide_b200_conv_layer_any_shape(input.ptr, filter.ptr, bias.ptr, relu.ptr))

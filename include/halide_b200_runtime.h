@@ -330,6 +330,20 @@ int halide_b200_local_laplacian_u8_interleaved_batch(struct halide_buffer_t *inp
 int halide_b200_bilateral_grid_s_sigma(struct halide_buffer_t *input, int32_t s_sigma, float r_sigma,
                                        struct halide_buffer_t *output);
 
+/* conv_layer (3x3 convolution + bias + relu, float32) at any shape: the generator's algorithm without its set_bounds /
+ * set_stride constraints,
+ *   relu(co, x, y, n) = max(0, bias(co) + sum over ky, kx, ci of filter(co, kx, ky, ci) * input(ci, x + kx, y + ky, n)).
+ * CO, W, H, N and the mins (c0, x0, y0, n0) are relu's; CI is filter's extent in dimension 3 (input's in dimension 0 when
+ * filter is the buffer of a bounds query).  Nothing is edge-clamped: input must cover [0, CI) x [x0, x0 + W + 2) x
+ * [y0, y0 + H + 2) x [n0, n0 + N), filter [c0, c0 + CO) x [0, 3) x [0, 3) x [0, CI) and bias [c0, c0 + CO), else
+ * halide_error_code_access_out_of_bounds; buffers may be larger, mins need not be 0, and every stride but dim[0].stride
+ * (1, else halide_error_code_constraint_violated) is free, so rows may be padded and buffers may be crops of larger
+ * tensors; elements of relu's memory outside its region are not written.  Types and dimension counts are conv_layer's.  A
+ * bounds query answers with the regions above and dense strides; a relu with a zero extent does nothing and returns 0.  At
+ * conv_layer's shape the result equals conv_layer's byte for byte. */
+int halide_b200_conv_layer_any_shape(struct halide_buffer_t *input, struct halide_buffer_t *filter,
+                                     struct halide_buffer_t *bias, struct halide_buffer_t *relu);
+
 /* local_laplacian with its pyramid_levels GeneratorParam J (the pyramid depth, 8 in local_laplacian) as an argument: the
  * result is what the generator built with pyramid_levels = J computes, bit for bit.  J must be in [1, 20] (else
  * halide_error_code_param_too_small / _too_large, checked after the buffer checks, the bounds query and the levels check,
