@@ -1,4 +1,5 @@
-// stencil_chain.cu — stencil_chain(input, output): 32 successive 5x5 uint16 stencils.
+// stencil_chain.cu — stencil_chain(input, output): 32 successive 5x5 uint16 stencils;
+// halide_b200_stencil_chain_stencils(input, stencils, output): the same chain with 1..100 stages.
 //
 // Reference algorithm: apps/stencil_chain/stencil_chain_generator.cpp:16-34.  Stage s+1 at (x,y) is
 //   e = u16(0); for i in -2..2 (x offset) for j in -2..2 (y offset): e += u16((i+3)*(j+3)) * stage_s(x+i, y+j)
@@ -13,15 +14,16 @@
 //
 // Kernel shape: ALU/shared-memory bound (800 MAC/px in the reference formulation, 4 B/px of
 // compulsory HBM traffic).  kFuse stages run per launch on a shared-memory tile with a 2*kFuse
-// apron; the frame itself (7.9 MB at the harness size) stays L2-resident between launches.
+// apron (a chain whose length is not a multiple of kFuse ends with one shorter launch); the frame
+// itself (7.9 MB at the harness size) stays L2-resident between launches.
 #include "hb_common.h"
 
 namespace {
 
-constexpr int kStages = 32;  // GeneratorParam `stencils` of the shipped app (generator :9)
-constexpr int kFuse = 4;     // stages per launch
-static_assert(kStages % kFuse == 0, "every launch runs kFuse stages");
-constexpr int kTile = 64;    // output tile edge per block
+constexpr int kStages = 32;     // GeneratorParam `stencils` of the shipped app (generator :9): stencil_chain's depth
+constexpr int kMaxStages = 100; // the range the generator declares for it is [1, 100]
+constexpr int kFuse = 4;        // stages per launch (the last launch of a chain may run fewer)
+constexpr int kTile = 64;       // output tile edge per block
 constexpr int kTileIn = kTile + 4 * kFuse;  // 80: input tile edge (2 px apron per fused stage, both sides)
 
 struct Plane {
@@ -120,6 +122,7 @@ struct StencilStages<EDGE, 0> {
 
 template<int FUSE>
 __global__ void __launch_bounds__(256) stencil_chain_window_kernel(Plane p) {
+    static_assert(FUSE >= 1 && FUSE <= kFuse, "the shared-memory tiles hold an input tile of kFuse stages at most");
     constexpr int IN = kTile + 4 * FUSE, INW = IN / 2;
     __shared__ uint32_t A[kTileIn * kPW];
     __shared__ uint32_t B[kTileIn * kPW];
@@ -172,9 +175,24 @@ const halide_filter_argument_t kArgs[2] = {
     {"input", halide_argument_kind_input_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
     {"output", halide_argument_kind_output_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
-}  // namespace
 
-extern "C" int stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
+// One launch of `fuse` stages (1..kFuse).  Every depth is the same kernel and carries the same name.
+void launch_window(int fuse, const Plane &p, cudaStream_t s) {
+    const dim3 grid((p.dst_w + kTile - 1) / kTile, (p.dst_h + kTile - 1) / kTile);
+    switch (fuse) {
+    case 1: HB_LAUNCH("stencil_chain_window", stencil_chain_window_kernel<1>, grid, 256, 0, s, p); break;
+    case 2: HB_LAUNCH("stencil_chain_window", stencil_chain_window_kernel<2>, grid, 256, 0, s, p); break;
+    case 3: HB_LAUNCH("stencil_chain_window", stencil_chain_window_kernel<3>, grid, 256, 0, s, p); break;
+    default: HB_LAUNCH("stencil_chain_window", stencil_chain_window_kernel<kFuse>, grid, 256, 0, s, p); break;
+    }
+}
+
+// The chain of S = `stencils` stages.  Launch plan: floor(S / kFuse) launches of kFuse stages, then, when S mod kFuse
+// is not 0, one launch of the remaining stages.  Launch k reads the region grown by Rin = 2 * (stages not yet run) and
+// writes it grown by Rout = Rin - 2 * (its stages); the last launch writes the output itself.  Putting the short launch
+// last keeps every intermediate apron, and with it the scratch (largest at launch 0: 2 * (S - kFuse)), as small as the
+// order allows.  S = 32 is stencil_chain: 8 launches of 4 stages.
+int run_stencil_chain(halide_buffer_t *input, int32_t stencils, halide_buffer_t *output) {
     int r;
     hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[1]}};
     if ((r = hb::check_args(args, 2))) return r;
@@ -188,11 +206,18 @@ extern "C" int stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
     if (input->dim[0].extent <= 0 || input->dim[1].extent <= 0) {
         return hb::fail(halide_error_code_access_out_of_bounds, "Input buffer input is empty");
     }
+    if (stencils < 1 || stencils > kMaxStages) {
+        return hb::fail(stencils < 1 ? halide_error_code_param_too_small : halide_error_code_param_too_large,
+                        "Parameter stencils is %d but must be in [1, %d]", (int)stencils, kMaxStages);
+    }
     if ((r = hb::acquire(args, 2))) return r;
 
+    const int S = stencils;
+    const int full = S / kFuse, rest = S % kFuse;
+    const int groups = full + (rest ? 1 : 0);
+
     // ping-pong buffers for the intermediate stages on their grown regions
-    const int groups = kStages / kFuse;
-    const int maxR = 2 * (kStages - kFuse);
+    const int maxR = groups > 1 ? 2 * (S - kFuse) : 0;
     hb::Scratch scratch;
     const int64_t bw = (W + 2 * maxR + 1) & ~(int64_t)1, bh = H + 2 * maxR;  // (even pitch: intermediate rows keep pixel pairs word-aligned)
     uint16_t *buf[2] = {nullptr, nullptr};
@@ -205,8 +230,9 @@ extern "C" int stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
     {
         hb::CallTimer timer(s);
         for (int g = 0; g < groups; g++) {
-            const int Rin = 2 * (kStages - g * kFuse);      // apron of the region this launch reads
-            const int Rout = Rin - 2 * kFuse;               // apron of the region it writes
+            const int F = g < full ? kFuse : rest;          // stages this launch runs
+            const int Rin = 2 * (S - g * kFuse);            // apron of the region this launch reads
+            const int Rout = Rin - 2 * F;                   // apron of the region it writes
             Plane p;
             p.dst_w = W + 2 * Rout;
             p.dst_h = H + 2 * Rout;
@@ -236,11 +262,21 @@ extern "C" int stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
             }
             p.src_words = ((reinterpret_cast<uintptr_t>(p.src) & 3) == 0 && (p.src_sy & 1) == 0) ? 1 : 0;
             p.dst_words = ((reinterpret_cast<uintptr_t>(p.dst) & 3) == 0 && (p.dst_sy & 1) == 0) ? 1 : 0;
-            dim3 grid((p.dst_w + kTile - 1) / kTile, (p.dst_h + kTile - 1) / kTile);
-            HB_LAUNCH("stencil_chain_window", stencil_chain_window_kernel<kFuse>, grid, 256, 0, s, p);
+            launch_window(F, p, s);
         }
     }
     return hb::finish(args, 2, "stencil_chain launch");
+}
+}  // namespace
+
+extern "C" int stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
+    return run_stencil_chain(input, kStages, output);
+}
+
+// stencil_chain with the stencils GeneratorParam as a run-time argument: what the generator built with stencils = S
+// computes, for S in [1, 100].  Buffer rules, error codes and the bounds query are stencil_chain's.
+extern "C" int halide_b200_stencil_chain_stencils(halide_buffer_t *input, int32_t stencils, halide_buffer_t *output) {
+    return run_stencil_chain(input, stencils, output);
 }
 HB_EXPORT_FILTER(stencil_chain, kArgs)
 HB_EXPORT_AUTO_SCHEDULE(stencil_chain, kArgs)

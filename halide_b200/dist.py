@@ -224,9 +224,13 @@ class InputHaloSharder:
         return self._run("nl_means", lambda bi, bo: filters.nl_means(bi, patch_size, search_area, sigma, bo), in_band,
                          frame_h, out_band, frame_h, patch_size=patch_size, search_area=search_area)
 
-    def stencil_chain(self, in_band, out_band, frame_h):
+    def stencil_chain(self, in_band, out_band, frame_h, stencils=32):
         from . import filters
-        return self._run("stencil_chain", lambda bi, bo: filters.stencil_chain(bi, bo), in_band, frame_h, out_band, frame_h)
+        if stencils == 32:
+            invoke = lambda bi, bo: filters.stencil_chain(bi, bo)  # noqa: E731
+        else:
+            invoke = lambda bi, bo: filters.stencil_chain_stencils(bi, stencils, bo)  # noqa: E731
+        return self._run("stencil_chain", invoke, in_band, frame_h, out_band, frame_h, stencils=stencils)
 
     def bilateral_grid(self, in_band, r_sigma, out_band, frame_h, s_sigma=8):
         from . import filters

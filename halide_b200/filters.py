@@ -99,6 +99,14 @@ def stencil_chain(input, output):
     return check(lib.stencil_chain(input.ptr, output.ptr))
 
 
+def stencil_chain_stencils(input, stencils, output):
+    """stencil_chain with the generator's stencils (the number of chained 5x5 stages, the depth of the chain and so the
+    reach of the filter: 2 * stencils px each way) chosen per call, 1 <= stencils <= 100: the result is what the generator
+    built with that stencils computes, bit for bit.  Buffers and error codes as stencil_chain; stencils = 32 is
+    stencil_chain itself."""
+    return check(lib.halide_b200_stencil_chain_stencils(input.ptr, ctypes.c_int32(stencils), output.ptr))
+
+
 def bilateral_grid(input, r_sigma, output):
     """apps/bilateral_grid/bilateral_grid_generator.cpp (s_sigma = 8), float32."""
     return check(lib.bilateral_grid(input.ptr, ctypes.c_float(r_sigma), output.ptr))

@@ -355,6 +355,15 @@ int halide_b200_local_laplacian_pyramid_levels(struct halide_buffer_t *input, in
  * on a frame_w x frame_h frame (the levels above it share one cooperative launch); -1 for arguments out of range. */
 int halide_b200_ll_last_own_level(int32_t frame_w, int32_t frame_h, int32_t pyramid_levels);
 
+/* stencil_chain with its stencils GeneratorParam S (the number of chained 5x5 stages, 32 in stencil_chain) as an argument:
+ * the result is what the generator built with stencils = S computes, bit for bit.  Stage s + 1 is the 5x5 stencil with
+ * weights (i+3)(j+3) in Z/2^16 applied to stage s; stage 0 is repeat_edge(input).  S must be in [1, 100] (else
+ * halide_error_code_param_too_small / _too_large, checked after the buffer checks, the bounds query and the empty-buffer
+ * handling, before any CUDA call); buffers (2-D uint16), error codes and the bounds query follow stencil_chain, which
+ * S == 32 runs.  The device scratch grows with S: two (W + 4S - 16) x (H + 4S - 16) uint16 planes from S = 9 up (one
+ * from S = 5 to 8, none below 5). */
+int halide_b200_stencil_chain_stencils(struct halide_buffer_t *input, int32_t stencils, struct halide_buffer_t *output);
+
 /* Host-only probe of the band geometry for tests: with level jr gathered, out[j*8..j*8+7] = {own.lo, own.hi, d.lo, d.hi,
  * u.lo, u.hi, S.lo, S.hi} per pyramid level j = 0..7 (rows owned in the gather partition / Gaussian-side rows computed and
  * held / outGPyramid rows needed / the level's rows on the whole frame), out[64..65] = input rows read. */
