@@ -206,10 +206,12 @@ int copy_nd(uint8_t *dst, const uint8_t *src, CopyDim *dims, int n, size_t eb, c
     for (int i = 0; i < n; i++) {
         if (dims[i].extent <= 0) return 0;
     }
-    // drop unit dimensions, sort by destination stride (insertion sort; n <= 4 in practice)
+    // drop unit dimensions and those of stride 0 on both sides (a broadcast buffer's device copy is laid out like its host
+    // memory: every index of such a dimension is the same bytes, copied once), sort by destination stride (insertion
+    // sort; n <= 4 in practice)
     int m = 0;
     for (int i = 0; i < n; i++) {
-        if (dims[i].extent != 1) dims[m++] = dims[i];
+        if (dims[i].extent != 1 && (dims[i].sstride != 0 || dims[i].dstride != 0)) dims[m++] = dims[i];
     }
     for (int i = 1; i < m; i++) {
         CopyDim d = dims[i];

@@ -831,6 +831,9 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
 
     cudaStream_t s = hb::stream();
     if ((r = get_lut(p, s))) return r;
+    // A halo pack that fails is reported only once the call is over: every rank still enters each exchange of the call,
+    // so that no neighbour is left waiting for this one.
+    cudaError_t pack_err = cudaSuccess;
     {
         hb::CallTimer timer(s);
         // pack my boundary rows per channel ([c][row][w], the layout of the receiver's halo arrays) and exchange — on a
@@ -854,18 +857,27 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
                 cudaEventRecord(ev_in, s);
                 cudaStreamWaitEvent(xs, ev_in, 0);
             }
+            // `rows` rows from `src` on, packed [row][w]: one 2-D copy when they run forward at least a row apart, else row
+            // by row (a flipped or zero row stride, which cudaMemcpy2D's unsigned pitch cannot express; a few rows each)
+            auto pack = [&](uint16_t *dst, const uint16_t *src, int rows) {
+                if (p.f.in_sy >= p.f.in_w) {
+                    return cudaMemcpy2DAsync(dst, rowb, src, (size_t)p.f.in_sy * sizeof(uint16_t), rowb, rows, cudaMemcpyDeviceToDevice, xs);
+                }
+                for (int i = 0; i < rows; i++) {
+                    cudaError_t e = cudaMemcpyAsync(dst + (size_t)i * p.f.in_w, src + (int64_t)i * p.f.in_sy, rowb, cudaMemcpyDeviceToDevice, xs);
+                    if (e != cudaSuccess) return e;
+                }
+                return cudaSuccess;
+            };
             hbdist::Msg msgs[4];
             int n = 0;
+            auto keep_first = [&](cudaError_t e) {
+                if (pack_err == cudaSuccess) pack_err = e;
+            };
             for (int c = 0; c < C; c++) {
                 const uint16_t *plane = p.f.in + (int64_t)c * p.f.in_sc;
-                if (up_need) {
-                    cudaMemcpy2DAsync(send_up + (size_t)c * up_need * p.f.in_w, rowb, plane, (size_t)p.f.in_sy * sizeof(uint16_t), rowb,
-                                      up_need, cudaMemcpyDeviceToDevice, xs);
-                }
-                if (dn_need) {
-                    cudaMemcpy2DAsync(send_dn + (size_t)c * dn_need * p.f.in_w, rowb, plane + (int64_t)(p.f.in_h - dn_need) * p.f.in_sy,
-                                      (size_t)p.f.in_sy * sizeof(uint16_t), rowb, dn_need, cudaMemcpyDeviceToDevice, xs);
-                }
+                if (up_need) keep_first(pack(send_up + (size_t)c * up_need * p.f.in_w, plane, up_need));
+                if (dn_need) keep_first(pack(send_dn + (size_t)c * dn_need * p.f.in_w, plane + (int64_t)(p.f.in_h - dn_need) * p.f.in_sy, dn_need));
             }
             if (up_need) msgs[n++] = {send_up, (size_t)C * up_need * rowb, rank - 1, true};
             if (dn_need) msgs[n++] = {send_dn, (size_t)C * dn_need * rowb, rank + 1, true};
@@ -939,6 +951,10 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
         launch_up(p, jr, s);
         for (int j = jr - 1; j >= first_up_level(p); j--) launch_up(p, j, s);
         launch_final(p, s);
+    }
+    if (pack_err != cudaSuccess) {
+        cudaGetLastError();  // (the copy's error, reported here instead)
+        return hb::check_cuda(pack_err, "local_laplacian_sharded halo pack", halide_error_code_device_run_failed);
     }
     return hb::finish(args, 2, "local_laplacian_sharded launch");
 }
