@@ -5,8 +5,9 @@
 //   blur_d        = box sum of d over the patch (y then x)
 //   w             = fast_exp(blur_d * (-1 / (sigma^2 * patch^2)))
 //   out_c         = clamp( sum_{dy,dx} w * I_c(x+dx,y+dy) / sum_{dy,dx} w , 0, 1 )
-// Float pipeline: parity bar 1e-4 relative against oracle/oracle_nl_means.cpp (the box sums are
-// taken in the reference's order anyway: y then x, ascending).
+// Float pipeline, bit-exact against oracle/oracle_nl_means.cpp: both kernels perform its float operations in its order
+// (d over channels 0..2, the box sums y then x, ascending, search rows outer and dx inner, the same fast_exp, an IEEE
+// divide) and the library builds with --fmad=false (tests/test_nl_means_exact_gpu.py).
 //
 // Compute-bound (~1.5 kflop/px at patch 3 / search 7 against 24 algorithmic B/px): the frame is
 // read once into a shared-memory tile with its (search/2 + patch/2) apron, then for each search row
@@ -20,6 +21,13 @@
 namespace {
 
 constexpr int TX = 32, TY = 16;  // output tile per block; 256 threads, 2 rows per thread
+
+// clamp(v, 0, 1) as the generator's min / max evaluate it, NaN included: min(NaN, 1) = 1, then max(1, 0) = 1 (every
+// weight is NaN when sigma^2 * patch^2 underflows and -1 / it is -inf).  hl::clampf alone is not enough: ptxas folds
+// fmaxf(fminf(v, 1), 0) into FADD.SAT, which returns 0 for NaN.
+__device__ __forceinline__ float clamp01(float v) {
+    return v != v ? 1.0f : hl::clampf(v, 0.0f, 1.0f);
+}
 
 struct NLParams {
     const float *in;  // element at input mins
@@ -109,7 +117,7 @@ __global__ void __launch_bounds__(256) nl_means_kernel(NLParams q) {
         if (lx < q.W && ly < q.H) {
 #pragma unroll
             for (int c = 0; c < 3; c++) {
-                float v = hl::clampf(__fdiv_rn(acc[r][c], acc[r][3]), 0.0f, 1.0f);
+                float v = clamp01(__fdiv_rn(acc[r][c], acc[r][3]));
                 q.out[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = v;
             }
         }
@@ -196,7 +204,7 @@ __global__ void __launch_bounds__(256) nl_means_window_kernel(NLParams q) {
         if (lx < q.W && ly < q.H) {
 #pragma unroll
             for (int c = 0; c < 3; c++) {
-                const float v = hl::clampf(__fdiv_rn(acc[r][c], acc[r][3]), 0.0f, 1.0f);
+                const float v = clamp01(__fdiv_rn(acc[r][c], acc[r][3]));
                 q.out[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = v;
             }
         }

@@ -1,8 +1,8 @@
 // oracle/oracle_nl_means.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE (see oracle.h).
 //
 // CPU restatement of apps/nl_means/nl_means_generator.cpp:24-63, op order per SURVEY.md
-// Appendix B.  Parity status: UNPINNED by the reference.  Float pipeline: the CUDA path is
-// compared within 1e-4 relative.
+// Appendix B.  Parity status: UNPINNED by the reference.  Float pipeline: the CUDA path matches it
+// bit for bit; tests/test_nl_means_exact.py pins it against a float64 restatement.
 #include <vector>
 
 #include "halide_math.h"

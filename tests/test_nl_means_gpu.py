@@ -1,8 +1,12 @@
-"""GPU parity tests for nl_means through the C ABI.  Float pipeline: 1e-4 relative tolerance
-(BASELINE.json north_star) against oracle/oracle_nl_means.cpp."""
+"""GPU parity tests for nl_means through the C ABI against oracle/oracle_nl_means.cpp, within a 1e-4 relative tolerance
+(BASELINE.json north_star).  The kernels match the oracle bit for bit; test_nl_means_exact_gpu.py holds them to that, on
+content where every search offset carries weight.  Uniform noise in [0, 1) at sigma 0.12 is not such content (every
+off-centre weight is about exp(-35)), so the tests here that compare kernels with each other or at config 4's size use
+nl_means_exact.sensitive_frame."""
 import numpy as np
 import pytest
 
+from nl_means_exact import sensitive_frame
 from util import f32_frame
 
 pytestmark = pytest.mark.gpu
@@ -63,10 +67,10 @@ def test_constant_frame_4k_band(hb):
 
 
 def test_4k_random_frame_regions(hb, oracle):
-    """Config 4 size (3840 x 2160 x 3) on a RANDOM frame: regions of the full-size result against the oracle on the crop
-    that determines them (footprint = search/2 + patch/2 = 4 px; margin 16)."""
+    """Config 4 size (3840 x 2160 x 3) on a sensitive frame: regions of the full-size result against the oracle on the
+    crop that determines them (footprint = search/2 + patch/2 = 4 px; margin 16)."""
     h, w = 2160, 3840
-    inp = f32_frame((3, h, w), 33)
+    inp = sensitive_frame(3, h, w, 0.12, 33)
     got = run(hb, inp, 3, 7, 0.12)
     for (y0, x0) in [(0, 0), (h - 64, w - 64), (1000, 1900), (540 - 32, 3000)]:
         n, m = 64, 16
@@ -85,13 +89,14 @@ def test_generic_and_window_kernels(hb, oracle, variant):
     try:
         l.halide_b200_nl_means_variant(variant)
         for h, w in ((1, 1), (16, 32), (33, 47), (70, 101)):
-            inp = f32_frame((3, h, w), 11 * variant + h + w)
+            inp = sensitive_frame(3, h, w, 0.12, 11 * variant + h + w)
             close(run(hb, inp, 3, 7, 0.12), oracle.nl_means(inp, 3, 7, 0.12))
-        inp = f32_frame((3, 40, 52), 77)
+        inp = sensitive_frame(3, 40, 52, 0.12, 77)
         close(run(hb, inp, 7, 7, 0.12), oracle.nl_means(inp, 7, 7, 0.12))
+        inp = sensitive_frame(3, 40, 52, 0.3, 77)
         close(run(hb, inp, 5, 9, 0.3), oracle.nl_means(inp, 5, 9, 0.3))
         kw = dict(out_shape=(3, 30, 41), in_mins=(-4, 2, 0), out_mins=(1, 6, 0))
-        inp = f32_frame((3, 50, 70), 5)
+        inp = sensitive_frame(3, 50, 70, 0.12, 5)
         close(run(hb, inp, 3, 7, 0.12, **kw), oracle.nl_means(inp, 3, 7, 0.12, **kw))
     finally:
         l.halide_b200_nl_means_variant(0)
