@@ -319,7 +319,8 @@ constexpr int kHistCols = 4096;
 void choose_hist_block(BGSParams &q, int nb, int gw, int gh) {
     const int S = q.S;
     int cslots = std::max(1, std::min(256 / nb, kHistCols / S));
-    while (cslots > 1 && (int64_t)gh * ((gw + cslots - 1) / cslots) < 2 * 132) cslots = (cslots + 1) / 2;
+    const int64_t min_blocks = 2 * (int64_t)hb::sm_count();
+    while (cslots > 1 && (int64_t)gh * ((gw + cslots - 1) / cslots) < min_blocks) cslots = (cslots + 1) / 2;
     int k = std::max(1, (256 + cslots * S - 1) / (cslots * S));
     while (k > 1 && (cslots * k * S > kHistCols || (size_t)cslots * k * nb * sizeof(float2) > 64 * 1024)) k--;
     q.cslots = cslots;
@@ -461,9 +462,9 @@ inline int fdiv(int a, int b) {  // floor division, b > 0
     return (a % b != 0 && a < 0) ? q - 1 : q;
 }
 
-}  // namespace
-
-extern "C" int bilateral_grid(halide_buffer_t *input, float r_sigma, halide_buffer_t *output) {
+// bilateral_grid with cell size s_sigma (the generator's GeneratorParam): the shipped S runs bg_hist_blurz, bg_blur_xy
+// and bg_slice; every other cell size runs bg_hist_blurz_s, bg_blur_xy and bg_slice_s.
+int run_bilateral_grid(halide_buffer_t *input, int s_sigma, float r_sigma, halide_buffer_t *output) {
     int r;
     hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[2]}};
     if ((r = hb::check_args(args, 2))) return r;
@@ -473,84 +474,10 @@ extern "C" int bilateral_grid(halide_buffer_t *input, float r_sigma, halide_buff
     if ((r = hb::check_shapes(args, 2)) || (r = hb::check_required(args, need, 2))) return r;
     const int W = output->dim[0].extent, H = output->dim[1].extent;
     if (W <= 0 || H <= 0) return 0;
-    if (!(r_sigma > 0.0f)) {
-        return hb::fail(halide_error_code_param_too_small, "Parameter r_sigma is %g but must be positive", (double)r_sigma);
-    }
-    BGParams p;
-    p.inv_r = 1.0f / r_sigma;
-    p.zmax = (int)(1.0f * p.inv_r + 0.5f);
-    p.nz = p.zmax + 2;
-    const size_t bins_bytes = (size_t)(p.zmax + 1) * 2 * 128 * sizeof(float);
-    if (bins_bytes > 200 * 1024) {
-        return hb::fail(halide_error_code_param_too_small,
-                        "Parameter r_sigma is %g: more than %d intensity bins are not supported by this build",
-                        (double)r_sigma, (int)(200 * 1024 / (2 * 128 * sizeof(float))));
-    }
-    if ((r = hb::acquire(args, 2))) return r;
-
-    const int ox = output->dim[0].min, oy = output->dim[1].min;
-    p.in = (const float *)args[0].dev;
-    p.in_sy = input->dim[1].stride;
-    p.in_x0 = input->dim[0].min; p.in_y0 = input->dim[1].min;
-    p.in_w = input->dim[0].extent; p.in_h = input->dim[1].extent;
-    p.out = (float *)args[1].dev;
-    p.out_sy = output->dim[1].stride;
-    p.out_x0 = ox; p.out_y0 = oy; p.W = W; p.H = H;
-    // cells the slice touches are xi..xi+1; blury/blurx add 2 cells on every side
-    p.gx0 = fdiv(ox, S) - 2;
-    p.gy0 = fdiv(oy, S) - 2;
-    p.gw = fdiv(ox + W - 1, S) + 1 + 2 - p.gx0 + 1;
-    p.gh = fdiv(oy + H - 1, S) + 1 + 2 - p.gy0 + 1;
-    hb::Scratch scratch;
-    const size_t gelems = (size_t)p.gw * p.gh * p.nz * 2;
-    p.grid_a = scratch.get<float>(gelems);
-    p.grid_b = scratch.get<float>(gelems);
-    if (!p.grid_a || !p.grid_b) return hb::fail(halide_error_code_device_malloc_failed, "bilateral_grid: scratch allocation failed");
-
-    cudaStream_t s = hb::stream();
-    {
-        hb::CallTimer timer(s);
-        static hb::PerDeviceOnce hist_attr;
-        if (bins_bytes > 48 * 1024) {
-            hist_attr.run([] { cudaFuncSetAttribute(bg_hist_blurz_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); });
-        }
-        dim3 g1((p.gw + 63) / 64, p.gh);
-        HB_LAUNCH("bg_hist_blurz", bg_hist_blurz_kernel, g1, 128, bins_bytes, s, p);
-        const int V = p.nz * 2;
-        const int cols = (p.gw - 4) * V;
-        int rows = 16;
-        while (rows > 2 && (int64_t)((cols + 255) / 256) * ((p.gh - 4 + rows - 1) / rows) < 132 * 4) rows >>= 1;
-        dim3 g2((cols + 255) / 256, (p.gh - 4 + rows - 1) / rows);
-        HB_LAUNCH("bg_blur_xy", bg_blur_xy_kernel, g2, 256, 0, s, p, rows);
-        const int tx0 = ox & ~(S - 1), ty0 = oy & ~(S - 1);
-        dim3 g3((ox + W - tx0 + kSliceW - 1) / kSliceW, (oy + H - ty0 + S - 1) / S);
-        const size_t slice_smem = (size_t)p.nz * 2 * kSlicePitch * sizeof(float2);
-        if (slice_smem > 48 * 1024) cudaFuncSetAttribute(bg_slice_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)slice_smem);
-        HB_LAUNCH("bg_slice", bg_slice_kernel, g3, dim3(32, 8), slice_smem, s, p);
-    }
-    return hb::finish(args, 2, "bilateral_grid launch");
-}
-HB_EXPORT_FILTER(bilateral_grid, kArgs)
-HB_EXPORT_AUTO_SCHEDULE(bilateral_grid, kArgs)
-
-// bilateral_grid with the s_sigma GeneratorParam as a run-time argument: what the generator built with s_sigma = S
-// computes.  S = 8 is bilateral_grid itself (its kernels, bit for bit); every other S runs bg_hist_blurz_s, bg_blur_xy
-// and bg_slice_s.  Buffer rules, error codes and the bounds query are bilateral_grid's.
-extern "C" int halide_b200_bilateral_grid_s_sigma(halide_buffer_t *input, int32_t s_sigma, float r_sigma,
-                                                  halide_buffer_t *output) {
-    int r;
-    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[2]}};
-    if ((r = hb::check_args(args, 2))) return r;
-    const hb::Region need[2] = {hb::region_of(output, true), hb::region_of(output, false)};
-    if (hb::answer_bounds_query(args, need, 2)) return 0;
-    if ((r = hb::check_shapes(args, 2)) || (r = hb::check_required(args, need, 2))) return r;
-    const int W = output->dim[0].extent, H = output->dim[1].extent;
-    if (W <= 0 || H <= 0) return 0;
     if (s_sigma < 1 || s_sigma > 128) {
         return hb::fail(s_sigma < 1 ? halide_error_code_param_too_small : halide_error_code_param_too_large,
                         "Parameter s_sigma is %d but must be in [1, 128]", (int)s_sigma);
     }
-    if (s_sigma == S) return bilateral_grid(input, r_sigma, output);
     if (!(r_sigma > 0.0f)) {
         return hb::fail(halide_error_code_param_too_small, "Parameter r_sigma is %g but must be positive", (double)r_sigma);
     }
@@ -558,19 +485,12 @@ extern "C" int halide_b200_bilateral_grid_s_sigma(halide_buffer_t *input, int32_
     p.inv_r = 1.0f / r_sigma;
     p.zmax = (int)(1.0f * p.inv_r + 0.5f);
     p.nz = p.zmax + 2;
-    // the same bin limit as bilateral_grid: one 128-thread block of lane-private bins
     const size_t bins_bytes = (size_t)(p.zmax + 1) * 2 * 128 * sizeof(float);
     if (bins_bytes > 200 * 1024) {
         return hb::fail(halide_error_code_param_too_small,
                         "Parameter r_sigma is %g: more than %d intensity bins are not supported by this build",
                         (double)r_sigma, (int)(200 * 1024 / (2 * 128 * sizeof(float))));
     }
-    const int Ss = s_sigma;
-    BGSParams q;
-    q.S = Ss;
-    q.inv_s = (float)(1.0 / (double)Ss);
-    q.mag = (uint32_t)(((1u << kMagShift) + Ss - 1) / Ss);
-    choose_slice_tile(q, p.nz);
     if ((r = hb::acquire(args, 2))) return r;
 
     const int ox = output->dim[0].min, oy = output->dim[1].min;
@@ -582,11 +502,10 @@ extern "C" int halide_b200_bilateral_grid_s_sigma(halide_buffer_t *input, int32_
     p.out_sy = output->dim[1].stride;
     p.out_x0 = ox; p.out_y0 = oy; p.W = W; p.H = H;
     // cells the slice touches are xi..xi+1; blury/blurx add 2 cells on every side
-    p.gx0 = fdiv(ox, Ss) - 2;
-    p.gy0 = fdiv(oy, Ss) - 2;
-    p.gw = fdiv(ox + W - 1, Ss) + 1 + 2 - p.gx0 + 1;
-    p.gh = fdiv(oy + H - 1, Ss) + 1 + 2 - p.gy0 + 1;
-    choose_hist_block(q, p.zmax + 1, p.gw, p.gh);
+    p.gx0 = fdiv(ox, s_sigma) - 2;
+    p.gy0 = fdiv(oy, s_sigma) - 2;
+    p.gw = fdiv(ox + W - 1, s_sigma) + 1 + 2 - p.gx0 + 1;
+    p.gh = fdiv(oy + H - 1, s_sigma) + 1 + 2 - p.gy0 + 1;
     hb::Scratch scratch;
     const size_t gelems = (size_t)p.gw * p.gh * p.nz * 2;
     p.grid_a = scratch.get<float>(gelems);
@@ -596,26 +515,57 @@ extern "C" int halide_b200_bilateral_grid_s_sigma(halide_buffer_t *input, int32_
     cudaStream_t s = hb::stream();
     {
         hb::CallTimer timer(s);
-        static hb::PerDeviceOnce hist_attr, slice_attr;
-        const size_t hist_bytes = hist_s_bytes(q, p.zmax + 1);
-        if (hist_bytes > 48 * 1024) {
-            hist_attr.run([] { cudaFuncSetAttribute(bg_hist_blurz_s_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024); });
+        BGSParams q;  // (the any-S kernels' shapes)
+        if (s_sigma == S) {
+            hb::allow_smem(bg_hist_blurz_kernel, bins_bytes);
+            dim3 g1((p.gw + 63) / 64, p.gh);
+            HB_LAUNCH("bg_hist_blurz", bg_hist_blurz_kernel, g1, 128, bins_bytes, s, p);
+        } else {
+            q.S = s_sigma;
+            q.inv_s = (float)(1.0 / (double)s_sigma);
+            q.mag = (uint32_t)(((1u << kMagShift) + s_sigma - 1) / s_sigma);
+            choose_slice_tile(q, p.nz);
+            choose_hist_block(q, p.zmax + 1, p.gw, p.gh);
+            const size_t hist_bytes = hist_s_bytes(q, p.zmax + 1);
+            hb::allow_smem(bg_hist_blurz_s_kernel, hist_bytes);
+            dim3 g1(p.gh, (p.gw + q.cpb - 1) / q.cpb);
+            HB_LAUNCH("bg_hist_blurz_s", bg_hist_blurz_s_kernel, g1, 256, hist_bytes, s, p, q);
         }
-        dim3 g1(p.gh, (p.gw + q.cpb - 1) / q.cpb);
-        HB_LAUNCH("bg_hist_blurz_s", bg_hist_blurz_s_kernel, g1, 256, hist_bytes, s, p, q);
         const int V = p.nz * 2;
         const int cols = (p.gw - 4) * V;
+        const int64_t min_blocks = (int64_t)hb::sm_count() * 4;
         int rows = 16;
-        while (rows > 2 && (int64_t)((cols + 255) / 256) * ((p.gh - 4 + rows - 1) / rows) < 132 * 4) rows >>= 1;
+        while (rows > 2 && (int64_t)((cols + 255) / 256) * ((p.gh - 4 + rows - 1) / rows) < min_blocks) rows >>= 1;
         dim3 g2((cols + 255) / 256, (p.gh - 4 + rows - 1) / rows);
         HB_LAUNCH("bg_blur_xy", bg_blur_xy_kernel, g2, 256, 0, s, p, rows);
-        const int tw = 4 * q.tx, tx0 = ox & ~3;
-        dim3 g3((H + q.th - 1) / q.th, (ox + W - tx0 + tw - 1) / tw);
-        const size_t slice_smem = slice_s_bytes(q, p.nz);
-        if (slice_smem > 48 * 1024) {
-            slice_attr.run([] { cudaFuncSetAttribute(bg_slice_s_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSliceMaxSmem); });
+        if (s_sigma == S) {
+            const int tx0 = ox & ~(S - 1), ty0 = oy & ~(S - 1);
+            dim3 g3((ox + W - tx0 + kSliceW - 1) / kSliceW, (oy + H - ty0 + S - 1) / S);
+            const size_t slice_smem = (size_t)p.nz * 2 * kSlicePitch * sizeof(float2);
+            hb::allow_smem(bg_slice_kernel, slice_smem);
+            HB_LAUNCH("bg_slice", bg_slice_kernel, g3, dim3(32, 8), slice_smem, s, p);
+        } else {
+            const int tw = 4 * q.tx, tx0 = ox & ~3;
+            dim3 g3((H + q.th - 1) / q.th, (ox + W - tx0 + tw - 1) / tw);
+            const size_t slice_smem = slice_s_bytes(q, p.nz);
+            hb::allow_smem(bg_slice_s_kernel, slice_smem);
+            HB_LAUNCH("bg_slice_s", bg_slice_s_kernel, g3, 256, slice_smem, s, p, q);
         }
-        HB_LAUNCH("bg_slice_s", bg_slice_s_kernel, g3, 256, slice_smem, s, p, q);
     }
     return hb::finish(args, 2, "bilateral_grid launch");
+}
+
+}  // namespace
+
+extern "C" int bilateral_grid(halide_buffer_t *input, float r_sigma, halide_buffer_t *output) {
+    return run_bilateral_grid(input, S, r_sigma, output);
+}
+HB_EXPORT_FILTER(bilateral_grid, kArgs)
+HB_EXPORT_AUTO_SCHEDULE(bilateral_grid, kArgs)
+
+// bilateral_grid with the s_sigma GeneratorParam as a run-time argument, in [1, 128].  S = 8 runs bilateral_grid's own
+// kernels (bit for bit).  Buffer rules, error codes and the bounds query are bilateral_grid's.
+extern "C" int halide_b200_bilateral_grid_s_sigma(halide_buffer_t *input, int32_t s_sigma, float r_sigma,
+                                                  halide_buffer_t *output) {
+    return run_bilateral_grid(input, s_sigma, r_sigma, output);
 }

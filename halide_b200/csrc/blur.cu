@@ -326,11 +326,11 @@ extern "C" int halide_blur(halide_buffer_t *input, halide_buffer_t *blur_y) {
     a.in_lo = lo - origin;
     a.in_hi = hi - origin;
 
-    // Enough warps to cover the 132 SMs of an H100 a few times over, but strips tall enough to amortise the
-    // two-row vertical apron.
+    // Enough warps to cover the SMs a few times over, but strips tall enough to amortise the two-row vertical apron.
     int strips_x = (w + kStripW - 1) / kStripW;
     int rows = 32;
-    while (rows > 4 && (int64_t)strips_x * ((h + rows - 1) / rows) < 132 * 8) rows >>= 1;
+    const int64_t min_warps = (int64_t)hb::sm_count() * 8;
+    while (rows > 4 && (int64_t)strips_x * ((h + rows - 1) / rows) < min_warps) rows >>= 1;
     a.rows_per_warp = rows;
     int warps_y = (h + rows - 1) / rows;
     dim3 grid(strips_x, (warps_y + kWarpsPerBlock - 1) / kWarpsPerBlock);
@@ -343,16 +343,8 @@ extern "C" int halide_blur(halide_buffer_t *input, halide_buffer_t *blur_y) {
         hb::CallTimer timer(s);
         if (pair_ok) {
             // strips of 128 columns; height such that the strips fill the resident warps a whole number of times
-            static int resident = 0;  // blocks per SM x SMs (per process: one device per process)
-            if (!resident) {
-                int per_sm = 0, dev = 0, sms = 0;
-                cudaGetDevice(&dev);
-                cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-                cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, blur3x3_u16_quad_kernel<6>, 32 * kQuadWarps, 0);
-                resident = (per_sm > 0 ? per_sm : 8) * (sms > 0 ? sms : 132);
-            }
             const int sxq = (w + kQuadW - 1) / kQuadW;
-            const int64_t slots = (int64_t)resident * kQuadWarps;
+            const int64_t slots = (int64_t)hb::resident_blocks(blur3x3_u16_quad_kernel<6>, 32 * kQuadWarps, 0) * kQuadWarps;
             int qrows = 8;
             for (int m = 1; m <= 64; m++) {
                 const int64_t sy = m * slots / sxq;

@@ -353,8 +353,7 @@ bool make_map(CUtensorMap *m, void *base, uint64_t rows, uint32_t box_rows, uint
 template<int TN, bool FOLD>
 void launch_any(unsigned grid, cudaStream_t s, const CUtensorMap &ma_hi, const CUtensorMap &ma_lo, const CUtensorMap &mb_hi,
                 const CUtensorMap &mb_lo, const ConvShape &sh, const float *bias, float *out) {
-    static hb::PerDeviceOnce attr;
-    attr.run([] { cudaFuncSetAttribute(conv_layer_tc_any_kernel<TN, FOLD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(TN)); });
+    hb::allow_smem(conv_layer_tc_any_kernel<TN, FOLD>, smem_bytes(TN));
     HB_LAUNCH(TN == 128 ? (FOLD ? "conv_layer_tc_n128_fold" : "conv_layer_tc_n128") : (FOLD ? "conv_layer_tc_n64_fold" : "conv_layer_tc_n64"),
               (conv_layer_tc_any_kernel<TN, FOLD>), grid, THREADS_ANY, smem_bytes(TN), s, ma_hi, ma_lo, mb_hi, mb_lo, sh, bias, out);
 }
@@ -374,8 +373,7 @@ int conv_layer_tc_run(const float *din, const float *df, const float *db, float 
         !make_map(&mb_lo, b_lo, 9 * CO, TILE_N)) {
         return hb::fail(halide_error_code_generic_error, "conv_layer: cuTensorMapEncodeTiled failed");
     }
-    static hb::PerDeviceOnce attr;
-    attr.run([] { cudaFuncSetAttribute(conv_layer_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(TILE_N)); });
+    hb::allow_smem(conv_layer_tc_kernel, smem_bytes(TILE_N));
     HB_LAUNCH("conv_split_input", conv_split_input_kernel, (unsigned)((a_elems / 4 + 255) / 256), 256, 0, s, (const float4 *)din, (float4 *)a_hi,
               (float4 *)a_lo, a_elems / 4);
     HB_LAUNCH("conv_prep_filter", conv_prep_filter_kernel, (unsigned)((b_elems + 255) / 256), 256, 0, s, df, b_hi, b_lo);

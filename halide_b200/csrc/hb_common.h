@@ -40,20 +40,25 @@ struct CallTimer {
     cudaStream_t s;
 };
 
-// ---- once-per-device set-up (function attributes are per device / context; keyed by the CURRENT device, and safe
-// to race: two threads at worst both run `fn`, which must be idempotent) -----------------------------------------
-struct PerDeviceOnce {
-    unsigned long long done = 0;  // bit d = device d set up (devices >= 64: always run fn)
-    template<typename F>
-    void run(F fn) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        const unsigned long long bit = dev < 64 ? 1ull << dev : 0ull;
-        if (bit && (__atomic_load_n(&done, __ATOMIC_ACQUIRE) & bit)) return;
-        fn();
-        if (bit) __atomic_fetch_or(&done, bit, __ATOMIC_RELEASE);
-    }
-};
+// ---- launch limits of the CURRENT device, cached per device (a process may drive several) ---------------------
+// A kernel launched with more than 48 KB of dynamic shared memory must first be allowed that much: allow_smem raises
+// the kernel's limit to at least `bytes`, never lowers it (calls of other sizes, from any thread, may rely on it) and
+// makes no driver call once the limit covers `bytes`.
+void allow_smem(const void *kernel, size_t bytes);
+// Blocks of the kernel that fit on the device at once with `threads` threads and `smem` bytes each: SMs x blocks per
+// SM (1 per SM if the occupancy query fails).  Allows `smem` first.  Cached per (kernel, device, smem): a kernel is
+// always launched with one block size.
+int resident_blocks(const void *kernel, int threads, size_t smem);
+template<typename F>
+void allow_smem(F *kernel, size_t bytes) {
+    allow_smem((const void *)kernel, bytes);
+}
+template<typename F>
+int resident_blocks(F *kernel, int threads, size_t smem) {
+    return resident_blocks((const void *)kernel, threads, smem);
+}
+int sm_count();
+bool cooperative_launch();  // whether the device takes cudaLaunchCooperativeKernel
 
 // ---- device scratch (callee-owned intermediates; pooled, src/runtime/cuda.cpp:760-870 analogue) ---
 void *scratch_alloc(size_t bytes);  // returns nullptr on failure (caller maps to -16)

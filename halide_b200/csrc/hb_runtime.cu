@@ -121,6 +121,43 @@ void prof_drain_locked() {
     g_prof_pending.clear();
 }
 
+// ---- launch limits ---------------------------------------------------------------------------
+// The driver queries behind them cost several microseconds each (a row-sharded local_laplacian frame is only ~17
+// short launches per rank), so every answer is kept.  One lock: loopback ranks are threads of one process.
+struct DeviceFacts {
+    int sms, coop;
+};
+struct KernelLimits {
+    size_t smem = 48 * 1024;         // dynamic shared memory the kernel is allowed (48 KB needs no opt-in)
+    std::map<size_t, int> resident;  // resident_blocks by dynamic shared-memory size
+};
+std::mutex g_limits_mu;
+std::map<int, DeviceFacts> g_devices;
+std::map<std::pair<const void *, int>, KernelLimits> g_kernels;  // by (kernel, device)
+
+int current_device() {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    return dev;
+}
+
+const DeviceFacts &device_facts_locked(int dev) {
+    auto it = g_devices.find(dev);
+    if (it != g_devices.end()) return it->second;
+    DeviceFacts f = {1, 0};  // (what a failed query leaves)
+    cudaDeviceGetAttribute(&f.sms, cudaDevAttrMultiProcessorCount, dev);
+    cudaDeviceGetAttribute(&f.coop, cudaDevAttrCooperativeLaunch, dev);
+    return g_devices[dev] = f;
+}
+
+KernelLimits &allow_smem_locked(const void *kernel, int dev, size_t bytes) {
+    KernelLimits &k = g_kernels[{kernel, dev}];
+    if (bytes > k.smem && cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) == cudaSuccess) {
+        k.smem = bytes;
+    }
+    return k;
+}
+
 // Span of a buffer in elements relative to the element at the mins: [lo, hi].
 void span_elems(const halide_buffer_t *b, int64_t *lo, int64_t *hi) {
     int64_t l = 0, h = 0;
@@ -510,6 +547,39 @@ CallTimer::~CallTimer() {
         cudaEventRecord(t_call_e1, s);
         t_call_valid = true;
     }
+}
+
+void allow_smem(const void *kernel, size_t bytes) {
+    if (bytes <= 48 * 1024) return;
+    const int dev = current_device();
+    std::lock_guard<std::mutex> lock(g_limits_mu);
+    allow_smem_locked(kernel, dev, bytes);
+}
+
+int resident_blocks(const void *kernel, int threads, size_t smem) {
+    const int dev = current_device();
+    std::lock_guard<std::mutex> lock(g_limits_mu);
+    KernelLimits &k = allow_smem_locked(kernel, dev, smem);
+    auto it = k.resident.find(smem);
+    if (it != k.resident.end()) return it->second;
+    int per_sm = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem) != cudaSuccess || per_sm < 1) {
+        cudaGetLastError();
+        per_sm = 1;
+    }
+    return k.resident[smem] = device_facts_locked(dev).sms * per_sm;
+}
+
+int sm_count() {
+    const int dev = current_device();
+    std::lock_guard<std::mutex> lock(g_limits_mu);
+    return device_facts_locked(dev).sms;
+}
+
+bool cooperative_launch() {
+    const int dev = current_device();
+    std::lock_guard<std::mutex> lock(g_limits_mu);
+    return device_facts_locked(dev).coop != 0;
 }
 
 void *scratch_alloc(size_t bytes) {

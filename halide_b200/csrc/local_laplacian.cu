@@ -7,7 +7,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <map>
 #include <mutex>
 #include <vector>
 
@@ -236,38 +235,6 @@ int alloc_levels(P &p, const ll::Geom &geom, hb::Scratch &scratch) {
 const dim3 kBlk(32, 8);
 dim3 grid_for(int w, int h) { return dim3((w + 31) / 32, (h + 7) / 8); }
 
-// Resident block slots of a kernel on the current device.  The driver queries behind it (function attribute,
-// occupancy) cost several microseconds each — a sharded frame is only ~17 short launches per rank — so
-// the answer is cached per (kernel, device, shared-memory size); a process may drive several devices.
-struct SlotKey {
-    const void *kern;
-    int dev;
-    size_t smem;
-    bool operator<(const SlotKey &o) const {
-        return kern != o.kern ? kern < o.kern : (dev != o.dev ? dev < o.dev : smem < o.smem);
-    }
-};
-std::mutex g_slots_mu;
-std::map<SlotKey, int> g_slots;
-
-template<typename Kern>
-int resident_slots(Kern kern, int threads, size_t smem) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    const SlotKey key = {(const void *)kern, dev, smem};
-    std::lock_guard<std::mutex> lock(g_slots_mu);
-    auto it = g_slots.find(key);
-    if (it != g_slots.end()) return it->second;
-    int sms = 132, per_sm = 0;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem) != cudaSuccess || per_sm < 1) {
-        cudaGetLastError();
-        per_sm = 1;
-    }
-    return g_slots[key] = sms * per_sm;
-}
-
 // Levels 1 and 2 from the frame (K == 8): stores level-1 rows cy1 and level-2 rows cy2, reading the frame through f
 // (the row-sharded path narrows both spans, and hides the halo rows from the launch that runs before they arrive).
 template<bool BETA1, bool FRAMES, bool IL, typename T>
@@ -278,7 +245,7 @@ void launch_level12_kernel(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2
     // one pair table and a stage per strip walker (warp pair or warp): one block per SM
     constexpr int pairs = kL1Walkers<FRAMES, T>;
     const size_t smem = kPairLutN * sizeof(float2) + pairs * sizeof(DownStage);
-    const int slots = resident_slots(ll_level1_kernel<BETA1, FRAMES, T, IL>, kDWarps * 32, smem);
+    const int slots = hb::resident_blocks(ll_level1_kernel<BETA1, FRAMES, T, IL>, kDWarps * 32, smem);
     // strips of 28 level-1 columns from xbase == xo (mod 4), far enough left that their level-2 columns (xbase/2 + 14k ..)
     // reach level 2's first column; chunks of 8 level-1 rows from an odd ybase, over the rows stored and the taps of
     // the level-2 rows stored
@@ -353,7 +320,7 @@ void launch_down(PlanT<T> &p, int j, cudaStream_t s) {  // produce level j (j >=
             const int ns = (lb[j].sx.n() + kRCols - 1) / kRCols, ng = (lb[j].cy.n() + kRG - 1) / kRG;
             const long long tasks = (long long)ns * ng * 5 * p.N;
             auto kern = p.N > 1 ? ll_down_rows_kernel<true> : ll_down_rows_kernel<false>;
-            const int slots = resident_slots(kern, 256, 0);
+            const int slots = hb::resident_blocks(kern, 256, 0);
             long long g = (tasks + 7) / 8;
             if (g > slots) g = slots;
             HB_LAUNCH("ll_down_rows", kern, (int)g, 256, 0, s, lb[j - 1], lb[j], ns, ng, p.N, fs_slot(p, j), p.fs);
@@ -466,7 +433,7 @@ void launch_final(PlanT<T> &p, cudaStream_t s) {
             auto launch = [&](auto kern, bool tma_on, int samples = 3) {
                 const int smem = up2_smem_bytes(true, tma_on, (int)sizeof(T), samples);
                 const dim3 g = up_grid(f.out_x0, f.out_x0 + f.W - 1, f.out_y0, f.out_y0 + f.H - 1, nf);
-                (void)resident_slots(kern, 256, smem);  // (sets the > 48 KB shared-memory attribute once per kernel and device)
+                hb::allow_smem(kern, smem);
                 HB_LAUNCH("ll_final2", kern, g, 256, smem, s, fg, at_frame(lb[1], 1, p.fs, n0), at_frame(lb[2], 2, p.fs, n0), in_map, 1,
                           p.fs);
             };
@@ -504,30 +471,14 @@ void launch_final(PlanT<T> &p, cudaStream_t s) {
 // Coarse tail in one cooperative launch: levels j0+1 .. J-1 down and up (see ll_coarse_fused_kernel).
 template<typename P>
 bool launch_coarse_fused(P &p, int j0, cudaStream_t s) {
-    int dev = 0, coop = 0;
-    cudaGetDevice(&dev);
-    static std::map<int, int> coop_ok;  // per device (guarded by g_slots_mu)
-    {
-        std::lock_guard<std::mutex> lock(g_slots_mu);
-        auto it = coop_ok.find(dev);
-        if (it == coop_ok.end()) {
-            cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
-            coop_ok[dev] = coop;
-        } else {
-            coop = it->second;
-        }
-    }
+    if (!hb::cooperative_launch()) return false;
     // J <= 8: the LevelSet instantiations, on the first 8 slots; a deeper pyramid (one frame) takes all of LevelSetDeep
     LevelSet ls8;
     memcpy(ls8.lv, p.ls.lv, sizeof ls8.lv);
     const bool deep = p.J > ll::kMaxJ;
     const void *kern = deep ? (const void *)ll_coarse_fused_kernel<false, LevelSetDeep>
                             : (p.N > 1 ? (const void *)ll_coarse_fused_kernel<true> : (const void *)ll_coarse_fused_kernel<false>);
-    const int slots = resident_slots(kern, 256, 0);  // sms * blocks per SM
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const int max_blocks = coop ? (slots > 2 * sms ? 2 * sms : slots) : 0;
-    if (max_blocks <= 0) return false;
+    const int max_blocks = std::min(hb::resident_blocks(kern, 256, 0), 2 * hb::sm_count());
     int J = p.J, K = p.f.levels, levels = p.f.levels, jd = fast_down(p) && j0 < 2 ? 2 : j0, nf = p.N;
     float flm1 = p.f.flm1;
     void *args[] = {deep ? (void *)&p.ls : (void *)&ls8, &J, &j0, &jd, &K, &flm1, &levels, &nf, &p.fs};
@@ -584,7 +535,7 @@ void launch_tone(Plan &p, cudaStream_t s) {
                      a16(f.out_sy * 2) && a16(f.out_sc * 2) && !(g_force_naive & 16);
     const size_t smem = (size_t)(2 * f.lut_half + 1) * sizeof(float);
     auto kern = vec ? ll_tone_kernel<true> : ll_tone_kernel<false>;
-    const int slots = resident_slots(kern, 256, smem);  // (also sets the > 48 KB shared-memory attribute: levels > 24)
+    const int slots = hb::resident_blocks(kern, 256, smem);  // (smem is above 48 KB for levels > 24)
     const int g = (int)std::min<long long>(slots, (units + 255) / 256);
     HB_LAUNCH("ll_tone", kern, g, 256, smem, s, f, upr, units);
 }

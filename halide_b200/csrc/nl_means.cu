@@ -287,8 +287,6 @@ extern "C" int nl_means(halide_buffer_t *input, int32_t patch_size, int32_t sear
     cudaStream_t s = hb::stream();
     {
         hb::CallTimer timer(s);
-        // (the limit is per device; setting it is cheap, so it is simply set for every call that needs it)
-        if (smem > 48 * 1024) cudaFuncSetAttribute(nl_means_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         dim3 grid((W + TX - 1) / TX, (H + TY - 1) / TY);
         const bool window = g_variant != 1;
         if (window && patch_size == 3 && search_area == 7) {
@@ -300,6 +298,7 @@ extern "C" int nl_means(halide_buffer_t *input, int32_t patch_size, int32_t sear
             static_assert(sm <= 48 * 1024, "no opt-in needed");
             HB_LAUNCH("nl_means_window", (nl_means_window_kernel<7, 7>), grid, 256, sm, s, q);
         } else {
+            hb::allow_smem(nl_means_kernel, smem);
             HB_LAUNCH("nl_means", nl_means_kernel, grid, 256, smem, s, q);
         }
     }

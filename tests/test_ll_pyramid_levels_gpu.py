@@ -136,6 +136,19 @@ def test_depth_1_runs_only_the_tone_kernel(hb):
     assert _names(hb, 1, 8, alpha) == {"ll_tone": 1}
 
 
+def test_depth_1_tables_above_48k_in_turn(hb, oracle):
+    """ll_tone stages the remap table, (2 * 256 * (levels - 1) + 1) floats, in shared memory: more than 48 KB at levels 30
+    and 26 alike.  The 26-level call must not leave the kernel's limit below what the following 30-level call needs.  (No
+    other test runs ll_tone at these level counts.)"""
+    img = u16_frame((3, 61, 83), 30)
+    for levels in (30, 26, 30):
+        alpha = 1.0 / (levels - 1)
+        with kernels_run(hb) as ran:
+            got = run(hb, img, 1, levels, alpha, 1.0)
+        assert "ll_tone" in ran, (levels, ran)
+        assert np.array_equal(got, want(oracle, img, 1, levels, alpha, 1.0)), levels
+
+
 def test_alternating_depths_leak_nothing(hb):
     img = u16_frame((3, 133, 201), 99)
     seq = [(1, 8), (14, 3), (2, 8), (8, 5), (20, 8), (3, 3), (1, 5), (11, 8), (2, 3)]
