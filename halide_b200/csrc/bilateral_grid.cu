@@ -5,8 +5,14 @@
 //   histogram(x,y,zi,c) += mux(c,{val,1}) over the 8x8 pixels of cell (x,y) (offset -4), zi = int(val/r_sigma + 0.5)
 //   blurz/blurx/blury: unnormalised 1-4-6-4-1 along z, x, y
 //   output = trilinear slice of blury at (x/8, y/8, val/r_sigma), channel 0 / channel 1
-// Float pipeline: parity bar is 1e-4 relative against oracle/oracle_bilateral_grid.cpp, so sums
-// may be re-associated (all terms are non-negative: no cancellation).
+// Float pipeline against oracle/oracle_bilateral_grid.cpp: the kernels perform the oracle's float operations in its order
+// (each bin summed rows, then columns; the same blur5 association; the lerp nest x -> y -> z; an IEEE divide; no
+// contraction: --fmad=false here, -ffp-contract=off there), and the input clamp maps NaN to 1 as Halide's select-based
+// min / max do (hl::clamp01).  So the any-S kernels are bit-exact on any input.  The one re-association is bg_hist_blurz
+// (S = 8): lanes 2c and 2c+1 each sum four columns of a cell and their sums are then added, which gives the oracle's bits
+// wherever every partial sum of a bin is exact (a uint16 frame / 65536: at most 64 terms of 16 bits), and stays within
+// 1e-4 relative on arbitrary float data (all terms are non-negative: no cancellation).
+// (tests/test_bilateral_grid_exact_gpu.py holds both bit for bit; tests/test_bilateral_grid_gpu.py S = 8 on noise.)
 //
 // HBM-bound: 8 algorithmic B/px (4 in + 4 out).  Three kernels:
 //   bg_hist_blurz   reads the frame once with coalesced float4 loads; each lane scatters its 4
@@ -73,7 +79,7 @@ __global__ void __launch_bounds__(128) bg_hist_blurz_kernel(BGParams p) {
         }
 #pragma unroll
         for (int i = 0; i < 4; i++) {
-            float val = hl::clampf(v[i], 0.0f, 1.0f);
+            float val = hl::clamp01(v[i]);
             int zi = (int)__fadd_rn(__fmul_rn(val, p.inv_r), 0.5f);
             zi = min(zi, p.zmax);
             s_bins[(zi * 2) * 128 + tid] += val;
@@ -180,7 +186,7 @@ __global__ void __launch_bounds__(256) bg_slice_kernel(BGParams p) {
     const float2 *c00 = s_grid + (lane & 15);  // cell (xi, yi) of this thread's four pixels; xi + 1: +1, yi + 1: +kSlicePitch
     const float yf = __fmul_rn((float)(y & (S - 1)), 0.125f);
     auto px = [&](float raw, int xx) -> float {
-        const float val = hl::clampf(raw, 0.0f, 1.0f);
+        const float val = hl::clamp01(raw);
         const float zv = __fmul_rn(val, p.inv_r);
         int zi = (int)zv;
         const float zf = __fsub_rn(zv, (float)zi);
@@ -270,7 +276,7 @@ __global__ void __launch_bounds__(256, 1) bg_hist_blurz_s_kernel(BGParams p, BGS
             const int y = hl::clampi(gy * S + r0 + r - S / 2, p.in_y0, p.in_y0 + p.in_h - 1) - p.in_y0;
             const float *row = p.in + (int64_t)y * p.in_sy;
             for (int c = tid; c < cols; c += 256) {
-                const float val = hl::clampf(__ldg(row + (hl::clampi(xb + c, xlo, xhi) - xlo)), 0.0f, 1.0f);
+                const float val = hl::clamp01(__ldg(row + (hl::clampi(xb + c, xlo, xhi) - xlo)));
                 int zi = (int)__fadd_rn(__fmul_rn(val, p.inv_r), 0.5f);
                 zi = min(zi, p.zmax);
                 const int cell = (int)(((uint32_t)c * q.mag) >> kMagShift);
@@ -380,7 +386,7 @@ __global__ void __launch_bounds__(256) bg_slice_s_kernel(BGParams p, BGSParams q
         const float *ip = p.in + (int64_t)(y - p.in_y0) * p.in_sy + (x - p.in_x0);
         float *op = p.out + (int64_t)(y - p.out_y0) * p.out_sy + (x - p.out_x0);
         auto px = [&](float raw, int i) -> float {
-            const float val = hl::clampf(raw, 0.0f, 1.0f);
+            const float val = hl::clamp01(raw);
             const float zv = __fmul_rn(val, p.inv_r);
             int zi = (int)zv;
             const float zf = __fsub_rn(zv, (float)zi);

@@ -22,13 +22,6 @@ namespace {
 
 constexpr int TX = 32, TY = 16;  // output tile per block; 256 threads, 2 rows per thread
 
-// clamp(v, 0, 1) as the generator's min / max evaluate it, NaN included: min(NaN, 1) = 1, then max(1, 0) = 1 (every
-// weight is NaN when sigma^2 * patch^2 underflows and -1 / it is -inf).  hl::clampf alone is not enough: ptxas folds
-// fmaxf(fminf(v, 1), 0) into FADD.SAT, which returns 0 for NaN.
-__device__ __forceinline__ float clamp01(float v) {
-    return v != v ? 1.0f : hl::clampf(v, 0.0f, 1.0f);
-}
-
 struct NLParams {
     const float *in;  // element at input mins
     int64_t in_sy, in_sc;
@@ -117,7 +110,8 @@ __global__ void __launch_bounds__(256) nl_means_kernel(NLParams q) {
         if (lx < q.W && ly < q.H) {
 #pragma unroll
             for (int c = 0; c < 3; c++) {
-                float v = clamp01(__fdiv_rn(acc[r][c], acc[r][3]));
+                // (NaN -> 1: every weight is NaN when sigma^2 * patch^2 underflows and -1 / it is -inf)
+                float v = hl::clamp01(__fdiv_rn(acc[r][c], acc[r][3]));
                 q.out[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = v;
             }
         }
@@ -204,7 +198,7 @@ __global__ void __launch_bounds__(256) nl_means_window_kernel(NLParams q) {
         if (lx < q.W && ly < q.H) {
 #pragma unroll
             for (int c = 0; c < 3; c++) {
-                const float v = clamp01(__fdiv_rn(acc[r][c], acc[r][3]));
+                const float v = hl::clamp01(__fdiv_rn(acc[r][c], acc[r][3]));
                 q.out[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = v;
             }
         }

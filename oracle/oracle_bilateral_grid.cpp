@@ -1,8 +1,12 @@
 // oracle/oracle_bilateral_grid.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE (see oracle.h).
 //
-// CPU restatement of apps/bilateral_grid/bilateral_grid_generator.cpp:17-67 (s_sigma = 8), op
+// CPU restatement of apps/bilateral_grid/bilateral_grid_generator.cpp:17-67 (any s_sigma), op
 // order per SURVEY.md Appendix B.  Parity status: UNPINNED by the reference (no golden output;
-// libHalide unbuildable here).  Float pipeline: the CUDA path is compared within 1e-4 relative.
+// libHalide unbuildable here); pinned instead to tests/bilateral_grid_exact.py's float64
+// restatement.  The clamp is Halide's select-based min / max (hl::clampf): NaN pixels become 1.
+// The CUDA path is compared bit for bit: the any-S kernels on any input, s_sigma = 8 wherever its
+// bin sums are exact (frames of multiples of 2^-16); only s_sigma = 8 on arbitrary float data is
+// compared within 1e-4 relative, because its histogram adds each bin as two 4-column partial sums.
 #include <algorithm>
 #include <vector>
 
