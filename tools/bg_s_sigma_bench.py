@@ -10,24 +10,14 @@ the algorithmic bytes (4 B read + 4 B written per pixel) and the bytes of one gr
 channels x 4 B; the histogram writes one, bg_blur_xy reads it and writes the second, the slice reads that).  The s_sigma = 8
 output must equal bilateral_grid's byte for byte.  The GPU's name, power limit and top SM clock are read in the same run.
 Writes OUT_DIR/bg_s_sigma_bench.json and prints one line per s_sigma."""
-import argparse
-import ctypes
-import json
-import os
 import statistics
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import torch
+
+import timing
+from halide_b200 import HalideBuffer, filters
 
 W, H, R_SIGMA = 7680, 4320, 0.1
-
-
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown (nvidia-smi failed)"
 
 
 def grid_shape(s, w=W, h=H, ox=0, oy=0, r_sigma=R_SIGMA):
@@ -41,43 +31,16 @@ def grid_shape(s, w=W, h=H, ox=0, oy=0, r_sigma=R_SIGMA):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("out_dir")
-    ap.add_argument("--window-ms", type=float, default=300.0)
-    ap.add_argument("--rounds", type=int, default=3)
+    ap = timing.common_args()
     ap.add_argument("--s", default="1,2,4,8,16,32,64,128")
     args = ap.parse_args()
     s_values = [int(v) for v in args.s.split(",")]
-
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("bg_s_sigma_bench needs a CUDA GPU")
-    torch.cuda.set_device(0)
-    import halide_b200
-    import halide_b200.lib as hlib
-    from halide_b200 import HalideBuffer, filters
-    l = halide_b200.load_library()
-    l.halide_b200_set_stream(ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-
-    def timed(fn, iters):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(iters):
-            fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / iters
+    timing.setup("bg_s_sigma_bench")
 
     def profile(fn):
-        hlib.profile(True)
-        hlib.profile_reset()
-        fn()
-        torch.cuda.synchronize()
-        prof = hlib.profile_report()
-        hlib.profile(False)
-        return {k: {"launches": c, "ms": t} for k, (c, t) in sorted(prof.items())}
+        return {k: {"launches": c, "ms": t} for k, (c, t) in sorted(timing.profile(fn).items())}
 
-    info = gpu_info()
+    info = timing.gpu_info()
     print(f"gpu: {info}", flush=True)
     gen = torch.Generator(device="cuda")
     gen.manual_seed(7680)
@@ -92,19 +55,12 @@ def main():
     for s in s_values:
         arms[f"s{s}"] = (lambda s=s: filters.bilateral_grid_s_sigma(bx, s, R_SIGMA, bouts[s]))
     arms["bilateral_grid"] = lambda: filters.bilateral_grid(bx, R_SIGMA, b_ref)
-    for fn in arms.values():
-        for _ in range(3):
-            fn()
-    torch.cuda.synchronize()
+    timing.warm_up(arms)
     same8 = None
     if 8 in outs:
         same8 = bool(torch.equal(outs[8].view(torch.int32), y_ref.view(torch.int32)))
         assert same8, "s_sigma = 8 differs from bilateral_grid"
-    iters = {k: max(3, int(args.window_ms / max(timed(fn, 3), 1e-3))) for k, fn in arms.items()}
-    ms = {k: [] for k in arms}
-    for _ in range(args.rounds):
-        for k, fn in arms.items():
-            ms[k].append(timed(fn, iters[k]))
+    iters, ms = timing.measure(arms, args.window_ms, args.rounds)
     med = {k: statistics.median(v) for k, v in ms.items()}
     if 8 in outs:
         assert torch.equal(outs[8].view(torch.int32), y_ref.view(torch.int32)), "s_sigma = 8 differs after timing"
@@ -125,11 +81,7 @@ def main():
         result["s_sigma"].append(entry)
         print(f"s_sigma {s}: {med[k]:.3f} ms (x{med[k] / med.get('s8', med['bilateral_grid']):.2f} of s_sigma 8), "
               f"grid {grid_bytes / 1e6:.1f} MB; " + ", ".join(f"{n} {v['ms']:.3f}" for n, v in prof.items()), flush=True)
-    os.makedirs(args.out_dir, exist_ok=True)
-    path = os.path.join(args.out_dir, "bg_s_sigma_bench.json")
-    with open(path, "w") as f:
-        json.dump(result, f, indent=1)
-    print(f"wrote {path}")
+    timing.write_json(args.out_dir, "bg_s_sigma_bench.json", result)
 
 
 if __name__ == "__main__":

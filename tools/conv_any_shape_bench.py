@@ -21,17 +21,16 @@ compute bound of the GEMM alone, which the split and re-lay kernels and a power 
 mean per-kernel times of 20 profiled calls, and the largest error over the derived float64 bound on signed data
 (tests/conv_any_exact.py: harness_bound).  The GPU's name, power limit and top SM clock are read in the same run.
 Writes OUT_DIR/conv_any_shape_bench.json and prints one line per shape.  Fails without a GPU."""
-import argparse
-import ctypes
-import json
 import os
 import statistics
-import subprocess
 import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
+import torch
+
+import timing
+from halide_b200 import HalideBuffer, filters
+
+sys.path.insert(0, os.path.join(timing.ROOT, "tests"))
 
 FIXED = (5, 128, 128, 100, 80)
 SHAPES = [FIXED, (1, 3, 64, 224, 224), (8, 64, 64, 56, 56), (8, 128, 128, 28, 28), (8, 256, 256, 14, 14), (32, 512, 512, 7, 7),
@@ -39,55 +38,20 @@ SHAPES = [FIXED, (1, 3, 64, 224, 224), (8, 64, 64, 56, 56), (8, 128, 128, 28, 28
 BOUND_TFLOPS = 495.0 / 3.0
 
 
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown (nvidia-smi failed)"
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("out_dir")
-    ap.add_argument("--window-ms", type=float, default=200.0)
-    ap.add_argument("--rounds", type=int, default=3)
-    args = ap.parse_args()
-
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("conv_any_shape_bench needs a CUDA GPU")
-    torch.cuda.set_device(0)
+    args = timing.common_args(window_ms=200.0).parse_args()
+    timing.setup("conv_any_shape_bench")
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     import numpy as np
     import conv_any_exact as cx
-    import halide_b200
-    import halide_b200.lib as hlib
-    from halide_b200 import HalideBuffer, filters
-    l = halide_b200.load_library()
-    l.halide_b200_set_stream(ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-
-    def timed(fn, iters):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(iters):
-            fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / iters
 
     def profile(fn, calls=20):
         """Microseconds per launch of each kernel, the mean over `calls` profiled calls (every launch bracketed by events,
         which keeps the kernels from overlapping: the times add up to more than an unprofiled call)."""
-        hlib.profile(True)
-        hlib.profile_reset()
-        for _ in range(calls):
-            fn()
-        torch.cuda.synchronize()
-        prof = hlib.profile_report()
-        hlib.profile(False)
-        return {k: round(t * 1e3 / c, 2) for k, (c, t) in sorted(prof.items())}
+        return {k: round(t * 1e3 / c, 2) for k, (c, t) in sorted(timing.profile(fn, calls).items())}
 
-    info = gpu_info()
+    info = timing.gpu_info()
     print(f"gpu: {info}", flush=True)
     result = {"gpu": info, "window_ms": args.window_ms, "rounds": args.rounds, "bound_tflops": BOUND_TFLOPS, "shapes": []}
     for shape in SHAPES:
@@ -106,20 +70,13 @@ def main():
         w_t = tf.permute(3, 0, 1, 2).contiguous(memory_format=torch.channels_last)
         b_t = tb.view(1, co, 1, 1)
         arms["torch"] = lambda: torch.relu_(torch.nn.functional.conv2d(x_t, w_t).add_(b_t))
-        for fn in arms.values():
-            for _ in range(3):
-                fn()
-        torch.cuda.synchronize()
+        timing.warm_up(arms)
         got = to.cpu().numpy()
         ratio = cx.worst_ratio(got, inp, filt, bias)
         assert np.isfinite(got).all() and ratio <= 1.0, (shape, ratio)
         if shape == FIXED:
             assert torch.equal(to.view(torch.int32), to_fixed.view(torch.int32)), "any_shape differs from conv_layer at its shape"
-        iters = {k: max(3, int(args.window_ms / max(timed(fn, 3), 1e-3))) for k, fn in arms.items()}
-        ms = {k: [] for k in arms}
-        for _ in range(args.rounds):
-            for k, fn in arms.items():
-                ms[k].append(timed(fn, iters[k]))
+        iters, ms = timing.measure(arms, args.window_ms, args.rounds)
         us = {k: statistics.median(v) * 1e3 for k, v in ms.items()}
         flop = 2.0 * 9 * ci * co * w * h * n
         tflops = flop / (us["any_shape"] * 1e-6) / 1e12
@@ -133,11 +90,7 @@ def main():
               f"3xTF32 bound; " + (f"conv_layer {us['conv_layer']:.1f} us; " if shape == FIXED else "") +
               f"torch fp32 {us['torch']:.1f} us; kernels " + ", ".join(f"{k} {v}" for k, v in entry["kernels_us"].items()) +
               f"; err/bound {ratio:.2f}", flush=True)
-    os.makedirs(args.out_dir, exist_ok=True)
-    path = os.path.join(args.out_dir, "conv_any_shape_bench.json")
-    with open(path, "w") as f:
-        json.dump(result, f, indent=1)
-    print(f"wrote {path}")
+    timing.write_json(args.out_dir, "conv_any_shape_bench.json", result)
 
 
 if __name__ == "__main__":

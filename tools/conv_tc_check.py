@@ -8,12 +8,12 @@ import json
 import os
 import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
+import numpy as np
+import torch
 
+import timing
+
+sys.path.insert(0, os.path.join(timing.ROOT, "tests"))
 import conv_exact  # noqa: E402
 import halide_b200 as hb  # noqa: E402
 from oracle import pyoracle  # noqa: E402
@@ -27,16 +27,14 @@ def time_call(calls=50):
     bi, bf, bb = (hb.HalideBuffer.from_torch(torch.rand(s, dtype=torch.float32, device=dev, generator=g))
                   for s in ((5, 82, 102, 128), (128, 3, 3, 128), (128,)))
     bo = hb.HalideBuffer.from_torch(torch.zeros((5, 80, 100, 128), dtype=torch.float32, device=dev))
+
+    def call():
+        hb.filters.conv_layer(bi, bf, bb, bo)
+
     for _ in range(5):
-        hb.filters.conv_layer(bi, bf, bb, bo)
+        call()
     torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(calls):
-        hb.filters.conv_layer(bi, bf, bb, bo)
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / calls * 1e3
+    return timing.timed(call, calls) * 1e3
 
 
 def rel_err(got, want):

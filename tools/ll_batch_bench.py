@@ -8,46 +8,23 @@ Every shape is warmed up first; each arm is then timed with CUDA events on one s
 window, batch and serial alternating, `rounds` times each.  The two arms' outputs are compared bit for bit at every timed
 size.  Writes OUT_DIR/ll_batch_bench.json (Mpx/s of both arms per round, and the per-kernel profile of one batch call)
 and prints one line per shape.  The GPU's name, power limit and top SM clock are read in the same run."""
-import argparse
-import ctypes
-import json
-import os
 import statistics
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import torch
+
+import timing
+from halide_b200 import HalideBuffer, filters
 
 SIZES = [(1920, 1080), (3840, 2160)]
 FRAMES = [1, 2, 4, 8]
 LEVELS, ALPHA, BETA = 8, 1.0 / 7.0, 1.0
 
 
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown (nvidia-smi failed)"
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("out_dir")
-    ap.add_argument("--window-ms", type=float, default=300.0)
-    ap.add_argument("--rounds", type=int, default=3)
-    args = ap.parse_args()
+    args = timing.common_args().parse_args()
+    timing.setup("ll_batch_bench")
 
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("ll_batch_bench needs a CUDA GPU")
-    torch.cuda.set_device(0)
-    import halide_b200
-    import halide_b200.lib as hlib
-    from halide_b200 import HalideBuffer, filters
-    l = halide_b200.load_library()
-    l.halide_b200_set_stream(ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-
-    info = gpu_info()
+    info = timing.gpu_info()
     print(f"gpu: {info}", flush=True)
     result = {"gpu": info, "levels": LEVELS, "alpha": ALPHA, "beta": BETA, "window_ms": args.window_ms,
               "rounds": args.rounds, "shapes": []}
@@ -68,34 +45,14 @@ def main():
                 for k in range(n):
                     filters.local_laplacian(si[k], LEVELS, ALPHA, BETA, so[k])
 
-            def timed(fn, iters):
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(iters):
-                    fn()
-                e1.record()
-                torch.cuda.synchronize()
-                return e0.elapsed_time(e1) / iters
-
-            for fn in (batch, serial):
-                for _ in range(3):
-                    fn()
-            torch.cuda.synchronize()
+            arms = {"batch": batch, "serial": serial}
+            timing.warm_up(arms)
             assert torch.equal(out_b, out_s), f"batch and serial outputs differ at {w}x{h} N={n}"
-            iters = {fn: max(3, int(args.window_ms / max(timed(fn, 3), 1e-3))) for fn in (batch, serial)}
-            ms = {"batch": [], "serial": []}
-            for _ in range(args.rounds):
-                ms["batch"].append(timed(batch, iters[batch]))
-                ms["serial"].append(timed(serial, iters[serial]))
+            iters, ms = timing.measure(arms, args.window_ms, args.rounds)
             assert torch.equal(out_b, out_s), f"batch and serial outputs differ at {w}x{h} N={n} after timing"
-            hlib.profile(True)
-            hlib.profile_reset()
-            batch()
-            torch.cuda.synchronize()
-            prof = hlib.profile_report()
-            hlib.profile(False)
+            prof = timing.profile(batch)
             mpx = n * w * h / 1e6
-            entry = {"w": w, "h": h, "n": n, "iters": {"batch": iters[batch], "serial": iters[serial]},
+            entry = {"w": w, "h": h, "n": n, "iters": iters,
                      "ms_per_call": ms, "mpx_s": {k: [mpx / (t / 1e3) for t in v] for k, v in ms.items()},
                      "median_mpx_s": {k: mpx / (statistics.median(v) / 1e3) for k, v in ms.items()},
                      "ms_per_frame_median": {k: statistics.median(v) / n for k, v in ms.items()},
@@ -107,11 +64,7 @@ def main():
                   f"({min(ms['serial']):.3f}-{max(ms['serial']):.3f} ms/call); profile "
                   + ", ".join(f"{k} {t:.3f}" for k, (c, t) in sorted(prof.items())), flush=True)
             del x, out_b, out_s, bi, bo, si, so
-    os.makedirs(args.out_dir, exist_ok=True)
-    path = os.path.join(args.out_dir, "ll_batch_bench.json")
-    with open(path, "w") as f:
-        json.dump(result, f, indent=1)
-    print(f"wrote {path}")
+    timing.write_json(args.out_dir, "ll_batch_bench.json", result)
 
 
 if __name__ == "__main__":

@@ -17,16 +17,12 @@ Every arm is warmed up, then timed with CUDA events over enough calls to fill th
 times each; the median round is reported.  The outputs of the three arms are compared bit for bit at every size.  Writes
 OUT_DIR/ll_interleaved_bench.json (ms per call of every round, and the per-kernel profile of one il and one planar call)
 and prints one line per case.  The GPU's name, power limit and top SM clock are read in the same run."""
-import argparse
-import ctypes
-import json
-import os
 import statistics
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import torch
+
+import timing
+from halide_b200 import HalideBuffer, filters
 
 SIZES = {"1080p": (1, 1920, 1080), "4k": (1, 3840, 2160), "16k": (1, 16384, 16384), "8x1080p": (8, 1920, 1080),
          "8x4k": (8, 3840, 2160)}
@@ -34,56 +30,18 @@ LAYOUTS = {"rgb": 3, "rgba": 4}  # input pixel pitch; the output is RGB (pitch 3
 LEVELS, ALPHA, BETA = 8, 1.0 / 7.0, 1.0
 
 
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown (nvidia-smi failed)"
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("out_dir")
-    ap.add_argument("--window-ms", type=float, default=300.0)
-    ap.add_argument("--rounds", type=int, default=3)
+    ap = timing.common_args()
     ap.add_argument("--sizes", default=",".join(SIZES))
     ap.add_argument("--types", default="u8,u16")
     ap.add_argument("--layouts", default=",".join(LAYOUTS))
     args = ap.parse_args()
-
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("ll_interleaved_bench needs a CUDA GPU")
-    torch.cuda.set_device(0)
-    import halide_b200
-    import halide_b200.lib as hlib
-    from halide_b200 import HalideBuffer, filters
-    l = halide_b200.load_library()
-    l.halide_b200_set_stream(ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-
-    def timed(fn, iters):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(iters):
-            fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / iters
+    timing.setup("ll_interleaved_bench")
 
     def profile(fn):
-        hlib.profile(True)
-        hlib.profile_reset()
-        fn()
-        torch.cuda.synchronize()
-        prof = hlib.profile_report()
-        hlib.profile(False)
-        return {k: {"launches": c, "ms": t} for k, (c, t) in sorted(prof.items())}
+        return {k: {"launches": c, "ms": t} for k, (c, t) in sorted(timing.profile(fn).items())}
 
-    def same(a, b):  # (compared as signed 16-bit views: torch's uint16 has copies, not comparisons)
-        if a.dtype == torch.uint16:
-            a, b = a.view(torch.int16), b.view(torch.int16)
-        return torch.equal(a, b)
-
-    info = gpu_info()
+    info = timing.gpu_info()
     print(f"gpu: {info}", flush=True)
     result = {"gpu": info, "levels": LEVELS, "alpha": ALPHA, "beta": BETA, "window_ms": args.window_ms,
               "rounds": args.rounds, "cases": []}
@@ -127,21 +85,14 @@ def main():
                     y_t.copy_(t_out.permute(*to_il))
 
                 arms = {"il": arm_il, "planar": arm_planar, "torch": arm_torch}
-                for fn in arms.values():
-                    for _ in range(3):
-                        fn()
-                torch.cuda.synchronize()
+                timing.warm_up(arms)
 
                 def check_outputs(when):
-                    assert same(y, y_t), f"il and torch arms differ at {name} {tname} {lname} {when}"
-                    assert same(y, yp.permute(*to_il)), f"il and planar arms differ at {name} {tname} {lname} {when}"
+                    assert timing.same(y, y_t), f"il and torch arms differ at {name} {tname} {lname} {when}"
+                    assert timing.same(y, yp.permute(*to_il)), f"il and planar arms differ at {name} {tname} {lname} {when}"
 
                 check_outputs("after warm-up")
-                iters = {k: max(3, int(args.window_ms / max(timed(fn, 3), 1e-3))) for k, fn in arms.items()}
-                ms = {k: [] for k in arms}
-                for _ in range(args.rounds):
-                    for k, fn in arms.items():
-                        ms[k].append(timed(fn, iters[k]))
+                iters, ms = timing.measure(arms, args.window_ms, args.rounds)
                 check_outputs("after timing")
                 med = {k: statistics.median(v) for k, v in ms.items()}
                 entry = {"size": name, "type": tname, "layout": lname, "n": n, "w": w, "h": h, "iters": iters,
@@ -155,11 +106,7 @@ def main():
                       flush=True)
                 del x, y, y_t, xp, yp, b_il_in, b_il_out, b_pl_in, b_pl_out
                 torch.cuda.empty_cache()
-    os.makedirs(args.out_dir, exist_ok=True)
-    path = os.path.join(args.out_dir, "ll_interleaved_bench.json")
-    with open(path, "w") as f:
-        json.dump(result, f, indent=1)
-    print(f"wrote {path}")
+    timing.write_json(args.out_dir, "ll_interleaved_bench.json", result)
 
 
 if __name__ == "__main__":

@@ -11,70 +11,27 @@ next to it.  Every arm is warmed up, then timed with CUDA events on one stream o
 read, three written) against the H100 SXM data sheet's 3.35 TB/s.  The J = 8 output must equal local_laplacian's byte for
 byte.  The GPU's name, power limit and top SM clock are read in the same run.  Writes OUT_DIR/ll_pyramid_levels_bench.json
 and prints one line per (frame, J)."""
-import argparse
-import ctypes
-import json
-import os
 import statistics
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import torch
+
+import timing
+from halide_b200 import HalideBuffer, filters
 
 SIZES = {"4k": (3840, 2160), "16k": (16384, 16384)}
 LEVELS, ALPHA, BETA = 8, 1.0 / 7.0, 1.0
 HBM_BYTES_PER_S = 3.35e12
 
 
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown (nvidia-smi failed)"
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("out_dir")
-    ap.add_argument("--window-ms", type=float, default=300.0)
-    ap.add_argument("--rounds", type=int, default=3)
+    ap = timing.common_args()
     ap.add_argument("--J", default="1,2,3,5,8,11,14,20")
     ap.add_argument("--sizes", default="4k,16k")
     args = ap.parse_args()
     js = [int(v) for v in args.J.split(",")]
+    timing.setup("ll_pyramid_levels_bench")
 
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("ll_pyramid_levels_bench needs a CUDA GPU")
-    torch.cuda.set_device(0)
-    import halide_b200
-    import halide_b200.lib as hlib
-    from halide_b200 import HalideBuffer, filters
-    l = halide_b200.load_library()
-    l.halide_b200_set_stream(ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-
-    def timed(fn, iters):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(iters):
-            fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / iters
-
-    def same(a, b):  # (compared as signed 16-bit views: torch's uint16 has copies, not comparisons)
-        return torch.equal(a.view(torch.int16), b.view(torch.int16))
-
-    def profile(fn):
-        hlib.profile(True)
-        hlib.profile_reset()
-        fn()
-        torch.cuda.synchronize()
-        prof = hlib.profile_report()
-        hlib.profile(False)
-        return {k: {"launches": c, "ms": t} for k, (c, t) in sorted(prof.items())}
-
-    info = gpu_info()
+    info = timing.gpu_info()
     print(f"gpu: {info}", flush=True)
     result = {"gpu": info, "levels": LEVELS, "alpha": ALPHA, "beta": BETA, "window_ms": args.window_ms,
               "rounds": args.rounds, "frames": []}
@@ -97,24 +54,18 @@ def main():
         frame = {"size": size, "w": W, "h": H, "J": []}
         for J in js:
             arm = lambda J=J: filters.local_laplacian_pyramid_levels(bx, J, LEVELS, ALPHA, BETA, b_y)  # noqa: E731
-            for fn in (arm, plain):
-                for _ in range(3):
-                    fn()
-            torch.cuda.synchronize()
+            arms = {"J": arm, "ll": plain}
+            timing.warm_up(arms)
             eq8 = None
             if J == 8:
-                eq8 = bool(same(y, y_ref))
+                eq8 = bool(timing.same(y, y_ref))
                 assert eq8, "J = 8 differs from local_laplacian"
-            iters = {k: max(3, int(args.window_ms / max(timed(fn, 3), 1e-3))) for k, fn in (("J", arm), ("ll", plain))}
-            ms_j, ms_ll = [], []
-            for _ in range(args.rounds):
-                ms_j.append(timed(arm, iters["J"]))
-                ms_ll.append(timed(plain, iters["ll"]))
+            iters, ms = timing.measure(arms, args.window_ms, args.rounds)
             if J == 8:
-                assert same(y, y_ref), "J = 8 differs from local_laplacian after timing"
-            prof = profile(arm)
-            entry = {"J": J, "iters": iters["J"], "ms_per_call": ms_j, "median_ms": statistics.median(ms_j),
-                     "local_laplacian_ms_per_call": ms_ll, "local_laplacian_median_ms": statistics.median(ms_ll),
+                assert timing.same(y, y_ref), "J = 8 differs from local_laplacian after timing"
+            prof = {k: {"launches": c, "ms": t} for k, (c, t) in sorted(timing.profile(arm).items())}
+            entry = {"J": J, "iters": iters["J"], "ms_per_call": ms["J"], "median_ms": statistics.median(ms["J"]),
+                     "local_laplacian_ms_per_call": ms["ll"], "local_laplacian_median_ms": statistics.median(ms["ll"]),
                      "equals_local_laplacian": eq8, "profile_ms": prof}
             if "ll_tone" in prof:
                 t = prof["ll_tone"]["ms"] / prof["ll_tone"]["launches"] * 1e-3
@@ -128,11 +79,7 @@ def main():
         result["frames"].append(frame)
         del x, y, y_ref, bx, b_y, b_ref
         torch.cuda.empty_cache()
-    os.makedirs(args.out_dir, exist_ok=True)
-    path = os.path.join(args.out_dir, "ll_pyramid_levels_bench.json")
-    with open(path, "w") as f:
-        json.dump(result, f, indent=1)
-    print(f"wrote {path}")
+    timing.write_json(args.out_dir, "ll_pyramid_levels_bench.json", result)
 
 
 if __name__ == "__main__":

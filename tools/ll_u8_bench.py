@@ -13,45 +13,23 @@ Every arm is warmed up, then timed with CUDA events on one stream over enough ca
 alternating, `rounds` times each; the median round is reported.  The outputs of the u8 and torch arms are compared bit
 for bit at every size.  Writes OUT_DIR/ll_u8_bench.json (ms per call of every round, and the per-kernel profile of one u8
 and one u16 call) and prints one line per size.  The GPU's name, power limit and top SM clock are read in the same run."""
-import argparse
-import ctypes
-import json
-import os
 import statistics
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import torch
+
+import timing
+from halide_b200 import HalideBuffer, filters
 
 SIZES = {"1080p": (1, 1920, 1080), "4k": (1, 3840, 2160), "16k": (1, 16384, 16384), "8x1080p": (8, 1920, 1080),
          "8x4k": (8, 3840, 2160)}
 LEVELS, ALPHA, BETA = 8, 1.0 / 7.0, 1.0
 
 
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown (nvidia-smi failed)"
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("out_dir")
-    ap.add_argument("--window-ms", type=float, default=300.0)
-    ap.add_argument("--rounds", type=int, default=3)
+    ap = timing.common_args()
     ap.add_argument("--sizes", default=",".join(SIZES))
     args = ap.parse_args()
-
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("ll_u8_bench needs a CUDA GPU")
-    torch.cuda.set_device(0)
-    import halide_b200
-    import halide_b200.lib as hlib
-    from halide_b200 import HalideBuffer, filters
-    l = halide_b200.load_library()
-    l.halide_b200_set_stream(ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+    timing.setup("ll_u8_bench")
 
     def to_u16(t8):  # convert<uint16_t, uint8_t>: v * 257
         return (t8.to(torch.int32) * 257).to(torch.int16).view(torch.uint16)
@@ -60,25 +38,10 @@ def main():
         w = t16.view(torch.int16).to(torch.int32) & 0xFFFF
         return (((w + 128) * 255 + 255) >> 16).to(torch.uint8)
 
-    def timed(fn, iters):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(iters):
-            fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / iters
-
     def profile(fn):
-        hlib.profile(True)
-        hlib.profile_reset()
-        fn()
-        torch.cuda.synchronize()
-        prof = hlib.profile_report()
-        hlib.profile(False)
-        return {k: {"launches": c, "ms": t} for k, (c, t) in sorted(prof.items())}
+        return {k: {"launches": c, "ms": t} for k, (c, t) in sorted(timing.profile(fn).items())}
 
-    info = gpu_info()
+    info = timing.gpu_info()
     print(f"gpu: {info}", flush=True)
     result = {"gpu": info, "levels": LEVELS, "alpha": ALPHA, "beta": BETA, "window_ms": args.window_ms,
               "rounds": args.rounds, "sizes": []}
@@ -109,16 +72,9 @@ def main():
             y8t.copy_(to_u8(o16))
 
         arms = {"u8": arm_u8, "u16": arm_u16, "torch": arm_torch}
-        for fn in arms.values():
-            for _ in range(3):
-                fn()
-        torch.cuda.synchronize()
+        timing.warm_up(arms)
         assert torch.equal(y8, y8t), f"u8 and torch arms differ at {name}"
-        iters = {k: max(3, int(args.window_ms / max(timed(fn, 3), 1e-3))) for k, fn in arms.items()}
-        ms = {k: [] for k in arms}
-        for _ in range(args.rounds):
-            for k, fn in arms.items():
-                ms[k].append(timed(fn, iters[k]))
+        iters, ms = timing.measure(arms, args.window_ms, args.rounds)
         assert torch.equal(y8, y8t), f"u8 and torch arms differ at {name} after timing"
         med = {k: statistics.median(v) for k, v in ms.items()}
         entry = {"size": name, "n": n, "w": w, "h": h, "iters": iters, "ms_per_call": ms, "median_ms": med,
@@ -130,11 +86,7 @@ def main():
               "; u16 profile " + ", ".join(f"{k} {v['ms']:.3f}" for k, v in entry["profile_u16_ms"].items()), flush=True)
         del x8, x16, y8, y16, y8t, b8i, b8o, b16i, b16o
         torch.cuda.empty_cache()
-    os.makedirs(args.out_dir, exist_ok=True)
-    path = os.path.join(args.out_dir, "ll_u8_bench.json")
-    with open(path, "w") as f:
-        json.dump(result, f, indent=1)
-    print(f"wrote {path}")
+    timing.write_json(args.out_dir, "ll_u8_bench.json", result)
 
 
 if __name__ == "__main__":

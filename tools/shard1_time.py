@@ -1,14 +1,11 @@
 """Times the row-sharded code path with a single rank (no neighbours): isolates the compute-side cost of sharding
 (per-level launches, halo-aware input path) from the communication cost.  torchrun --nproc-per-node 1 tools/shard1_time.py"""
-import os, sys
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import itertools, sys
 import torch, torch.distributed as td
+import timing
 torch.cuda.set_device(0)
 td.init_process_group("nccl", device_id=torch.device("cuda", 0))
-import halide_b200
 from halide_b200 import HalideBuffer, dist, filters
-import halide_b200.lib as hlib
 W, H = (int(sys.argv[1]), int(sys.argv[2])) if len(sys.argv) > 2 else (3840, 2160)
 NS = 4 if W * H < 2e7 else 1
 g = torch.Generator(device="cuda"); g.manual_seed(1)
@@ -16,16 +13,16 @@ ins = [torch.randint(-32768, 32768, (3, H, W), dtype=torch.int16, device="cuda",
 outs = [torch.zeros((3, H, W), dtype=torch.uint16, device="cuda") for _ in range(NS)]
 bi = [HalideBuffer.from_torch(t) for t in ins]; bo = [HalideBuffer.from_torch(t) for t in outs]
 sh = dist.RowSharder(0, 1, W, H)
-for name, fn in (("sharded(1 rank)", lambda i: sh.local_laplacian(bi[i % NS], 8, 1 / 7, 1.0, bo[i % NS])),
-                 ("single", lambda i: filters.local_laplacian(bi[i % NS], 8, 1 / 7, 1.0, bo[i % NS]))):
-    for i in range(5): fn(i)
+step = itertools.count()
+def rotating(f):  # each call takes the next frame pair
+    def call():
+        i = next(step) % NS
+        f(bi[i], 8, 1 / 7, 1.0, bo[i])
+    return call
+for name, fn in (("sharded(1 rank)", rotating(sh.local_laplacian)), ("single", rotating(filters.local_laplacian))):
+    for _ in range(5): fn()
     torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for i in range(20): fn(i)
-    e1.record(); torch.cuda.synchronize()
-    hlib.profile(True); hlib.profile_reset()
-    for i in range(5): fn(i)
-    torch.cuda.synchronize(); rep = hlib.profile_report(); hlib.profile(False)
-    print(name, f"{e0.elapsed_time(e1) / 20 * 1e3:.1f} us/step", {k: (c // 5, round(ms / 5 * 1e3, 1)) for k, (c, ms) in rep.items()})
+    us = timing.timed(fn, 20) * 1e3
+    rep = timing.profile(fn, 5)
+    print(name, f"{us:.1f} us/step", {k: (c // 5, round(ms / 5 * 1e3, 1)) for k, (c, ms) in rep.items()})
 td.destroy_process_group()

@@ -13,26 +13,16 @@ reports the time per call, ns per stage per Mpx, the launch count and the work r
 run after it), sum(region area x stages) / (S x W x H), computed from the shapes.  The S = 32 output must equal
 stencil_chain's byte for byte.  The GPU's name, power limit and top SM clock are read in the same run.  Writes
 OUT_DIR/stencil_chain_stencils_bench.json and prints one line per S."""
-import argparse
-import ctypes
-import json
-import os
 import statistics
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import torch
+
+import timing
+from halide_b200 import HalideBuffer, filters
 
 S_VALUES = "1,2,3,4,5,8,16,31,32,33,64,100"
 FRAMES = "1536x2560,3840x2160,7680x4320"
 FUSE = 4  # stages per launch in stencil_chain.cu
-
-
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown (nvidia-smi failed)"
 
 
 def launch_plan(s):
@@ -52,38 +42,15 @@ def work_ratio(s, w, h):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("out_dir")
-    ap.add_argument("--window-ms", type=float, default=300.0)
-    ap.add_argument("--rounds", type=int, default=3)
+    ap = timing.common_args()
     ap.add_argument("--s", default=S_VALUES)
     ap.add_argument("--frames", default=FRAMES)
     args = ap.parse_args()
     s_values = [int(v) for v in args.s.split(",")]
     frames = [tuple(int(v) for v in f.split("x")) for f in args.frames.split(",")]
+    timing.setup("stencil_chain_stencils_bench")
 
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("stencil_chain_stencils_bench needs a CUDA GPU")
-    torch.cuda.set_device(0)
-    import halide_b200
-    from halide_b200 import HalideBuffer, filters
-    l = halide_b200.load_library()
-    l.halide_b200_set_stream(ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-
-    def timed(fn, iters):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(iters):
-            fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / iters
-
-    def same(a, b):
-        return bool(torch.equal(a.view(torch.int16), b.view(torch.int16)))
-
-    info = gpu_info()
+    info = timing.gpu_info()
     print(f"gpu: {info}", flush=True)
     result = {"gpu": info, "window_ms": args.window_ms, "rounds": args.rounds, "frames": []}
     for w, h in frames:
@@ -101,22 +68,15 @@ def main():
         for s in s_values:
             arms[f"s{s}"] = (lambda s=s: filters.stencil_chain_stencils(bx, s, bouts[s]))
         arms["stencil_chain"] = lambda: filters.stencil_chain(bx, b_ref)
-        for fn in arms.values():
-            for _ in range(3):
-                fn()
-        torch.cuda.synchronize()
+        timing.warm_up(arms)
         same32 = None
         if 32 in outs:
-            same32 = same(outs[32], y_ref)
+            same32 = timing.same(outs[32], y_ref)
             assert same32, f"{w}x{h}: stencils = 32 differs from stencil_chain"
-        iters = {k: max(3, int(args.window_ms / max(timed(fn, 3), 1e-3))) for k, fn in arms.items()}
-        ms = {k: [] for k in arms}
-        for _ in range(args.rounds):
-            for k, fn in arms.items():
-                ms[k].append(timed(fn, iters[k]))
+        iters, ms = timing.measure(arms, args.window_ms, args.rounds)
         med = {k: statistics.median(v) for k, v in ms.items()}
         if 32 in outs:
-            assert same(outs[32], y_ref), f"{w}x{h}: stencils = 32 differs from stencil_chain after timing"
+            assert timing.same(outs[32], y_ref), f"{w}x{h}: stencils = 32 differs from stencil_chain after timing"
 
         mpx = w * h / 1e6
         entry = {"w": w, "h": h, "s32_equals_stencil_chain": same32,
@@ -136,11 +96,7 @@ def main():
                   f"{e['ns_per_stage_per_mpx']:.1f} ns/stage/Mpx, {e['launches']} launches, work x{e['work_ratio']:.3f}",
                   flush=True)
         result["frames"].append(entry)
-    os.makedirs(args.out_dir, exist_ok=True)
-    path = os.path.join(args.out_dir, "stencil_chain_stencils_bench.json")
-    with open(path, "w") as f:
-        json.dump(result, f, indent=1)
-    print(f"wrote {path}")
+    timing.write_json(args.out_dir, "stencil_chain_stencils_bench.json", result)
 
 
 if __name__ == "__main__":
