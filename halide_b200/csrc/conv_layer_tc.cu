@@ -62,6 +62,8 @@ struct ConvShape {
     int co_tiles, co_pad;        // CO tiles of TN channels; Bt rows per tap = co_tiles * TN
     int vec2;                    // relu's base and strides keep channel pairs 8-byte aligned
     long long out_sx, out_sy, out_sn;
+    int CI;                      // the recompute's view of input and filter (conv_recompute)
+    long long in_sx, in_sy, in_sn, f_skx, f_sky, f_sci;
 };
 
 // K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma (PTX ISA "Matrix Descriptor Format"): start address >> 4
@@ -100,6 +102,9 @@ template<int REGS>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
 
 // ---- operand preparation ----------------------------------------------------------------------------------------------
+// The split of a non-finite x gives lo = NaN (inf - inf, or NaN - hi), so every product it enters, including the ones
+// against a zero, is NaN, and so is the sum of every output whose receptive field holds it: the epilogue recomputes
+// those outputs (conv_recompute).
 __global__ void conv_split_input_kernel(const float4 *__restrict__ in, float4 *__restrict__ hi, float4 *__restrict__ lo, size_t n4) {
     size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
     if (i >= n4) return;
@@ -199,12 +204,44 @@ __device__ __forceinline__ void consume_step(float (&d)[TN / 2], const uint8_t *
     if (it > 0 && lane == 0) tma::mbar_arrive(&empty_bar[(it - 1) % STAGES]);
 }
 
+// The generator's relu, max(0, conv), as Halide lowers it: select(conv > 0, conv, 0).  +inf stays +inf; NaN and -0.0
+// give +0.0.
+__device__ __forceinline__ float relu(float v) { return v > 0.f ? v : 0.f; }
+
+// One output in the generator's order: bias, then ky, kx, ci ascending, each term a separate fp32 multiply and add (the
+// library builds with --fmad=false), then relu.  `in` is the input at the output's (x, y, n), `f` the filter at its co.
+// The epilogue calls it for the sums that are not finite, where the split's products say nothing about which of +inf,
+// -inf and NaN the generator's sum is.
+__device__ float conv_recompute(const float *in, long long in_sx, long long in_sy, const float *f, long long f_skx, long long f_sky,
+                                long long f_sci, int ci_n, float acc) {
+    for (int ky = 0; ky < 3; ky++)
+        for (int kx = 0; kx < 3; kx++) {
+            const float *a = in + kx * in_sx + ky * in_sy, *w = f + kx * f_skx + ky * f_sky;
+            for (int ci = 0; ci < ci_n; ci++) acc = acc + w[ci * f_sci] * a[ci];
+        }
+    return relu(acc);
+}
+
+// Output pixel (n, y, x) of row q of the output enumeration; false for a discarded row.
+template<bool ANY>
+__device__ __forceinline__ bool output_pixel(int q, int img, const ConvShape &sh, int &n, int &y, int &x) {
+    if (!ANY) {
+        n = img, y = q / WP, x = q - y * WP;
+        return y < H && x < W;
+    }
+    if (q >= sh.m_rows) return false;
+    n = q / sh.rows_per_image;  // q runs over the whole padded batch
+    const int r = q - n * sh.rows_per_image;
+    y = r / sh.wp, x = r - y * sh.wp;
+    return y < sh.H && x < sh.W;
+}
+
 // The kernel body.  ANY = false is the fixed shape (every quantity a constant, `sh` unused, grid (tiles, images));
 // ANY = true reads the shape from `sh` (1-D grid, CO tile fastest).  TN is the N tile; FOLD adds the third register set.
 template<int TN, bool ANY, bool FOLD>
 __device__ __forceinline__ void conv_tc_body(const CUtensorMap *map_a_hi, const CUtensorMap *map_a_lo, const CUtensorMap *map_b_hi,
-                                             const CUtensorMap *map_b_lo, const ConvShape &sh, const float *__restrict__ bias,
-                                             float *__restrict__ out) {
+                                             const CUtensorMap *map_b_lo, const ConvShape &sh, const float *__restrict__ in,
+                                             const float *__restrict__ filt, const float *__restrict__ bias, float *__restrict__ out) {
     constexpr int NACC = TN / 2;  // accumulator registers per set
     extern __shared__ uint8_t smem_raw[];
     uint8_t *tiles = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);  // SWIZZLE_128B needs 1024-byte alignment
@@ -281,27 +318,24 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap *map_a_hi, const 
 
     // ===== epilogue: + bias, relu, float2 stores of the valid pixels =====
     const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+    uint64_t redo = 0;  // bit i: accumulator i's sum is not finite
 #pragma unroll
     for (int h = 0; h < 2; h++) {
         const int q = tile * TILE_M + r0 + 8 * h;  // output index over the padded width
+        int n, y, x;
+        if (!output_pixel<ANY>(q, img, sh, n, y, x)) continue;
         if constexpr (!ANY) {
-            const int y = q / WP, x = q - y * WP;
-            if (y >= H || x >= W) continue;
             float *orow = out + (((size_t)img * H + y) * W + x) * CO;
 #pragma unroll
             for (int j = 0; j < TN / 8; j++) {
                 const int c = 8 * j + 2 * (lane & 3);
                 const float2 b = __ldg(reinterpret_cast<const float2 *>(bias + c));
-                float2 v;
-                v.x = fmaxf((acc0[4 * j + 2 * h] + acc1[4 * j + 2 * h]) + b.x, 0.f);
-                v.y = fmaxf((acc0[4 * j + 2 * h + 1] + acc1[4 * j + 2 * h + 1]) + b.y, 0.f);
-                *reinterpret_cast<float2 *>(orow + c) = v;
+                const float s0 = (acc0[4 * j + 2 * h] + acc1[4 * j + 2 * h]) + b.x;
+                const float s1 = (acc0[4 * j + 2 * h + 1] + acc1[4 * j + 2 * h + 1]) + b.y;
+                redo |= (uint64_t)!isfinite(s0) << (4 * j + 2 * h) | (uint64_t)!isfinite(s1) << (4 * j + 2 * h + 1);
+                *reinterpret_cast<float2 *>(orow + c) = make_float2(relu(s0), relu(s1));
             }
         } else {
-            if (q >= sh.m_rows) continue;
-            const int n = q / sh.rows_per_image, r = q - n * sh.rows_per_image;  // q runs over the whole padded batch
-            const int y = r / sh.wp, x = r - y * sh.wp;
-            if (y >= sh.H || x >= sh.W) continue;
             float *orow = out + n * sh.out_sn + y * sh.out_sy + x * sh.out_sx;
 #pragma unroll
             for (int j = 0; j < TN / 8; j++) {
@@ -310,9 +344,10 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap *map_a_hi, const 
                 const bool pair = c + 1 < sh.CO;
                 float s0 = acc0[4 * j + 2 * h] + acc1[4 * j + 2 * h], s1 = acc0[4 * j + 2 * h + 1] + acc1[4 * j + 2 * h + 1];
                 if (FOLD) s0 += sum[4 * j + 2 * h], s1 += sum[4 * j + 2 * h + 1];
-                float2 v;
-                v.x = fmaxf(s0 + __ldg(bias + c), 0.f);
-                v.y = pair ? fmaxf(s1 + __ldg(bias + c + 1), 0.f) : 0.f;
+                s0 += __ldg(bias + c);
+                s1 = pair ? s1 + __ldg(bias + c + 1) : 0.f;
+                redo |= (uint64_t)!isfinite(s0) << (4 * j + 2 * h) | (uint64_t)!isfinite(s1) << (4 * j + 2 * h + 1);
+                const float2 v = make_float2(relu(s0), relu(s1));
                 if (pair && sh.vec2) {
                     *reinterpret_cast<float2 *>(orow + c) = v;
                 } else {
@@ -322,14 +357,32 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap *map_a_hi, const 
             }
         }
     }
+    // Outputs whose sum is not finite: an operand is +-inf or NaN (conv_split_input_kernel), or the sum overflowed.  Each
+    // is computed again in the generator's order and overwrites what the loop above stored.  Rare, so a plain loop.
+#pragma unroll 1
+    while (redo) {
+        const int i = __ffsll((long long)redo) - 1;
+        redo &= redo - 1;
+        const int h = (i >> 1) & 1, c = co0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        int n, y, x;
+        output_pixel<ANY>(tile * TILE_M + r0 + 8 * h, img, sh, n, y, x);
+        if constexpr (!ANY) {
+            out[(((size_t)n * H + y) * W + x) * CO + c] =
+                conv_recompute(in + (((size_t)n * HP + y) * WP + x) * CI, CI, WP * CI, filt + c, CO, 3 * CO, 9 * CO, CI, bias[c]);
+        } else {
+            out[n * sh.out_sn + y * sh.out_sy + x * sh.out_sx + c] = conv_recompute(
+                in + x * sh.in_sx + y * sh.in_sy + n * sh.in_sn, sh.in_sx, sh.in_sy, filt + c, sh.f_skx, sh.f_sky, sh.f_sci, sh.CI, bias[c]);
+        }
+    }
 }
 
 __global__ void __launch_bounds__(THREADS, 1) conv_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
                                                                    const __grid_constant__ CUtensorMap map_a_lo,
                                                                    const __grid_constant__ CUtensorMap map_b_hi,
                                                                    const __grid_constant__ CUtensorMap map_b_lo,
+                                                                   const float *__restrict__ in, const float *__restrict__ filt,
                                                                    const float *__restrict__ bias, float *__restrict__ out) {
-    conv_tc_body<TILE_N, false, false>(&map_a_hi, &map_a_lo, &map_b_hi, &map_b_lo, ConvShape{}, bias, out);
+    conv_tc_body<TILE_N, false, false>(&map_a_hi, &map_a_lo, &map_b_hi, &map_b_lo, ConvShape{}, in, filt, bias, out);
 }
 
 template<int TN, bool FOLD>
@@ -338,8 +391,9 @@ __global__ void __launch_bounds__(THREADS_ANY, 1) conv_layer_tc_any_kernel(const
                                                                            const __grid_constant__ CUtensorMap map_b_hi,
                                                                            const __grid_constant__ CUtensorMap map_b_lo,
                                                                            const __grid_constant__ ConvShape sh,
+                                                                           const float *__restrict__ in, const float *__restrict__ filt,
                                                                            const float *__restrict__ bias, float *__restrict__ out) {
-    conv_tc_body<TN, true, FOLD>(&map_a_hi, &map_a_lo, &map_b_hi, &map_b_lo, sh, bias, out);
+    conv_tc_body<TN, true, FOLD>(&map_a_hi, &map_a_lo, &map_b_hi, &map_b_lo, sh, in, filt, bias, out);
 }
 
 // rows x pitch floats, boxes of box_rows x 32
@@ -352,10 +406,11 @@ bool make_map(CUtensorMap *m, void *base, uint64_t rows, uint32_t box_rows, uint
 
 template<int TN, bool FOLD>
 void launch_any(unsigned grid, cudaStream_t s, const CUtensorMap &ma_hi, const CUtensorMap &ma_lo, const CUtensorMap &mb_hi,
-                const CUtensorMap &mb_lo, const ConvShape &sh, const float *bias, float *out) {
+                const CUtensorMap &mb_lo, const ConvShape &sh, const ConvProblem &p) {
     hb::allow_smem(conv_layer_tc_any_kernel<TN, FOLD>, smem_bytes(TN));
     HB_LAUNCH(TN == 128 ? (FOLD ? "conv_layer_tc_n128_fold" : "conv_layer_tc_n128") : (FOLD ? "conv_layer_tc_n64_fold" : "conv_layer_tc_n64"),
-              (conv_layer_tc_any_kernel<TN, FOLD>), grid, THREADS_ANY, smem_bytes(TN), s, ma_hi, ma_lo, mb_hi, mb_lo, sh, bias, out);
+              (conv_layer_tc_any_kernel<TN, FOLD>), grid, THREADS_ANY, smem_bytes(TN), s, ma_hi, ma_lo, mb_hi, mb_lo, sh, p.in, p.filt,
+              p.bias, p.out);
 }
 
 }  // namespace
@@ -377,8 +432,8 @@ int conv_layer_tc_run(const float *din, const float *df, const float *db, float 
     HB_LAUNCH("conv_split_input", conv_split_input_kernel, (unsigned)((a_elems / 4 + 255) / 256), 256, 0, s, (const float4 *)din, (float4 *)a_hi,
               (float4 *)a_lo, a_elems / 4);
     HB_LAUNCH("conv_prep_filter", conv_prep_filter_kernel, (unsigned)((b_elems + 255) / 256), 256, 0, s, df, b_hi, b_lo);
-    HB_LAUNCH("conv_layer_tc", conv_layer_tc_kernel, dim3(TILES_PER_IMAGE, N), THREADS, smem_bytes(TILE_N), s, ma_hi, ma_lo, mb_hi, mb_lo, db,
-              dout);
+    HB_LAUNCH("conv_layer_tc", conv_layer_tc_kernel, dim3(TILES_PER_IMAGE, N), THREADS, smem_bytes(TILE_N), s, ma_hi, ma_lo, mb_hi, mb_lo, din,
+              df, db, dout);
     return 0;
 }
 
@@ -399,6 +454,9 @@ int conv_layer_tc_run_any_shape(const ConvProblem &p, cudaStream_t s) {
     sh.co_pad = sh.co_tiles * tn;
     sh.out_sx = p.out_sx, sh.out_sy = p.out_sy, sh.out_sn = p.out_sn;
     sh.vec2 = ((uintptr_t)p.out % 8 == 0) && p.out_sx % 2 == 0 && p.out_sy % 2 == 0 && p.out_sn % 2 == 0;
+    sh.CI = p.CI;
+    sh.in_sx = p.in_sx, sh.in_sy = p.in_sy, sh.in_sn = p.in_sn;
+    sh.f_skx = p.f_skx, sh.f_sky = p.f_sky, sh.f_sci = p.f_sci;
     const int rows = p.N * sh.rows_per_image;  // fits: input's extents multiply to less than 2^31
     const long long m_tiles = ((long long)sh.m_rows + TILE_M - 1) / TILE_M;
     if (m_tiles * sh.co_tiles > 0x7fffffffLL) {
@@ -423,11 +481,11 @@ int conv_layer_tc_run_any_shape(const ConvProblem &p, cudaStream_t s) {
     const unsigned grid = (unsigned)(m_tiles * sh.co_tiles);
     const bool fold = sh.k_steps > FOLD_STEPS;
     if (tn == 128) {
-        if (fold) launch_any<128, true>(grid, s, ma_hi, ma_lo, mb_hi, mb_lo, sh, p.bias, p.out);
-        else launch_any<128, false>(grid, s, ma_hi, ma_lo, mb_hi, mb_lo, sh, p.bias, p.out);
+        if (fold) launch_any<128, true>(grid, s, ma_hi, ma_lo, mb_hi, mb_lo, sh, p);
+        else launch_any<128, false>(grid, s, ma_hi, ma_lo, mb_hi, mb_lo, sh, p);
     } else {
-        if (fold) launch_any<64, true>(grid, s, ma_hi, ma_lo, mb_hi, mb_lo, sh, p.bias, p.out);
-        else launch_any<64, false>(grid, s, ma_hi, ma_lo, mb_hi, mb_lo, sh, p.bias, p.out);
+        if (fold) launch_any<64, true>(grid, s, ma_hi, ma_lo, mb_hi, mb_lo, sh, p);
+        else launch_any<64, false>(grid, s, ma_hi, ma_lo, mb_hi, mb_lo, sh, p);
     }
     return 0;
 }
