@@ -194,9 +194,15 @@ int get_lut(PlanT<T> &p, cudaStream_t s) {
     return 0;
 }
 
-// the fast level-1 kernel also produces level 2 (so the pyramid must have one: J >= 3)
+// the fast level-1 kernel also produces level 2 (so the pyramid must have one: J >= 3).  It and ll_down_rows sum a
+// downsample's 16 taps before one * 1/64 where the generator scales by 1/8 after each pass, which overflows 8 times
+// sooner.  A level value is at most |beta| + 1 + 0.61 |alpha| in magnitude (remap(x) <= e^-1/2 |alpha|), so with both
+// scalars below 2^100 no such sum comes near the float range; larger or non-finite ones take the generic kernels, which
+// scale as the generator does.
 template<typename P>
-bool fast_down(const P &p) { return p.f.levels == 8 && p.J >= 3 && !(g_force_naive & 1); }
+bool fast_down(const P &p) {
+    return p.f.levels == 8 && p.J >= 3 && !(g_force_naive & 1) && fabsf(p.alpha) < 0x1p100f && fabsf(p.f.beta) < 0x1p100f;
+}
 // the fast final kernel also produces outGPyramid[1] (for its own tile) from level 2, so no up-sweep launch runs for
 // level 1 (J >= 3 as well)
 template<typename P>

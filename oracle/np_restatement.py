@@ -56,14 +56,18 @@ def halide_exp(x_full):
 
 def _down(f, xlo, xhi, ylo, yhi):
     """downsample(f) on [xlo, xhi] x [ylo, yhi]: 1-3-3-1 in y, then in x (generator :266-272)."""
-    three, eighth = F(3.0), F(0.125)
     xs_wide = np.arange(2 * xlo - 1, 2 * xhi + 3)
     ys = np.arange(ylo, yhi + 1)
-    downy = (f.at(xs_wide, 2 * ys - 1) + three * (f.at(xs_wide, 2 * ys) + f.at(xs_wide, 2 * ys + 1)) + f.at(xs_wide, 2 * ys + 2)) * eighth
+    downy = _down4(f.at(xs_wide, 2 * ys - 1), f.at(xs_wide, 2 * ys), f.at(xs_wide, 2 * ys + 1), f.at(xs_wide, 2 * ys + 2))
     dy = Field(downy, 2 * xlo - 1, ylo)
     xs = np.arange(xlo, xhi + 1)
-    downx = (dy.at(2 * xs - 1, ys) + three * (dy.at(2 * xs, ys) + dy.at(2 * xs + 1, ys)) + dy.at(2 * xs + 2, ys)) * eighth
+    downx = _down4(dy.at(2 * xs - 1, ys), dy.at(2 * xs, ys), dy.at(2 * xs + 1, ys), dy.at(2 * xs + 2, ys))
     return Field(downx.astype(F), xlo, ylo)
+
+
+def _down4(a, b, c, d):
+    """(f(2x-1) + 3 * (f(2x) + f(2x+1)) + f(2x+2)) / 8, summed left to right; / 8 folds to * 0.125."""
+    return (a + F(3.0) * (b + c) + d) * F(0.125)
 
 
 def _lerp(zero, one, w):
@@ -86,7 +90,24 @@ def _up(f, xlo, xhi, ylo, yhi):
 def local_laplacian(inp, levels, alpha, beta, out_shape=None, in_mins=(0, 0, 0), out_mins=(0, 0, 0), J=8):
     """inp: uint16 [c, h, w] whose element [0, 0, 0] sits at coordinates in_mins = (x, y, c); alpha as the filter
     receives it (already divided by levels - 1).  Returns uint16 [C, H, W] at out_mins."""
-    alpha, beta = F(alpha), F(beta)
+    return clamp_u16(local_laplacian_color(inp, levels, alpha, beta, out_shape, in_mins, out_mins, J))
+
+
+def clamp_u16(color):
+    """u16(clamp(color, 0, 65535)) (generator :87).  Halide's min and max select on a comparison, which is false for NaN:
+    min(NaN, 65535) = 65535, then max(65535, 0) = 65535.  (np.minimum / np.maximum would pass the NaN on to the cast.)"""
+    m = np.where(color < F(65535.0), color, F(65535.0))
+    return np.where(m > F(0.0), m, F(0.0)).astype(np.uint16)
+
+
+def local_laplacian_color(inp, levels, alpha, beta, out_shape=None, in_mins=(0, 0, 0), out_mins=(0, 0, 0), J=8):
+    """local_laplacian's colour before the final clamp and cast: float32 [C, H, W].  Every float alpha and beta is
+    accepted; large ones overflow the pyramid's sums to infinities and NaN, as they do in Halide."""
+    with np.errstate(over="ignore", invalid="ignore", under="ignore"):
+        return _color(inp, levels, F(alpha), F(beta), out_shape, in_mins, out_mins, J)
+
+
+def _color(inp, levels, alpha, beta, out_shape, in_mins, out_mins, J):
     ic, ih, iw = inp.shape
     if out_shape is None:
         out_shape = inp.shape
@@ -155,11 +176,10 @@ def local_laplacian(inp, levels, alpha, beta, out_shape=None, in_mins=(0, 0, 0),
     g_out = inG[0].at(xs, ys)
     num = outG[0].arr + eps
     den = g_out + eps
-    out = np.empty((C, H, W), np.uint16)
+    out = np.empty((C, H, W), F)
     for c in range(C):
         ch = inp[oc0 + c - ic0][(ys - iy0)[:, None], (xs - ix0)[None, :]].astype(F)  # unclamped read: must be inside the input
-        color = (ch * num) / den
-        out[c] = np.maximum(np.minimum(color, F(65535.0)), F(0.0)).astype(np.uint16)
+        out[c] = (ch * num) / den
     return out
 
 
