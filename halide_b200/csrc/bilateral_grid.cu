@@ -25,6 +25,9 @@
 //                   4 pixels per thread (float4 in / float4 out), 8 shared 8-byte corner loads per pixel.
 // Grid layout in HBM: [cell_y][cell_x][z][2] f32 — the (z, z+1) x (value, weight) quad a pixel
 // needs at one corner is 16 contiguous bytes.
+// halide_b200_bilateral_grid_u8 runs the same three kernels on uint8 frames (2 algorithmic B/px): bg_hist_blurz and
+// bg_slice take the frame's element type as a template parameter and convert at the load and the store
+// (hl::frame_to_f32 / hl::frame_from_f32), everything between them is the float path's.
 #include <algorithm>
 
 #include "hb_common.h"
@@ -35,10 +38,10 @@ namespace {
 constexpr int S = 8;  // s_sigma GeneratorParam of the shipped app (generator :8)
 
 struct BGParams {
-    const float *in;  // element at input mins
+    const float *in;  // element at input mins (a uint8_t frame's for bg_hist_blurz<uint8_t> / bg_slice<uint8_t>)
     int64_t in_sy;
     int in_x0, in_y0, in_w, in_h;
-    float *out;  // element at output mins
+    float *out;  // element at output mins (the same)
     int64_t out_sy;
     int out_x0, out_y0, W, H;
     float inv_r;
@@ -52,6 +55,9 @@ struct BGParams {
 // ---- K1: histogram + blurz --------------------------------------------------------------------------
 // One warp handles 16 horizontally adjacent cells (128 px): lane l covers columns 4l..4l+3 of the
 // strip for all 8 rows of the cell row.  Bins live in shared memory as [bin][channel][thread].
+// T: the frame's element type.  A float frame is read with float4 loads, an 8-bit one with uchar4 loads (4 bytes), each
+// sample converted to the float the float path sees for it (hl::frame_to_f32).
+template<typename T>
 __global__ void __launch_bounds__(128) bg_hist_blurz_kernel(BGParams p) {
     extern __shared__ float s_bins[];  // (zmax+1) * 2 * 128
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -65,16 +71,21 @@ __global__ void __launch_bounds__(128) bg_hist_blurz_kernel(BGParams p) {
 #pragma unroll
     for (int ry = 0; ry < S; ry++) {
         int y = hl::clampi(gy * S + ry - S / 2, p.in_y0, p.in_y0 + p.in_h - 1) - p.in_y0;
-        const float *row = p.in + (int64_t)y * p.in_sy;
+        const T *row = reinterpret_cast<const T *>(p.in) + (int64_t)y * p.in_sy;
         float v[4];
-        if (interior_x && ((reinterpret_cast<uintptr_t>(row + (px0 - p.in_x0)) & 15) == 0)) {
-            float4 t = __ldg(reinterpret_cast<const float4 *>(row + (px0 - p.in_x0)));
-            v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+        if (interior_x && ((reinterpret_cast<uintptr_t>(row + (px0 - p.in_x0)) & (4 * sizeof(T) - 1)) == 0)) {
+            if constexpr (sizeof(T) == 1) {
+                const uchar4 t = __ldg(reinterpret_cast<const uchar4 *>(row + (px0 - p.in_x0)));
+                v[0] = hl::frame_to_f32(t.x); v[1] = hl::frame_to_f32(t.y); v[2] = hl::frame_to_f32(t.z); v[3] = hl::frame_to_f32(t.w);
+            } else {
+                float4 t = __ldg(reinterpret_cast<const float4 *>(row + (px0 - p.in_x0)));
+                v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+            }
         } else {
 #pragma unroll
             for (int i = 0; i < 4; i++) {
                 int x = hl::clampi(px0 + i, p.in_x0, p.in_x0 + p.in_w - 1) - p.in_x0;
-                v[i] = __ldg(row + x);
+                v[i] = hl::frame_to_f32(__ldg(row + x));
             }
         }
 #pragma unroll
@@ -162,6 +173,9 @@ __global__ void __launch_bounds__(256) bg_blur_xy_kernel(BGParams p, int rows_pe
 // image, where the two lanes' planes zi differ.)
 constexpr int kSliceW = 128, kSliceCells = 17, kSlicePitch = 24;
 
+// T: the frame's element type.  An 8-bit frame's 4 pixels move as one uchar4 in and one uchar4 out; the value sliced on is
+// hl::frame_to_f32 of the sample and the result is stored as hl::frame_from_f32<T>.
+template<typename T>
 __global__ void __launch_bounds__(256) bg_slice_kernel(BGParams p) {
     extern __shared__ float2 s_grid[];  // [nz][2][kSlicePitch]
     const int lane = threadIdx.x, row = threadIdx.y, tid = row * 32 + lane;
@@ -181,8 +195,8 @@ __global__ void __launch_bounds__(256) bg_slice_kernel(BGParams p) {
     __syncthreads();
     const int y = Y0 + row, x = X0 + 8 * (lane & 15) + 4 * (lane >> 4);
     if (y < p.out_y0 || y >= p.out_y0 + p.H || x + 3 < p.out_x0 || x >= p.out_x0 + p.W) return;
-    const float *ip = p.in + (int64_t)(y - p.in_y0) * p.in_sy + (x - p.in_x0);
-    float *op = p.out + (int64_t)(y - p.out_y0) * p.out_sy + (x - p.out_x0);
+    const T *ip = reinterpret_cast<const T *>(p.in) + (int64_t)(y - p.in_y0) * p.in_sy + (x - p.in_x0);
+    T *op = reinterpret_cast<T *>(p.out) + (int64_t)(y - p.out_y0) * p.out_sy + (x - p.out_x0);
     const float2 *c00 = s_grid + (lane & 15);  // cell (xi, yi) of this thread's four pixels; xi + 1: +1, yi + 1: +kSlicePitch
     const float yf = __fmul_rn((float)(y & (S - 1)), 0.125f);
     auto px = [&](float raw, int xx) -> float {
@@ -203,17 +217,27 @@ __global__ void __launch_bounds__(256) bg_slice_kernel(BGParams p) {
         return __fdiv_rn(v0, v1);
     };
     const bool full = x >= p.out_x0 && x + 3 < p.out_x0 + p.W;
-    if (full && ((reinterpret_cast<uintptr_t>(ip) | reinterpret_cast<uintptr_t>(op)) & 15) == 0) {
-        const float4 v = __ldg(reinterpret_cast<const float4 *>(ip));
-        float4 o;
-        o.x = px(v.x, x);
-        o.y = px(v.y, x + 1);
-        o.z = px(v.z, x + 2);
-        o.w = px(v.w, x + 3);
-        *reinterpret_cast<float4 *>(op) = o;
+    if (full && ((reinterpret_cast<uintptr_t>(ip) | reinterpret_cast<uintptr_t>(op)) & (4 * sizeof(T) - 1)) == 0) {
+        if constexpr (sizeof(T) == 1) {
+            const uchar4 v = __ldg(reinterpret_cast<const uchar4 *>(ip));
+            uchar4 o;
+            o.x = hl::frame_from_f32<T>(px(hl::frame_to_f32(v.x), x));
+            o.y = hl::frame_from_f32<T>(px(hl::frame_to_f32(v.y), x + 1));
+            o.z = hl::frame_from_f32<T>(px(hl::frame_to_f32(v.z), x + 2));
+            o.w = hl::frame_from_f32<T>(px(hl::frame_to_f32(v.w), x + 3));
+            *reinterpret_cast<uchar4 *>(op) = o;
+        } else {
+            const float4 v = __ldg(reinterpret_cast<const float4 *>(ip));
+            float4 o;
+            o.x = px(v.x, x);
+            o.y = px(v.y, x + 1);
+            o.z = px(v.z, x + 2);
+            o.w = px(v.w, x + 3);
+            *reinterpret_cast<float4 *>(op) = o;
+        }
     } else {
         for (int i = 0; i < 4; i++) {
-            if (x + i >= p.out_x0 && x + i < p.out_x0 + p.W) op[i] = px(__ldg(ip + i), x + i);
+            if (x + i >= p.out_x0 && x + i < p.out_x0 + p.W) op[i] = hl::frame_from_f32<T>(px(hl::frame_to_f32(__ldg(ip + i)), x + i));
         }
     }
 }
@@ -462,6 +486,11 @@ const halide_filter_argument_t kArgs[3] = {
     {"r_sigma", halide_argument_kind_input_scalar, 0, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, &sv_rsigma, nullptr},
     {"bilateral_grid", halide_argument_kind_output_buffer, 2, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
+// halide_b200_bilateral_grid_u8: the same buffers in uint8.
+const halide_filter_argument_t kU8Args[2] = {
+    {"input", halide_argument_kind_input_buffer, 2, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+    {"bilateral_grid", halide_argument_kind_output_buffer, 2, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+};
 
 inline int fdiv(int a, int b) {  // floor division, b > 0
     int q = a / b;
@@ -469,10 +498,13 @@ inline int fdiv(int a, int b) {  // floor division, b > 0
 }
 
 // bilateral_grid with cell size s_sigma (the generator's GeneratorParam): the shipped S runs bg_hist_blurz, bg_blur_xy
-// and bg_slice; every other cell size runs bg_hist_blurz_s, bg_blur_xy and bg_slice_s.
-int run_bilateral_grid(halide_buffer_t *input, int s_sigma, float r_sigma, halide_buffer_t *output) {
+// and bg_slice; every other cell size runs bg_hist_blurz_s, bg_blur_xy and bg_slice_s.  T is the frames' element type and
+// rec their argument records: float (kArgs), or uint8_t (kU8Args), which runs S only.
+template<typename T>
+int run_bilateral_grid(halide_buffer_t *input, int s_sigma, float r_sigma, halide_buffer_t *output,
+                       const halide_filter_argument_t &in_rec, const halide_filter_argument_t &out_rec) {
     int r;
-    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[2]}};
+    hb::Arg args[2] = {{input, in_rec}, {output, out_rec}};
     if ((r = hb::check_args(args, 2))) return r;
     // the slice reads input(x,y) unclamped (generator :50): the input must cover the output region
     const hb::Region need[2] = {hb::region_of(output, true), hb::region_of(output, false)};
@@ -523,10 +555,10 @@ int run_bilateral_grid(halide_buffer_t *input, int s_sigma, float r_sigma, halid
         hb::CallTimer timer(s);
         BGSParams q;  // (the any-S kernels' shapes)
         if (s_sigma == S) {
-            hb::allow_smem(bg_hist_blurz_kernel, bins_bytes);
+            hb::allow_smem(bg_hist_blurz_kernel<T>, bins_bytes);
             dim3 g1((p.gw + 63) / 64, p.gh);
-            HB_LAUNCH("bg_hist_blurz", bg_hist_blurz_kernel, g1, 128, bins_bytes, s, p);
-        } else {
+            HB_LAUNCH("bg_hist_blurz", bg_hist_blurz_kernel<T>, g1, 128, bins_bytes, s, p);
+        } else if constexpr (std::is_same<T, float>::value) {
             q.S = s_sigma;
             q.inv_s = (float)(1.0 / (double)s_sigma);
             q.mag = (uint32_t)(((1u << kMagShift) + s_sigma - 1) / s_sigma);
@@ -548,9 +580,9 @@ int run_bilateral_grid(halide_buffer_t *input, int s_sigma, float r_sigma, halid
             const int tx0 = ox & ~(S - 1), ty0 = oy & ~(S - 1);
             dim3 g3((ox + W - tx0 + kSliceW - 1) / kSliceW, (oy + H - ty0 + S - 1) / S);
             const size_t slice_smem = (size_t)p.nz * 2 * kSlicePitch * sizeof(float2);
-            hb::allow_smem(bg_slice_kernel, slice_smem);
-            HB_LAUNCH("bg_slice", bg_slice_kernel, g3, dim3(32, 8), slice_smem, s, p);
-        } else {
+            hb::allow_smem(bg_slice_kernel<T>, slice_smem);
+            HB_LAUNCH("bg_slice", bg_slice_kernel<T>, g3, dim3(32, 8), slice_smem, s, p);
+        } else if constexpr (std::is_same<T, float>::value) {
             const int tw = 4 * q.tx, tx0 = ox & ~3;
             dim3 g3((H + q.th - 1) / q.th, (ox + W - tx0 + tw - 1) / tw);
             const size_t slice_smem = slice_s_bytes(q, p.nz);
@@ -558,13 +590,13 @@ int run_bilateral_grid(halide_buffer_t *input, int s_sigma, float r_sigma, halid
             HB_LAUNCH("bg_slice_s", bg_slice_s_kernel, g3, 256, slice_smem, s, p, q);
         }
     }
-    return hb::finish(args, 2, "bilateral_grid launch");
+    return hb::finish(args, 2, sizeof(T) == 1 ? "bilateral_grid_u8 launch" : "bilateral_grid launch");
 }
 
 }  // namespace
 
 extern "C" int bilateral_grid(halide_buffer_t *input, float r_sigma, halide_buffer_t *output) {
-    return run_bilateral_grid(input, S, r_sigma, output);
+    return run_bilateral_grid<float>(input, S, r_sigma, output, kArgs[0], kArgs[2]);
 }
 HB_EXPORT_FILTER(bilateral_grid, kArgs)
 HB_EXPORT_AUTO_SCHEDULE(bilateral_grid, kArgs)
@@ -573,5 +605,13 @@ HB_EXPORT_AUTO_SCHEDULE(bilateral_grid, kArgs)
 // kernels (bit for bit).  Buffer rules, error codes and the bounds query are bilateral_grid's.
 extern "C" int halide_b200_bilateral_grid_s_sigma(halide_buffer_t *input, int32_t s_sigma, float r_sigma,
                                                   halide_buffer_t *output) {
-    return run_bilateral_grid(input, s_sigma, r_sigma, output);
+    return run_bilateral_grid<float>(input, s_sigma, r_sigma, output, kArgs[0], kArgs[2]);
+}
+
+// 8-bit entry point (library extension): out8 = to_u8(bilateral_grid(to_f32(in8), r_sigma)) bit for bit, with the
+// reference's element conversions (to_f32(v) = v / 255.0f, to_u8(f) = lround(f * 255.0f)) done inside bg_hist_blurz and
+// bg_slice, the two kernels that read or write the frame.  Buffer rules, error codes and the bounds query are
+// bilateral_grid's.
+extern "C" int halide_b200_bilateral_grid_u8(halide_buffer_t *input, float r_sigma, halide_buffer_t *output) {
+    return run_bilateral_grid<uint8_t>(input, S, r_sigma, output, kU8Args[0], kU8Args[1]);
 }

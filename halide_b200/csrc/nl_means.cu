@@ -15,6 +15,9 @@
 //   A  d for all dx over the tile grown by the patch apron          -> smem D[dx][y][x]
 //   B  vertical patch sums                                          -> smem V[dx][y][x]
 //   C  horizontal patch sums, fast_exp, accumulate 4 running sums in registers (2 px per thread)
+// halide_b200_nl_means_u8 runs the same kernels on uint8 frames: they take the frame's element type T as a template
+// parameter and convert while they fill the float tile sI (hl::frame_to_f32) and in the final store (hl::frame_from_f32);
+// the phases in between are the float path's.
 #include "hb_common.h"
 #include "hl_math.cuh"
 
@@ -23,10 +26,10 @@ namespace {
 constexpr int TX = 32, TY = 16;  // output tile per block; 256 threads, 2 rows per thread
 
 struct NLParams {
-    const float *in;  // element at input mins
+    const float *in;  // element at input mins (a uint8_t frame's for the <uint8_t> kernels)
     int64_t in_sy, in_sc;
     int in_x0, in_y0, in_c0, in_w, in_h, in_c;
-    float *out;
+    float *out;       // (the same)
     int64_t out_sy, out_sc;
     int out_x0, out_y0, W, H;
     int p, s, p_lo, s_lo;  // patch/search extents and their first offsets (-(n/2))
@@ -36,6 +39,7 @@ struct NLParams {
     int dw, dh;            // D tile extent (TX + p - 1, TY + p - 1)
 };
 
+template<typename T>
 __global__ void __launch_bounds__(256) nl_means_kernel(NLParams q) {
     extern __shared__ float smem[];
     float *sI = smem;                              // [3][ih][iw]
@@ -51,7 +55,7 @@ __global__ void __launch_bounds__(256) nl_means_kernel(NLParams q) {
         int x = hl::clampi(ax0 + u, q.in_x0, q.in_x0 + q.in_w - 1) - q.in_x0;
         int y = hl::clampi(ay0 + v, q.in_y0, q.in_y0 + q.in_h - 1) - q.in_y0;
         int cc = hl::clampi(c, q.in_c0, q.in_c0 + q.in_c - 1) - q.in_c0;
-        sI[t] = __ldg(q.in + (int64_t)cc * q.in_sc + (int64_t)y * q.in_sy + x);
+        sI[t] = hl::frame_to_f32(__ldg(reinterpret_cast<const T *>(q.in) + (int64_t)cc * q.in_sc + (int64_t)y * q.in_sy + x));
     }
     __syncthreads();
     const int plane = q.ih * q.iw;
@@ -112,7 +116,7 @@ __global__ void __launch_bounds__(256) nl_means_kernel(NLParams q) {
             for (int c = 0; c < 3; c++) {
                 // (NaN -> 1: every weight is NaN when sigma^2 * patch^2 underflows and -1 / it is -inf)
                 float v = hl::clamp01(__fdiv_rn(acc[r][c], acc[r][3]));
-                q.out[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = v;
+                reinterpret_cast<T *>(q.out)[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = hl::frame_from_f32<T>(v);
             }
         }
     }
@@ -129,7 +133,7 @@ __global__ void __launch_bounds__(256) nl_means_kernel(NLParams q) {
 //   phase 2: as before (horizontal patch sum, fast_exp, four running sums per pixel, two rows per thread), unrolled.
 // All S offsets of a search row are batched between two barriers.  Same float operations in the same order as the
 // generic kernel (results are bit-identical to it; tests/test_nl_means_gpu.py runs both against the oracle).
-template<int P, int S>
+template<typename T, int P, int S>
 __global__ void __launch_bounds__(256) nl_means_window_kernel(NLParams q) {
     constexpr int IW = TX + P + S - 2, IH = TY + P + S - 2, DW = TX + P - 1, DH = TY + P - 1, PLANE = IH * IW;
     constexpr int PLO = -(P / 2), SLO = -(S / 2), OFFS = -SLO;
@@ -145,7 +149,7 @@ __global__ void __launch_bounds__(256) nl_means_window_kernel(NLParams q) {
         const int x = hl::clampi(ax0 + u, q.in_x0, q.in_x0 + q.in_w - 1) - q.in_x0;
         const int y = hl::clampi(ay0 + v, q.in_y0, q.in_y0 + q.in_h - 1) - q.in_y0;
         const int cc = hl::clampi(c, q.in_c0, q.in_c0 + q.in_c - 1) - q.in_c0;
-        sI[t] = __ldg(q.in + (int64_t)cc * q.in_sc + (int64_t)y * q.in_sy + x);
+        sI[t] = hl::frame_to_f32(__ldg(reinterpret_cast<const T *>(q.in) + (int64_t)cc * q.in_sc + (int64_t)y * q.in_sy + x));
     }
     __syncthreads();
     const int tx = tid & 31, ty = tid >> 5;  // rows ty and ty + 8
@@ -199,7 +203,7 @@ __global__ void __launch_bounds__(256) nl_means_window_kernel(NLParams q) {
 #pragma unroll
             for (int c = 0; c < 3; c++) {
                 const float v = hl::clamp01(__fdiv_rn(acc[r][c], acc[r][3]));
-                q.out[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = v;
+                reinterpret_cast<T *>(q.out)[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = hl::frame_from_f32<T>(v);
             }
         }
     }
@@ -221,15 +225,19 @@ const halide_filter_argument_t kArgs[5] = {
     {"sigma", halide_argument_kind_input_scalar, 0, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, &sv_sigma, nullptr},
     {"non_local_means", halide_argument_kind_output_buffer, 3, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
-}  // namespace
+// halide_b200_nl_means_u8: the same buffers in uint8.
+const halide_filter_argument_t kU8Args[2] = {
+    {"input", halide_argument_kind_input_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+    {"non_local_means", halide_argument_kind_output_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+};
 
-extern "C" void halide_b200_nl_means_variant(int v) {
-    g_variant = v;
-}
-
-extern "C" int nl_means(halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma, halide_buffer_t *output) {
+// nl_means on frames of element type T (float, or uint8_t for halide_b200_nl_means_u8) described by the argument records
+// in_rec / out_rec.
+template<typename T>
+int run_nl_means(halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma, halide_buffer_t *output,
+                 const halide_filter_argument_t &in_rec, const halide_filter_argument_t &out_rec) {
     int r;
-    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[4]}};
+    hb::Arg args[2] = {{input, in_rec}, {output, out_rec}};
     if ((r = hb::check_args(args, 2))) return r;
     // every input access is clamped: a query is answered with the output's x/y region and 3 channels
     const hb::Region region = {{output->dim[0].min, output->dim[1].min, 0}, {output->dim[0].extent, output->dim[1].extent, 3}, false};
@@ -286,17 +294,35 @@ extern "C" int nl_means(halide_buffer_t *input, int32_t patch_size, int32_t sear
         if (window && patch_size == 3 && search_area == 7) {
             constexpr size_t sm = nl_window_smem<3, 7>();
             static_assert(sm <= 48 * 1024, "no opt-in needed");
-            HB_LAUNCH("nl_means_window", (nl_means_window_kernel<3, 7>), grid, 256, sm, s, q);
+            HB_LAUNCH("nl_means_window", (nl_means_window_kernel<T, 3, 7>), grid, 256, sm, s, q);
         } else if (window && patch_size == 7 && search_area == 7) {
             constexpr size_t sm = nl_window_smem<7, 7>();
             static_assert(sm <= 48 * 1024, "no opt-in needed");
-            HB_LAUNCH("nl_means_window", (nl_means_window_kernel<7, 7>), grid, 256, sm, s, q);
+            HB_LAUNCH("nl_means_window", (nl_means_window_kernel<T, 7, 7>), grid, 256, sm, s, q);
         } else {
-            hb::allow_smem(nl_means_kernel, smem);
-            HB_LAUNCH("nl_means", nl_means_kernel, grid, 256, smem, s, q);
+            hb::allow_smem(nl_means_kernel<T>, smem);
+            HB_LAUNCH("nl_means", nl_means_kernel<T>, grid, 256, smem, s, q);
         }
     }
-    return hb::finish(args, 2, "nl_means launch");
+    return hb::finish(args, 2, sizeof(T) == 1 ? "nl_means_u8 launch" : "nl_means launch");
+}
+}  // namespace
+
+extern "C" void halide_b200_nl_means_variant(int v) {
+    g_variant = v;
+}
+
+extern "C" int nl_means(halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma, halide_buffer_t *output) {
+    return run_nl_means<float>(input, patch_size, search_area, sigma, output, kArgs[0], kArgs[4]);
 }
 HB_EXPORT_FILTER(nl_means, kArgs)
 HB_EXPORT_AUTO_SCHEDULE(nl_means, kArgs)
+
+// 8-bit entry point (library extension): out8 = to_u8(nl_means(to_f32(in8), patch_size, search_area, sigma)) bit for
+// bit, with the reference's element conversions (to_f32(v) = v / 255.0f, to_u8(f) = lround(f * 255.0f)) done inside the
+// kernels.  Buffer rules (channels clamped, the output's channels [0, 3)), parameter checks, error codes, the bounds query
+// and the variant hook are nl_means'.
+extern "C" int halide_b200_nl_means_u8(halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma,
+                                       halide_buffer_t *output) {
+    return run_nl_means<uint8_t>(input, patch_size, search_area, sigma, output, kU8Args[0], kU8Args[1]);
+}

@@ -126,6 +126,30 @@ def nl_means(input, patch_size, search_area, sigma, output):
                               ctypes.c_float(sigma), output.ptr))
 
 
+_U8_CONVERSIONS = """
+
+    The conversions are the reference's image I/O (image_io.convert): to_f32(v) = v / 255.0f, an IEEE float division, and
+    to_u8(f) = lround(f * 255.0f), the product rounded to float32 and then to the nearest integer with halves away from
+    zero.  Both run inside the kernels that read and write the frame: no float copy of either frame is made."""
+
+
+def bilateral_grid_u8(input, r_sigma, output):
+    return check(lib.halide_b200_bilateral_grid_u8(input.ptr, ctypes.c_float(r_sigma), output.ptr))
+
+
+def nl_means_u8(input, patch_size, search_area, sigma, output):
+    return check(lib.halide_b200_nl_means_u8(input.ptr, ctypes.c_int32(patch_size), ctypes.c_int32(search_area),
+                                             ctypes.c_float(sigma), output.ptr))
+
+
+bilateral_grid_u8.__doc__ = ("bilateral_grid on 2-D (x, y) uint8 buffers, e.g. an (H, W) uint8 torch tensor:\n"
+                             "output = to_u8(bilateral_grid(to_f32(input), r_sigma)) byte for byte.  Buffer rules and error "
+                             "codes as bilateral_grid." + _U8_CONVERSIONS)
+nl_means_u8.__doc__ = ("nl_means on 3-D (x, y, c) uint8 buffers, e.g. a (3, H, W) uint8 torch tensor:\n"
+                       "output = to_u8(nl_means(to_f32(input), patch_size, search_area, sigma)) byte for byte.  Buffer "
+                       "rules (output channels exactly [0, 3)) and error codes as nl_means." + _U8_CONVERSIONS)
+
+
 def camera_pipe(input, matrix_3200, matrix_7000, color_temp, gamma, contrast, sharpen_strength, blackLevel, whiteLevel,
                 processed):
     """apps/camera_pipe/camera_pipe_generator.cpp: uint16 Bayer raw -> uint8 RGB."""

@@ -330,6 +330,21 @@ int halide_b200_local_laplacian_u8_interleaved_batch(struct halide_buffer_t *inp
 int halide_b200_bilateral_grid_s_sigma(struct halide_buffer_t *input, int32_t s_sigma, float r_sigma,
                                        struct halide_buffer_t *output);
 
+/* The float pipelines bilateral_grid and nl_means on 8-bit frames (a decoded photo, a uint8 torch tensor):
+ *   halide_b200_bilateral_grid_u8(in8, r_sigma, out8) == to_u8(bilateral_grid(to_f32(in8), r_sigma))
+ *   halide_b200_nl_means_u8(in8, patch_size, search_area, sigma, out8)
+ *       == to_u8(nl_means(to_f32(in8), patch_size, search_area, sigma))
+ * byte for byte, with the element conversions of the reference's image I/O (tools/halide_image_io.h, Internal::convert):
+ * to_f32(v) = v / 255.0f (an IEEE division) and to_u8(f) = (uint8_t)lround(f * 255.0f) (the product rounded to float, then
+ * halves away from zero).  Both happen inside the kernels that read and write the frame, so no float copy of either frame
+ * exists.  Both buffers must be uint8 (else halide_error_code_bad_type); the float entry points keep refusing uint8.
+ * Dimensions, the input's coverage of the output (bilateral_grid), the output's channels [0, 3) (nl_means), the parameter
+ * checks and their order, empty outputs, size limits, error codes and the bounds query are those of the float entry
+ * point.  bilateral_grid_u8 runs s_sigma = 8. */
+int halide_b200_bilateral_grid_u8(struct halide_buffer_t *input, float r_sigma, struct halide_buffer_t *output);
+int halide_b200_nl_means_u8(struct halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma,
+                            struct halide_buffer_t *output);
+
 /* conv_layer (3x3 convolution + bias + relu, float32) at any shape: the generator's algorithm without its set_bounds /
  * set_stride constraints,
  *   relu(co, x, y, n) = max(0, bias(co) + sum over ky, kx, ci of filter(co, kx, ky, ci) * input(ci, x + kx, y + ky, n)).

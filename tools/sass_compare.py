@@ -8,8 +8,11 @@ halide_b200/csrc/local_laplacian.o in a scratch checkout, build this tree's, and
 Kernels are matched by demangled name.  A template parameter that a change appends with a default value changes the
 mangled name of every existing instantiation without changing its code, so the new object's names are also tried with
 such trailing defaults removed: the interleaved-layout parameters `bool IL = false` (ll_level1_kernel, the generic
-kernels), `int PI = 1, int PO = 1` (ll_up2_kernel) and the level set type `typename LS = LevelSet` (ll_coarse_fused_kernel).  Instruction addresses and padding are dropped before comparing; opcodes,
-operands and encodings must match.  Prints each old kernel that is missing or differs, then a count; exits 1 if any.
+kernels), `int PI = 1, int PO = 1` (ll_up2_kernel) and the level set type `typename LS = LevelSet` (ll_coarse_fused_kernel).  A kernel that gained the frame element type as its
+first template parameter is also tried without it when that type is float: `f<float>(` as the plain function `f(` (the
+demangled name of a template instance also carries its return type, `void `), `f<float, 3, 7>(` as `f<3, 7>(`
+(bg_hist_blurz_kernel, bg_slice_kernel, nl_means_kernel, nl_means_window_kernel).  Instruction addresses and padding are
+dropped before comparing; opcodes, operands and encodings must match.  Prints each old kernel that is missing or differs, then a count; exits 1 if any.
 """
 import re
 import subprocess
@@ -18,6 +21,8 @@ import sys
 CUOBJDUMP = "/usr/local/cuda/bin/cuobjdump"
 # trailing template arguments that stand for the defaults of appended parameters
 DEFAULT_TAILS = [", 1, 1>(", ", false>(", ", llk::LevelSet>("]
+# a leading element type parameter: its float instance against the kernel before it had the parameter
+FLOAT_HEADS = [(re.compile(r"^void (.*)<float>\("), r"\1("), (re.compile(r"<float, "), "<")]
 
 
 def kernels(obj):
@@ -49,6 +54,9 @@ def main():
         for tail in DEFAULT_TAILS:
             if tail in k:
                 by_name.setdefault(k.replace(tail, ">("), []).append(v)
+        for pat, repl in FLOAT_HEADS:
+            if pat.search(k):
+                by_name.setdefault(pat.sub(repl, k, count=1), []).append(v)
     bad = 0
     for k, v in old.items():
         cands = by_name.get(k, [])
