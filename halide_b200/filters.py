@@ -158,6 +158,57 @@ def camera_pipe(input, matrix_3200, matrix_7000, color_temp, gamma, contrast, sh
                                  ctypes.c_int32(blackLevel), ctypes.c_int32(whiteLevel), processed.ptr))
 
 
+def _camera_pipe_scalars(color_temp, gamma, contrast, sharpen_strength, blackLevel, whiteLevel):
+    return (ctypes.c_float(color_temp), ctypes.c_float(gamma), ctypes.c_float(contrast), ctypes.c_float(sharpen_strength),
+            ctypes.c_int32(blackLevel), ctypes.c_int32(whiteLevel))
+
+
+def camera_pipe_batch(input, matrix_3200, matrix_7000, color_temp, gamma, contrast, sharpen_strength, blackLevel,
+                      whiteLevel, processed):
+    """camera_pipe on every frame of a raw burst, in one launch: input (x, y, n), e.g. an (N, H, W) uint16 tensor, and a
+    planar output (x, y, c, n), e.g. an (N, 3, H, W) uint8 tensor.  Output frame n is camera_pipe(input frame n) byte for
+    byte; the matrices and scalars are shared by all frames.  The input must cover the raw region camera_pipe needs and
+    the output's frames, else -4."""
+    return check(lib.halide_b200_camera_pipe_batch(input.ptr, matrix_3200.ptr, matrix_7000.ptr,
+                                                   *_camera_pipe_scalars(color_temp, gamma, contrast, sharpen_strength,
+                                                                         blackLevel, whiteLevel), processed.ptr))
+
+
+_CAMERA_PIPE_INTERLEAVED = """
+    The output is pixel-interleaved (RGBRGB..., RGBA...): ``dim[2].stride == 1``, ``dim[0].stride`` is the pixel pitch, at
+    least the channel extent, and ``dim[1].stride`` (and ``dim[3].stride``) positive; anything else, a planar buffer
+    included, is refused with -8.  The bytes are those the planar entry point writes, transposed; samples the output's
+    channels do not cover (the alpha of an RGBA frame) are left untouched.  The common outputs:
+
+    - an ``(N, H, W, 3)`` uint8 tensor (torchvision's video layout) passed as ``t.permute(0, 3, 1, 2)``, or an
+      ``(N, 3, H, W)`` tensor in ``torch.channels_last`` memory format, which ``HalideBuffer.from_torch`` already
+      describes as interleaved;
+    - a numpy ``(H, W, 3)`` array (PIL, OpenCV, image encoders): ``HalideBuffer.from_numpy(arr.transpose(2, 0, 1))``.
+    """
+
+
+def camera_pipe_interleaved(input, matrix_3200, matrix_7000, color_temp, gamma, contrast, sharpen_strength, blackLevel,
+                            whiteLevel, processed):
+    return check(lib.halide_b200_camera_pipe_interleaved(input.ptr, matrix_3200.ptr, matrix_7000.ptr,
+                                                         *_camera_pipe_scalars(color_temp, gamma, contrast, sharpen_strength,
+                                                                               blackLevel, whiteLevel), processed.ptr))
+
+
+def camera_pipe_interleaved_batch(input, matrix_3200, matrix_7000, color_temp, gamma, contrast, sharpen_strength,
+                                  blackLevel, whiteLevel, processed):
+    return check(lib.halide_b200_camera_pipe_interleaved_batch(input.ptr, matrix_3200.ptr, matrix_7000.ptr,
+                                                               *_camera_pipe_scalars(color_temp, gamma, contrast,
+                                                                                     sharpen_strength, blackLevel,
+                                                                                     whiteLevel), processed.ptr))
+
+
+camera_pipe_interleaved.__doc__ = ("camera_pipe into a 3-D (x, y, c) uint8 interleaved output; the raw input is camera_pipe's "
+                                   "(H, W) uint16 frame.\n" + _CAMERA_PIPE_INTERLEAVED)
+camera_pipe_interleaved_batch.__doc__ = ("camera_pipe_batch into a 4-D (x, y, c, n) uint8 interleaved output: a raw burst, an "
+                                         "(N, H, W) uint16 tensor, to (N, H, W, 3) RGB in one launch.\n" +
+                                         _CAMERA_PIPE_INTERLEAVED)
+
+
 def conv_layer(input, filter, bias, relu):
     """apps/conv_layer/conv_layer_generator.cpp: 3x3 conv + bias + relu, fixed shapes (N5 CI128 CO128 100x80), f32."""
     return check(lib.conv_layer(input.ptr, filter.ptr, bias.ptr, relu.ptr))

@@ -323,6 +323,34 @@ int halide_b200_local_laplacian_u8_interleaved(struct halide_buffer_t *input, in
 int halide_b200_local_laplacian_u8_interleaved_batch(struct halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                                      struct halide_buffer_t *output);
 
+/* camera_pipe on raw bursts and into pixel-interleaved RGB.  Matrices and scalars are camera_pipe's, in the same order,
+ * and shared by every frame; the tables they give are computed once per call, and every frame runs in one launch.
+ *   halide_b200_camera_pipe_batch:             input uint16 (x, y, n), processed uint8 (x, y, c, n), planar;
+ *   halide_b200_camera_pipe_interleaved:       input uint16 (x, y),    processed uint8 (x, y, c), interleaved;
+ *   halide_b200_camera_pipe_interleaved_batch: input uint16 (x, y, n), processed uint8 (x, y, c, n), interleaved.
+ * Output frame n (absolute coordinate) is, byte for byte, camera_pipe(input frame n), and the same bytes the planar entry
+ * point gives on planar copies.  Checks, in camera_pipe's order: types (else halide_error_code_bad_type) and dimension
+ * counts (else halide_error_code_bad_dimensions); the bounds query; the layout rules; an empty output (W, H, C or N 0)
+ * returns 0; the input must cover, in x and y, the raw region camera_pipe reads for the output's x and y region and, in n,
+ * the output's frames, and the output's channels must lie in [0, 3) (else halide_error_code_access_out_of_bounds).
+ * Layout: the raw input and a planar output keep camera_pipe's dim[0].stride == 1; an interleaved output must have
+ * dim[2].stride == 1, dim[0].stride (the pixel pitch) >= dim[2].extent and positive dim[1].stride (and dim[3].stride),
+ * else halide_error_code_constraint_violated.  Samples an interleaved output's channels do not cover (an RGBA frame's
+ * alpha under channels [0, 3)) keep their bytes.  A bounds query proposes the raw region over the output's frames with
+ * dense strides, and an interleaved output dense interleaved strides (C, W*C, 1[, W*H*C]). */
+int halide_b200_camera_pipe_batch(struct halide_buffer_t *input, struct halide_buffer_t *matrix_3200,
+                                  struct halide_buffer_t *matrix_7000, float color_temp, float gamma, float contrast,
+                                  float sharpen_strength, int32_t blackLevel, int32_t whiteLevel,
+                                  struct halide_buffer_t *processed);
+int halide_b200_camera_pipe_interleaved(struct halide_buffer_t *input, struct halide_buffer_t *matrix_3200,
+                                        struct halide_buffer_t *matrix_7000, float color_temp, float gamma, float contrast,
+                                        float sharpen_strength, int32_t blackLevel, int32_t whiteLevel,
+                                        struct halide_buffer_t *processed);
+int halide_b200_camera_pipe_interleaved_batch(struct halide_buffer_t *input, struct halide_buffer_t *matrix_3200,
+                                              struct halide_buffer_t *matrix_7000, float color_temp, float gamma,
+                                              float contrast, float sharpen_strength, int32_t blackLevel, int32_t whiteLevel,
+                                              struct halide_buffer_t *processed);
+
 /* bilateral_grid with its s_sigma GeneratorParam (the grid cell size in pixels, 8 in bilateral_grid) as an argument:
  * the result is what the generator built with s_sigma computes.  s_sigma must be in [1, 128] (else
  * halide_error_code_param_too_small / _too_large, checked after the buffer checks and the bounds query, before any CUDA
