@@ -153,44 +153,82 @@ void fill_frame(PlanT<T> &p, const hb::Arg *args, int levels, float alpha, float
 // after call: the 2*256*(levels-1)+1 halide_exp evaluations and their launch are kept per device and reused.  The table
 // is immutable once built (a change of parameters builds a new one; the old ones are kept: kernels of an earlier call
 // may still be reading them on another stream), and it is built synchronously, so any stream may read it afterwards.
+// A call holds its table (holders > 0, LutHold) from the lookup until its last launch that reads it is enqueued: another
+// thread's miss may evict in between, and cudaDeviceSynchronize only waits for work already enqueued.  Eviction frees the
+// unheld tables once 64 of them are cached; held ones stay until a later eviction.
 struct LutEntry {
     int device, levels;
     float alpha;
     float *lut;
+    int holders;
 };
 std::mutex g_lut_mu;
 std::vector<LutEntry> g_luts;
 
-template<typename T>
-int get_lut(PlanT<T> &p, cudaStream_t s) {
+// The table of (current device, levels, alpha), built on stream s if missing, with one hold taken on it.
+int lut_acquire(int levels, float alpha, cudaStream_t s, float **out) {
     int dev = 0;
     cudaGetDevice(&dev);
     std::lock_guard<std::mutex> lock(g_lut_mu);
-    for (const LutEntry &e : g_luts) {
-        if (e.device == dev && e.levels == p.f.levels && memcmp(&e.alpha, &p.alpha, sizeof(float)) == 0) {
-            p.f.lut = e.lut;
+    for (LutEntry &e : g_luts) {
+        if (e.device == dev && e.levels == levels && memcmp(&e.alpha, &alpha, sizeof(float)) == 0) {
+            e.holders++;
+            *out = e.lut;
             return 0;
         }
     }
-    if (g_luts.size() >= 64) {  // a caller sweeping alpha: drop the oldest tables once nothing can still be reading them
+    // a caller sweeping alpha: drop the unheld tables once nothing can still be reading them
+    if (std::count_if(g_luts.begin(), g_luts.end(), [](const LutEntry &e) { return e.holders == 0; }) >= 64) {
         cudaDeviceSynchronize();
-        for (const LutEntry &e : g_luts) cudaFree(e.lut);
-        g_luts.clear();
+        auto unheld = std::stable_partition(g_luts.begin(), g_luts.end(), [](const LutEntry &e) { return e.holders > 0; });
+        for (auto it = unheld; it != g_luts.end(); ++it) cudaFree(it->lut);
+        g_luts.erase(unheld, g_luts.end());
     }
     float *lut = nullptr;
-    const int n = 2 * p.f.lut_half + 1;
+    const int lut_half = 256 * (levels - 1), n = 2 * lut_half + 1;
     if (cudaMalloc((void **)&lut, ((size_t)n + 3) / 4 * 16) != cudaSuccess) {
         cudaGetLastError();
         return hb::fail(halide_error_code_device_malloc_failed, "local_laplacian: remap table allocation failed");
     }
-    HB_LAUNCH("ll_lut", ll_lut_kernel, (n + 255) / 256, 256, 0, s, lut, p.f.lut_half, p.alpha);
+    HB_LAUNCH("ll_lut", ll_lut_kernel, (n + 255) / 256, 256, 0, s, lut, lut_half, alpha);
     if (cudaStreamSynchronize(s) != cudaSuccess) {
         cudaGetLastError();
         cudaFree(lut);
         return hb::fail(halide_error_code_device_run_failed, "local_laplacian: remap table kernel failed");
     }
-    g_luts.push_back({dev, p.f.levels, p.alpha, lut});
-    p.f.lut = lut;
+    g_luts.push_back({dev, levels, alpha, lut, 1});
+    *out = lut;
+    return 0;
+}
+
+// Drops one hold taken by lut_acquire; false if the table is not held.
+bool lut_release(const float *lut) {
+    std::lock_guard<std::mutex> lock(g_lut_mu);
+    for (LutEntry &e : g_luts) {
+        if (e.lut == lut && e.holders > 0) {
+            e.holders--;
+            return true;
+        }
+    }
+    return false;
+}
+
+// A call's hold on its remap table, dropped when the call returns (after its last launch, or on an error).
+struct LutHold {
+    float *lut = nullptr;
+    LutHold() = default;
+    LutHold(const LutHold &) = delete;
+    LutHold &operator=(const LutHold &) = delete;
+    ~LutHold() {
+        if (lut) lut_release(lut);
+    }
+};
+
+template<typename T>
+int get_lut(PlanT<T> &p, cudaStream_t s, LutHold &hold) {
+    int r;
+    if ((r = lut_acquire(p.f.levels, p.alpha, s, &hold.lut))) return r;
+    p.f.lut = hold.lut;
     return 0;
 }
 
@@ -565,7 +603,8 @@ int run_local_laplacian(hb::Arg *args, int levels, float alpha, float beta, int 
     if ((r = alloc_levels(p, ll::make_geom(outx, outy, inx, iny, J), scratch))) return r;
 
     cudaStream_t s = hb::stream();
-    if ((r = get_lut(p, s))) return r;
+    LutHold lut;
+    if ((r = get_lut(p, s, lut))) return r;
     {
         hb::CallTimer timer(s);
         if constexpr (std::is_same<T, uint16_t>::value) {
@@ -787,7 +826,8 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
     p.f.halo_top_rows = ht; p.f.halo_bot_rows = hbn;
 
     cudaStream_t s = hb::stream();
-    if ((r = get_lut(p, s))) return r;
+    LutHold lut;  // (held through the exchanges too: this rank waits there for its peers before it launches)
+    if ((r = get_lut(p, s, lut))) return r;
     // A halo pack that fails is reported only once the call is over: every rank still enters each exchange of the call,
     // so that no neighbour is left waiting for this one.
     cudaError_t pack_err = cudaSuccess;
@@ -921,6 +961,31 @@ int run_local_laplacian_sharded(halide_buffer_t *input, int levels, float alpha,
 // Test hook: route K == 8 calls through the generic (any `levels`) kernels so both paths stay covered.
 extern "C" void halide_b200_ll_force_generic(int enable) {
     g_force_naive = enable;
+}
+
+// Test hook: take (hold = 1) or drop (hold = 0) one hold on the remap table of (levels, alpha) on the current device, as a
+// call does between its lookup and its last launch; taking builds the table (on the calling thread's stream) if it is
+// missing.  A held table survives evictions.  0, or a negative halide_error_code_t.
+extern "C" int halide_b200_ll_lut_hold(int32_t levels, float alpha, int32_t hold) {
+    if (levels < 2 || levels > 32) {
+        return hb::fail(levels < 2 ? halide_error_code_param_too_small : halide_error_code_param_too_large,
+                        "Parameter levels is %d but must be in [2, 32]", levels);
+    }
+    float *lut = nullptr;
+    if (hold) return lut_acquire(levels, alpha, hb::stream(), &lut);
+    int dev = 0;
+    cudaGetDevice(&dev);
+    {
+        std::lock_guard<std::mutex> lock(g_lut_mu);
+        for (const LutEntry &e : g_luts) {
+            if (e.device == dev && e.levels == levels && memcmp(&e.alpha, &alpha, sizeof(float)) == 0) lut = e.lut;
+        }
+    }
+    if (!lut || !lut_release(lut)) {
+        return hb::fail(halide_error_code_generic_error, "halide_b200_ll_lut_hold: the remap table of levels %d, alpha %g is not held",
+                        levels, (double)alpha);
+    }
+    return 0;
 }
 
 // Row-sharded path: which pyramid level is gathered all-to-all (see run_local_laplacian_sharded).  Collective

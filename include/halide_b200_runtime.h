@@ -422,6 +422,10 @@ int halide_b200_ll_shard_plan_level(int32_t frame_w, int32_t frame_h, int32_t nr
  * 8 no fused coarse launch, 16 general-layout final kernel, 64 no TMA frame tile in the final
  * kernel) so every code path stays covered by the parity tests. */
 void halide_b200_ll_force_generic(int mask);
+/* Test hook: take (hold = 1) or drop (hold = 0) one hold on local_laplacian's cached remap table of (levels, alpha), as a
+ * call does from its lookup to its last launch; taking builds the table if it is missing.  A held table is never evicted
+ * from the cache.  0, or a negative halide_error_code_t (dropping a table that is not held: generic_error). */
+int halide_b200_ll_lut_hold(int32_t levels, float alpha, int32_t hold);
 /* halide_blur test hook: 1 = route 4-byte-aligned frames through the general (any alignment) kernel as well;
  * >= 8 = aligned kernel with strips of that many rows (0 restores the defaults). */
 void halide_b200_blur_force_general(int enable);
