@@ -375,8 +375,8 @@ void launch_down(PlanT<T> &p, int j, cudaStream_t s) {  // produce level j (j >=
         for_frame_groups(p, [&](int n0, int nf) {
             dim3 g = grid_for(lb[1].sx.n(), lb[1].cy.n());
             g.z = nf;
-            HB_LAUNCH("ll_level1_generic", (p.il ? ll_level1_naive_kernel<T, true> : ll_level1_naive_kernel<T, false>), g, kBlk, 0, s,
-                      at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), p.fs);
+            HB_LAUNCH("ll_level1_generic", ll_level1_naive_kernel<T>, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0),
+                      p.fs);
         });
     } else {
         const int js = fs_slot(p, j);
@@ -506,8 +506,7 @@ void launch_final(PlanT<T> &p, cudaStream_t s) {
         for_frame_groups(p, [&](int n0, int nf) {
             dim3 g = grid_for(p.f.W, p.f.H);
             g.z = nf;
-            HB_LAUNCH("ll_final", (p.il ? ll_final_naive_kernel<T, true> : ll_final_naive_kernel<T, false>), g, kBlk, 0, s, at_frame(p.f, p.fs, n0),
-                      at_frame(lb[1], 1, p.fs, n0), 1, p.fs);
+            HB_LAUNCH("ll_final", ll_final_naive_kernel<T>, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), 1, p.fs);
         });
     }
 }

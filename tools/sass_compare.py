@@ -7,8 +7,8 @@ halide_b200/csrc/local_laplacian.o in a scratch checkout, build this tree's, and
 
 Kernels are matched by demangled name.  A template parameter that a change appends with a default value changes the
 mangled name of every existing instantiation without changing its code, so the new object's names are also tried with
-such trailing defaults removed: the interleaved-layout parameters `bool IL = false` (ll_level1_kernel, the generic
-kernels), `int PI = 1, int PO = 1` (ll_up2_kernel) and the level set type `typename LS = LevelSet` (ll_coarse_fused_kernel).  A kernel that gained the frame element type as its
+such trailing defaults removed: the interleaved-layout parameters `bool IL = false` (ll_level1_kernel),
+`int PI = 1, int PO = 1` (ll_up2_kernel) and the level set type `typename LS = LevelSet` (ll_coarse_fused_kernel).  A kernel that gained the frame element type as its
 first template parameter is also tried without it when that type is float: `f<float>(` as the plain function `f(` (the
 demangled name of a template instance also carries its return type, `void `), `f<float, 3, 7>(` as `f<3, 7>(`
 (bg_hist_blurz_kernel, bg_slice_kernel, nl_means_kernel, nl_means_window_kernel).  Instruction addresses and padding are
