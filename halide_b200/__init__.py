@@ -12,5 +12,6 @@ from .buffer import HalideBuffer, halide_buffer_t, halide_dimension_t  # noqa: F
 from .lib import lib as capi, load_library, HalideError, capture_errors  # noqa: F401
 from . import lib  # noqa: F401  (module: loader + profile helpers)
 from . import filters  # noqa: F401
+from . import nl_means_video  # noqa: F401  (batch and interleaved nl_means)
 from .pipeline import FramePipeline  # noqa: F401
 from . import image_io  # noqa: F401  (host-side: file formats + the reference's type-conversion rules)

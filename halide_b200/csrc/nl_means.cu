@@ -18,15 +18,25 @@
 // halide_b200_nl_means_u8 runs the same kernels on uint8 frames: they take the frame's element type T as a template
 // parameter and convert while they fill the float tile sI (hl::frame_to_f32) and in the final store (hl::frame_from_f32);
 // the phases in between are the float path's.
+//
+// The batch and interleaved entry points run the same kernels too, with two more template parameters: IL (the frames are
+// pixel-interleaved: the tile fill reads them in memory order and the final store writes a pixel's channels side by side)
+// and FR (the grid's blocks walk the frames of a 4-D buffer, frame n = blockIdx.z, + gridDim.z, ...).  Only the fill of
+// sI and the final store differ; the phases, and so every float operation, are the planar one-frame kernels'.
+#include <algorithm>
+#include <type_traits>
+
 #include "hb_common.h"
 #include "hl_math.cuh"
 
 namespace {
 
 constexpr int TX = 32, TY = 16;  // output tile per block; 256 threads, 2 rows per thread
+constexpr int kMaxGridZ = 65535;  // grid z extent limit: larger batches are walked by the blocks
 
 struct NLParams {
-    const float *in;  // element at input mins (a uint8_t frame's for the <uint8_t> kernels)
+    const float *in;  // element at input mins (a uint8_t frame's for the <uint8_t> kernels; a batch's: of the input frame
+                      // that output frame 0 reads)
     int64_t in_sy, in_sc;
     int in_x0, in_y0, in_c0, in_w, in_h, in_c;
     float *out;       // (the same)
@@ -38,24 +48,104 @@ struct NLParams {
     int iw, ih;            // input tile extent (TX + p + s - 2, TY + p + s - 2)
     int dw, dh;            // D tile extent (TX + p - 1, TY + p - 1)
 };
+// The parameters of the IL and FR kernels: NLParams and, after it, the frame strides and pixel pitches.  (A separate
+// type, so that the planar one-frame kernels keep their parameter block byte for byte: any field appended to it changes
+// their code.)
+struct NLVideoParams : NLParams {
+    int64_t in_sn, out_sn;  // frame strides (FR kernels)
+    int in_px, out_px;      // pixel pitches (IL kernels, whose channel strides in_sc / out_sc are 1)
+    int N;                  // frames (FR kernels)
+};
 
+// The IL tile fill: sI[c][v][u] (planes of npix = ih * iw floats) from an interleaved frame.  The warp's loads take the
+// tile's samples in memory order, channel innermost (32 consecutive samples of a pixel row per load), and a warp
+// shuffle hands each lane the three channels of one pixel, so that each store writes 32 consecutive floats of one plane:
+// storing the loaded samples directly would put the three channels of a pixel into one bank (npix is a multiple of 32
+// at patch 3 / search 7).  Channels clamp to the input's as in the planar fill.
 template<typename T>
-__global__ void __launch_bounds__(256) nl_means_kernel(NLParams q) {
+__device__ __forceinline__ void fill_tile_interleaved(float *sI, const NLVideoParams &q, const T *in, int tid, int ax0, int ay0,
+                                                      int iw, int npix) {
+    const int lane = tid & 31;
+    for (int p0 = (tid >> 5) * 32; p0 < npix; p0 += 256) {  // (warp-uniform: every lane takes the shuffles)
+        float smp[3];  // samples 3 * p0 + 32 * k + lane of the tile, pixel (that / 3), channel (that % 3)
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            const int j = 3 * p0 + 32 * k + lane, pix = j / 3, c = j - 3 * pix;
+            smp[k] = 0.f;
+            if (pix < npix) {
+                const int v = pix / iw, u = pix - v * iw;
+                const int x = hl::clampi(ax0 + u, q.in_x0, q.in_x0 + q.in_w - 1) - q.in_x0;
+                const int y = hl::clampi(ay0 + v, q.in_y0, q.in_y0 + q.in_h - 1) - q.in_y0;
+                const int cc = hl::clampi(c, q.in_c0, q.in_c0 + q.in_c - 1) - q.in_c0;
+                smp[k] = hl::frame_to_f32(__ldg(in + (int64_t)y * q.in_sy + (int64_t)x * q.in_px + cc));
+            }
+        }
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            // Lane p takes sample 3p + c, held in smp[(3p + c) / 32] of lane (3p + c) % 32.  This lane holds it for the one
+            // p with 3p + c == lane (mod 32), p = 11 (lane - c) mod 32 (3 * 11 == 1 mod 32), and sends that register.
+            const int p = ((lane - c) * 11) & 31, k = (3 * p + c) >> 5;
+            const float send = k == 0 ? smp[0] : (k == 1 ? smp[1] : smp[2]);
+            const float got = __shfl_sync(0xffffffffu, send, (3 * lane + c) & 31);
+            if (p0 + lane < npix) sI[c * npix + p0 + lane] = got;
+        }
+    }
+}
+
+// Frame n's input (the element at the input's x/y/c mins) and output (at the output's mins), formed where they are used;
+// the one-frame kernels (FR false) read q.in and q.out there as they always did.
+template<typename T, bool FR, typename Q>
+__device__ __forceinline__ const T *frame_in(const Q &q, int n) {
+    if constexpr (FR) return reinterpret_cast<const T *>(q.in) + n * q.in_sn;
+    else return reinterpret_cast<const T *>(q.in);
+}
+template<typename T, bool FR, typename Q>
+__device__ __forceinline__ T *frame_out(const Q &q, int n) {
+    if constexpr (FR) return reinterpret_cast<T *>(q.out) + n * q.out_sn;
+    else return reinterpret_cast<T *>(q.out);
+}
+template<bool FR, typename Q>
+__device__ __forceinline__ int frames(const Q &q) {
+    if constexpr (FR) return q.N;
+    else return 1;
+}
+
+// The thread index, read anew for every frame of an FR kernel: read once, everything the phases derive from it is
+// invariant across the frame loop and the compiler keeps it live across the frames (the planar window kernels then take
+// 62-64 registers instead of 32, and the uint8 one at 3/7 spills).
+template<bool FR>
+__device__ __forceinline__ int thread_index() {
+    if constexpr (FR) {
+        int tid;
+        asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
+        return tid;
+    } else {
+        return threadIdx.x;
+    }
+}
+
+// nl_means_kernel on frame n; Q = NLParams for the planar one-frame kernels (IL and FR false), else NLVideoParams.
+template<typename T, bool IL, bool FR, typename Q>
+__device__ __forceinline__ void nl_means_frame(const Q &q, int n) {
     extern __shared__ float smem[];
     float *sI = smem;                              // [3][ih][iw]
     float *sD = sI + 3 * q.ih * q.iw;              // [nd][dh][dw]
     float *sV = sD + q.nd * q.dh * q.dw;           // [nd][TY][dw]
-    const int tid = threadIdx.x;
+    const int tid = thread_index<FR>();
     const int X0 = q.out_x0 + blockIdx.x * TX, Y0 = q.out_y0 + blockIdx.y * TY;
     // tile coordinate (u,v) <-> absolute (X0 + p_lo + s_lo + u, Y0 + p_lo + s_lo + v)
     const int ax0 = X0 + q.p_lo + q.s_lo, ay0 = Y0 + q.p_lo + q.s_lo;
-    for (int t = tid; t < 3 * q.ih * q.iw; t += 256) {
-        int c = t / (q.ih * q.iw), rem = t - c * q.ih * q.iw;
-        int v = rem / q.iw, u = rem - v * q.iw;
-        int x = hl::clampi(ax0 + u, q.in_x0, q.in_x0 + q.in_w - 1) - q.in_x0;
-        int y = hl::clampi(ay0 + v, q.in_y0, q.in_y0 + q.in_h - 1) - q.in_y0;
-        int cc = hl::clampi(c, q.in_c0, q.in_c0 + q.in_c - 1) - q.in_c0;
-        sI[t] = hl::frame_to_f32(__ldg(reinterpret_cast<const T *>(q.in) + (int64_t)cc * q.in_sc + (int64_t)y * q.in_sy + x));
+    if constexpr (IL) {
+        fill_tile_interleaved(sI, q, frame_in<T, FR>(q, n), tid, ax0, ay0, q.iw, q.ih * q.iw);
+    } else {
+        for (int t = tid; t < 3 * q.ih * q.iw; t += 256) {
+            int c = t / (q.ih * q.iw), rem = t - c * q.ih * q.iw;
+            int v = rem / q.iw, u = rem - v * q.iw;
+            int x = hl::clampi(ax0 + u, q.in_x0, q.in_x0 + q.in_w - 1) - q.in_x0;
+            int y = hl::clampi(ay0 + v, q.in_y0, q.in_y0 + q.in_h - 1) - q.in_y0;
+            int cc = hl::clampi(c, q.in_c0, q.in_c0 + q.in_c - 1) - q.in_c0;
+            sI[t] = hl::frame_to_f32(__ldg(frame_in<T, FR>(q, n) + (int64_t)cc * q.in_sc + (int64_t)y * q.in_sy + x));
+        }
     }
     __syncthreads();
     const int plane = q.ih * q.iw;
@@ -116,9 +206,23 @@ __global__ void __launch_bounds__(256) nl_means_kernel(NLParams q) {
             for (int c = 0; c < 3; c++) {
                 // (NaN -> 1: every weight is NaN when sigma^2 * patch^2 underflows and -1 / it is -inf)
                 float v = hl::clamp01(__fdiv_rn(acc[r][c], acc[r][3]));
-                reinterpret_cast<T *>(q.out)[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = hl::frame_from_f32<T>(v);
+                T *out = frame_out<T, FR>(q, n);
+                if constexpr (IL) out[(int64_t)ly * q.out_sy + (int64_t)lx * q.out_px + c] = hl::frame_from_f32<T>(v);
+                else out[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = hl::frame_from_f32<T>(v);
             }
         }
+    }
+}
+template<typename T, bool IL = false, bool FR = false>
+__global__ void __launch_bounds__(256) nl_means_kernel(NLParams q) {
+    static_assert(!IL && !FR, "the IL and FR kernels take NLVideoParams");
+    nl_means_frame<T, false, false>(q, 0);
+}
+template<typename T, bool IL, bool FR>
+__global__ void __launch_bounds__(256) nl_means_kernel(NLVideoParams q) {
+    for (int n = FR ? blockIdx.z : 0; n < frames<FR>(q); n += FR ? gridDim.z : 1) {
+        if (n != (int)blockIdx.z) __syncthreads();  // the previous frame's last phase C may still read sI
+        nl_means_frame<T, IL, FR>(q, n);
     }
 }
 
@@ -133,23 +237,28 @@ __global__ void __launch_bounds__(256) nl_means_kernel(NLParams q) {
 //   phase 2: as before (horizontal patch sum, fast_exp, four running sums per pixel, two rows per thread), unrolled.
 // All S offsets of a search row are batched between two barriers.  Same float operations in the same order as the
 // generic kernel (results are bit-identical to it; tests/test_nl_means_gpu.py runs both against the oracle).
-template<typename T, int P, int S>
-__global__ void __launch_bounds__(256) nl_means_window_kernel(NLParams q) {
+// (A frame's last search row ends in a barrier after its last read of sI and sV: the next frame's fill needs no other.)
+template<typename T, int P, int S, bool IL, bool FR, typename Q>
+__device__ __forceinline__ void nl_means_window_frame(const Q &q, int n) {
     constexpr int IW = TX + P + S - 2, IH = TY + P + S - 2, DW = TX + P - 1, DH = TY + P - 1, PLANE = IH * IW;
     constexpr int PLO = -(P / 2), SLO = -(S / 2), OFFS = -SLO;
     extern __shared__ float smem[];
     float *sI = smem;             // [3][IH][IW]
     float *sV = sI + 3 * PLANE;   // [S][TY][DW]
-    const int tid = threadIdx.x;
+    const int tid = thread_index<FR>();
     const int X0 = q.out_x0 + blockIdx.x * TX, Y0 = q.out_y0 + blockIdx.y * TY;
     const int ax0 = X0 + PLO + SLO, ay0 = Y0 + PLO + SLO;  // tile (u, v) <-> absolute (ax0 + u, ay0 + v)
-    for (int t = tid; t < 3 * PLANE; t += 256) {
-        const int c = t / PLANE, rem = t - c * PLANE;
-        const int v = rem / IW, u = rem - v * IW;
-        const int x = hl::clampi(ax0 + u, q.in_x0, q.in_x0 + q.in_w - 1) - q.in_x0;
-        const int y = hl::clampi(ay0 + v, q.in_y0, q.in_y0 + q.in_h - 1) - q.in_y0;
-        const int cc = hl::clampi(c, q.in_c0, q.in_c0 + q.in_c - 1) - q.in_c0;
-        sI[t] = hl::frame_to_f32(__ldg(reinterpret_cast<const T *>(q.in) + (int64_t)cc * q.in_sc + (int64_t)y * q.in_sy + x));
+    if constexpr (IL) {
+        fill_tile_interleaved(sI, q, frame_in<T, FR>(q, n), tid, ax0, ay0, IW, PLANE);
+    } else {
+        for (int t = tid; t < 3 * PLANE; t += 256) {
+            const int c = t / PLANE, rem = t - c * PLANE;
+            const int v = rem / IW, u = rem - v * IW;
+            const int x = hl::clampi(ax0 + u, q.in_x0, q.in_x0 + q.in_w - 1) - q.in_x0;
+            const int y = hl::clampi(ay0 + v, q.in_y0, q.in_y0 + q.in_h - 1) - q.in_y0;
+            const int cc = hl::clampi(c, q.in_c0, q.in_c0 + q.in_c - 1) - q.in_c0;
+            sI[t] = hl::frame_to_f32(__ldg(frame_in<T, FR>(q, n) + (int64_t)cc * q.in_sc + (int64_t)y * q.in_sy + x));
+        }
     }
     __syncthreads();
     const int tx = tid & 31, ty = tid >> 5;  // rows ty and ty + 8
@@ -203,10 +312,30 @@ __global__ void __launch_bounds__(256) nl_means_window_kernel(NLParams q) {
 #pragma unroll
             for (int c = 0; c < 3; c++) {
                 const float v = hl::clamp01(__fdiv_rn(acc[r][c], acc[r][3]));
-                reinterpret_cast<T *>(q.out)[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = hl::frame_from_f32<T>(v);
+                T *out = frame_out<T, FR>(q, n);
+                if constexpr (IL) out[(int64_t)ly * q.out_sy + (int64_t)lx * q.out_px + c] = hl::frame_from_f32<T>(v);
+                else out[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = hl::frame_from_f32<T>(v);
             }
         }
     }
+}
+template<typename T, int P, int S, bool IL = false, bool FR = false>
+__global__ void __launch_bounds__(256) nl_means_window_kernel(NLParams q) {
+    static_assert(!IL && !FR, "the IL and FR kernels take NLVideoParams");
+    nl_means_window_frame<T, P, S, false, false>(q, 0);
+}
+// The uint8 IL kernels are held to 8 blocks per SM, which the planar kernels reach with 32 registers: left to itself the
+// compiler gives them 40, room for 6 blocks, and the interleaved call at 3/7 takes 1.08x the planar one's time at 4K
+// instead of 1.06x.  The same bound on the other kernels, which take 32 registers anyway, slows them by 2-3 %.
+template<typename T, bool IL>
+constexpr bool kHeldTo8 = IL && sizeof(T) == 1;
+template<typename T, int P, int S, bool IL, bool FR, std::enable_if_t<!kHeldTo8<T, IL>, int> = 0>
+__global__ void __launch_bounds__(256) nl_means_window_kernel(NLVideoParams q) {
+    for (int n = FR ? blockIdx.z : 0; n < frames<FR>(q); n += FR ? gridDim.z : 1) nl_means_window_frame<T, P, S, IL, FR>(q, n);
+}
+template<typename T, int P, int S, bool IL, bool FR, std::enable_if_t<kHeldTo8<T, IL>, int> = 0>
+__global__ void __launch_bounds__(256, 8) nl_means_window_kernel(NLVideoParams q) {
+    for (int n = FR ? blockIdx.z : 0; n < frames<FR>(q); n += FR ? gridDim.z : 1) nl_means_window_frame<T, P, S, IL, FR>(q, n);
 }
 template<int P, int S>
 constexpr size_t nl_window_smem() {
@@ -230,17 +359,54 @@ const halide_filter_argument_t kU8Args[2] = {
     {"input", halide_argument_kind_input_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
     {"non_local_means", halide_argument_kind_output_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
 };
+// The batch entry points: the same buffers with a fourth dimension, the frame index n (float32, then uint8).  The
+// interleaved entry points use these records and the ones above with hb::Arg::interleaved set.
+const halide_filter_argument_t kBatchArgs[2] = {
+    {"input", halide_argument_kind_input_buffer, 4, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+    {"non_local_means", halide_argument_kind_output_buffer, 4, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+};
+const halide_filter_argument_t kU8BatchArgs[2] = {
+    {"input", halide_argument_kind_input_buffer, 4, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+    {"non_local_means", halide_argument_kind_output_buffer, 4, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+};
 
-// nl_means on frames of element type T (float, or uint8_t for halide_b200_nl_means_u8) described by the argument records
-// in_rec / out_rec.
+// The one launch of a call: the register-window kernel at patch / search 3/7 and 7/7 (unless the variant hook asks for
+// the generic one), else the generic kernel.
+template<typename T, bool IL, bool FR>
+void launch(const NLVideoParams &v, dim3 grid, size_t smem, cudaStream_t s) {
+    using Q = std::conditional_t<IL || FR, NLVideoParams, NLParams>;
+    const Q &q = v;
+    const bool window = g_variant != 1;
+    if (window && q.p == 3 && q.s == 7) {
+        constexpr size_t sm = nl_window_smem<3, 7>();
+        static_assert(sm <= 48 * 1024, "no opt-in needed");
+        HB_LAUNCH("nl_means_window", (static_cast<void (*)(Q)>(nl_means_window_kernel<T, 3, 7, IL, FR>)), grid, 256, sm, s, q);
+    } else if (window && q.p == 7 && q.s == 7) {
+        constexpr size_t sm = nl_window_smem<7, 7>();
+        static_assert(sm <= 48 * 1024, "no opt-in needed");
+        HB_LAUNCH("nl_means_window", (static_cast<void (*)(Q)>(nl_means_window_kernel<T, 7, 7, IL, FR>)), grid, 256, sm, s, q);
+    } else {
+        void (*kernel)(Q) = nl_means_kernel<T, IL, FR>;
+        hb::allow_smem(kernel, smem);
+        HB_LAUNCH("nl_means", kernel, grid, 256, smem, s, q);
+    }
+}
+
+// Every nl_means entry point, on args = {input, output} of element type T (float, or uint8_t for the 8-bit ones): 3-D
+// (x, y, c) buffers for one frame, 4-D (x, y, c, n) for a batch; args[*].interleaved selects the pixel-interleaved layout.
 template<typename T>
-int run_nl_means(halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma, halide_buffer_t *output,
-                 const halide_filter_argument_t &in_rec, const halide_filter_argument_t &out_rec) {
+int run_nl_means(hb::Arg *args, int32_t patch_size, int32_t search_area, float sigma, const char *what) {
     int r;
-    hb::Arg args[2] = {{input, in_rec}, {output, out_rec}};
     if ((r = hb::check_args(args, 2))) return r;
-    // every input access is clamped: a query is answered with the output's x/y region and 3 channels
-    const hb::Region region = {{output->dim[0].min, output->dim[1].min, 0}, {output->dim[0].extent, output->dim[1].extent, 3}, false};
+    halide_buffer_t *input = args[0].b, *output = args[1].b;
+    const bool batch = output->dimensions == 4, il = args[0].interleaved;
+    // every input access is clamped in x, y and c: a query is answered with the output's x/y region, 3 channels and (a
+    // batch) the output's frames
+    hb::Region region = {{output->dim[0].min, output->dim[1].min, 0}, {output->dim[0].extent, output->dim[1].extent, 3}, false};
+    if (batch) {
+        region.min[3] = output->dim[3].min;
+        region.extent[3] = output->dim[3].extent;
+    }
     const hb::Region need[2] = {region, region};
     if (hb::answer_bounds_query(args, need, 2)) return 0;
     if ((r = hb::check_shapes(args, 2))) return r;
@@ -250,10 +416,19 @@ int run_nl_means(halide_buffer_t *input, int32_t patch_size, int32_t search_area
                         "Constraint violated: non_local_means.min.2 (%d) == 0 and non_local_means.extent.2 (%d) == 3",
                         output->dim[2].min, output->dim[2].extent);
     }
-    const int W = output->dim[0].extent, H = output->dim[1].extent;
-    if (W <= 0 || H <= 0) return 0;
+    const int W = output->dim[0].extent, H = output->dim[1].extent, N = batch ? output->dim[3].extent : 1;
+    if (W <= 0 || H <= 0 || N <= 0) return 0;
     if (input->dim[0].extent <= 0 || input->dim[1].extent <= 0 || input->dim[2].extent <= 0) {
         return hb::fail(halide_error_code_access_out_of_bounds, "Input buffer input is empty");
+    }
+    // output frame n reads input frame n, which is not clamped: the input's frames must cover the output's
+    if (batch) {
+        const int n0 = output->dim[3].min, n1 = n0 + N - 1, have0 = input->dim[3].min, have1 = have0 + input->dim[3].extent - 1;
+        if (n0 < have0 || n1 > have1) {
+            return hb::fail(halide_error_code_access_out_of_bounds,
+                            "Input buffer input is accessed at %d, which is %s the %s (%d) in dimension 3", n0 < have0 ? n0 : n1,
+                            n0 < have0 ? "before" : "beyond", n0 < have0 ? "min" : "max", n0 < have0 ? have0 : have1);
+        }
     }
     if (patch_size < 1 || search_area < 1 || patch_size > 31 || search_area > 63) {
         return hb::fail(patch_size < 1 || search_area < 1 ? halide_error_code_param_too_small : halide_error_code_param_too_large,
@@ -262,7 +437,7 @@ int run_nl_means(halide_buffer_t *input, int32_t patch_size, int32_t search_area
     }
     if ((r = hb::acquire(args, 2))) return r;
 
-    NLParams q;
+    NLVideoParams q;
     q.in = (const float *)args[0].dev;
     q.in_sy = input->dim[1].stride; q.in_sc = input->dim[2].stride;
     q.in_x0 = input->dim[0].min; q.in_y0 = input->dim[1].min; q.in_c0 = input->dim[2].min;
@@ -276,6 +451,13 @@ int run_nl_means(halide_buffer_t *input, int32_t patch_size, int32_t search_area
     q.inv_sigma_sq = -1.0f / (((sigma * sigma) * (float)patch_size) * (float)patch_size);
     q.iw = TX + patch_size + search_area - 2; q.ih = TY + patch_size + search_area - 2;
     q.dw = TX + patch_size - 1; q.dh = TY + patch_size - 1;
+    q.in_px = input->dim[0].stride; q.out_px = output->dim[0].stride;
+    q.in_sn = batch ? input->dim[3].stride : 0;
+    q.out_sn = batch ? output->dim[3].stride : 0;
+    q.N = N;
+    if (batch) {  // the input frame output frame 0 reads
+        q.in = (const float *)((const T *)q.in + (int64_t)(output->dim[3].min - input->dim[3].min) * q.in_sn);
+    }
     const size_t fixed = (size_t)3 * q.iw * q.ih * sizeof(float);
     const size_t per_dx = (size_t)(q.dh + TY) * q.dw * sizeof(float);
     const size_t budget = 100 * 1024;
@@ -289,22 +471,13 @@ int run_nl_means(halide_buffer_t *input, int32_t patch_size, int32_t search_area
     cudaStream_t s = hb::stream();
     {
         hb::CallTimer timer(s);
-        dim3 grid((W + TX - 1) / TX, (H + TY - 1) / TY);
-        const bool window = g_variant != 1;
-        if (window && patch_size == 3 && search_area == 7) {
-            constexpr size_t sm = nl_window_smem<3, 7>();
-            static_assert(sm <= 48 * 1024, "no opt-in needed");
-            HB_LAUNCH("nl_means_window", (nl_means_window_kernel<T, 3, 7>), grid, 256, sm, s, q);
-        } else if (window && patch_size == 7 && search_area == 7) {
-            constexpr size_t sm = nl_window_smem<7, 7>();
-            static_assert(sm <= 48 * 1024, "no opt-in needed");
-            HB_LAUNCH("nl_means_window", (nl_means_window_kernel<T, 7, 7>), grid, 256, sm, s, q);
-        } else {
-            hb::allow_smem(nl_means_kernel<T>, smem);
-            HB_LAUNCH("nl_means", nl_means_kernel<T>, grid, 256, smem, s, q);
-        }
+        dim3 grid((W + TX - 1) / TX, (H + TY - 1) / TY, std::min(N, kMaxGridZ));
+        if (il && batch) launch<T, true, true>(q, grid, smem, s);
+        else if (il) launch<T, true, false>(q, grid, smem, s);
+        else if (batch) launch<T, false, true>(q, grid, smem, s);
+        else launch<T, false, false>(q, grid, smem, s);
     }
-    return hb::finish(args, 2, sizeof(T) == 1 ? "nl_means_u8 launch" : "nl_means launch");
+    return hb::finish(args, 2, what);
 }
 }  // namespace
 
@@ -313,7 +486,8 @@ extern "C" void halide_b200_nl_means_variant(int v) {
 }
 
 extern "C" int nl_means(halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma, halide_buffer_t *output) {
-    return run_nl_means<float>(input, patch_size, search_area, sigma, output, kArgs[0], kArgs[4]);
+    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[4]}};
+    return run_nl_means<float>(args, patch_size, search_area, sigma, "nl_means launch");
 }
 HB_EXPORT_FILTER(nl_means, kArgs)
 HB_EXPORT_AUTO_SCHEDULE(nl_means, kArgs)
@@ -324,5 +498,40 @@ HB_EXPORT_AUTO_SCHEDULE(nl_means, kArgs)
 // and the variant hook are nl_means'.
 extern "C" int halide_b200_nl_means_u8(halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma,
                                        halide_buffer_t *output) {
-    return run_nl_means<uint8_t>(input, patch_size, search_area, sigma, output, kU8Args[0], kU8Args[1]);
+    hb::Arg args[2] = {{input, kU8Args[0]}, {output, kU8Args[1]}};
+    return run_nl_means<uint8_t>(args, patch_size, search_area, sigma, "nl_means_u8 launch");
+}
+
+// Batch and interleaved entry points (library extensions): nl_means / nl_means_u8 on every frame of a 4-D (x, y, c, n)
+// buffer in one launch, and on pixel-interleaved buffers (dim[2].stride == 1, dim[0].stride = the pixel pitch, at least
+// the channel extent), bit for bit what the planar one-frame entry points give frame by frame on planar copies.
+extern "C" int halide_b200_nl_means_batch(halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma,
+                                          halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kBatchArgs[0]}, {output, kBatchArgs[1]}};
+    return run_nl_means<float>(args, patch_size, search_area, sigma, "nl_means_batch launch");
+}
+extern "C" int halide_b200_nl_means_interleaved(halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma,
+                                                halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kArgs[0], nullptr, true}, {output, kArgs[4], nullptr, true}};
+    return run_nl_means<float>(args, patch_size, search_area, sigma, "nl_means_interleaved launch");
+}
+extern "C" int halide_b200_nl_means_interleaved_batch(halide_buffer_t *input, int32_t patch_size, int32_t search_area,
+                                                      float sigma, halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kBatchArgs[0], nullptr, true}, {output, kBatchArgs[1], nullptr, true}};
+    return run_nl_means<float>(args, patch_size, search_area, sigma, "nl_means_interleaved_batch launch");
+}
+extern "C" int halide_b200_nl_means_u8_batch(halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma,
+                                             halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kU8BatchArgs[0]}, {output, kU8BatchArgs[1]}};
+    return run_nl_means<uint8_t>(args, patch_size, search_area, sigma, "nl_means_u8_batch launch");
+}
+extern "C" int halide_b200_nl_means_u8_interleaved(halide_buffer_t *input, int32_t patch_size, int32_t search_area,
+                                                   float sigma, halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kU8Args[0], nullptr, true}, {output, kU8Args[1], nullptr, true}};
+    return run_nl_means<uint8_t>(args, patch_size, search_area, sigma, "nl_means_u8_interleaved launch");
+}
+extern "C" int halide_b200_nl_means_u8_interleaved_batch(halide_buffer_t *input, int32_t patch_size, int32_t search_area,
+                                                         float sigma, halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kU8BatchArgs[0], nullptr, true}, {output, kU8BatchArgs[1], nullptr, true}};
+    return run_nl_means<uint8_t>(args, patch_size, search_area, sigma, "nl_means_u8_interleaved_batch launch");
 }

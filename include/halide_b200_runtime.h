@@ -373,6 +373,36 @@ int halide_b200_bilateral_grid_u8(struct halide_buffer_t *input, float r_sigma, 
 int halide_b200_nl_means_u8(struct halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma,
                             struct halide_buffer_t *output);
 
+/* nl_means and halide_b200_nl_means_u8 on video clips and pixel-interleaved frames, with nl_means' arguments:
+ *   halide_b200_nl_means_batch / _u8_batch:                   4-D (x, y, c, n) float32 / uint8 buffers, planar;
+ *   halide_b200_nl_means_interleaved / _u8_interleaved:       3-D (x, y, c), interleaved;
+ *   halide_b200_nl_means_interleaved_batch / _u8_interleaved_batch: 4-D, interleaved.
+ * Batch: output frame n is, bit for bit, what nl_means (nl_means_u8) gives on input frame n, with x, y and c clamped
+ * inside each frame as nl_means clamps them; every frame runs in one launch.  The input's frames must cover the output's
+ * (else halide_error_code_access_out_of_bounds); a bounds query gives the input the output's x/y region, channels [0, 3)
+ * and the output's frames.
+ * Interleaved: the result is, bit for bit, what the planar entry point gives on planar copies of the same buffers.  Every
+ * buffer must have dim[2].stride == 1, dim[0].stride (the pixel pitch) >= dim[2].extent and positive dim[1].stride (and
+ * dim[3].stride), else halide_error_code_constraint_violated, a planar buffer included.  The output keeps nl_means'
+ * channels [0, 3); the samples of an output pixel it does not cover (an RGBA frame's alpha) keep their values, and an
+ * RGBA input's alpha is never read.  A bounds query proposes dense interleaved strides (C, W*C, 1[, W*H*C]).
+ * Everything else is nl_means' (nl_means_u8's): element types (float32 entry points refuse uint8 and the reverse), the
+ * argument checks and their order, the patch_size / search_area ranges and codes, empty outputs (0, before any CUDA
+ * call), size limits, the 8-bit conversions and halide_b200_nl_means_variant.  nl_means and nl_means_u8 themselves keep
+ * refusing 4-D and interleaved buffers. */
+int halide_b200_nl_means_batch(struct halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma,
+                               struct halide_buffer_t *output);
+int halide_b200_nl_means_interleaved(struct halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma,
+                                     struct halide_buffer_t *output);
+int halide_b200_nl_means_interleaved_batch(struct halide_buffer_t *input, int32_t patch_size, int32_t search_area,
+                                           float sigma, struct halide_buffer_t *output);
+int halide_b200_nl_means_u8_batch(struct halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma,
+                                  struct halide_buffer_t *output);
+int halide_b200_nl_means_u8_interleaved(struct halide_buffer_t *input, int32_t patch_size, int32_t search_area,
+                                        float sigma, struct halide_buffer_t *output);
+int halide_b200_nl_means_u8_interleaved_batch(struct halide_buffer_t *input, int32_t patch_size, int32_t search_area,
+                                              float sigma, struct halide_buffer_t *output);
+
 /* conv_layer (3x3 convolution + bias + relu, float32) at any shape: the generator's algorithm without its set_bounds /
  * set_stride constraints,
  *   relu(co, x, y, n) = max(0, bias(co) + sum over ky, kx, ci of filter(co, kx, ky, ci) * input(ci, x + kx, y + ky, n)).

@@ -7,7 +7,8 @@ halide_b200/csrc/local_laplacian.o in a scratch checkout, build this tree's, and
 
 Kernels are matched by demangled name.  A template parameter that a change appends with a default value changes the
 mangled name of every existing instantiation without changing its code, so the new object's names are also tried with
-such trailing defaults removed: the interleaved-layout parameters `bool IL = false` (ll_level1_kernel),
+such trailing defaults removed, one after another: the interleaved-layout parameters `bool IL = false` (ll_level1_kernel;
+nl_means_kernel and nl_means_window_kernel, with the frame-walk parameter `bool FR = false` after it),
 `int PI = 1, int PO = 1` (ll_up2_kernel) and the level set type `typename LS = LevelSet` (ll_coarse_fused_kernel).  A kernel that gained the frame element type as its
 first template parameter is also tried without it when that type is float: `f<float>(` as the plain function `f(` (the
 demangled name of a template instance also carries its return type, `void `), `f<float, 3, 7>(` as `f<3, 7>(`
@@ -51,9 +52,11 @@ def main():
     by_name = {}
     for k, v in new.items():
         by_name.setdefault(k, []).append(v)
-        for tail in DEFAULT_TAILS:
-            if tail in k:
-                by_name.setdefault(k.replace(tail, ">("), []).append(v)
+        stripped = k
+        while any(tail in stripped for tail in DEFAULT_TAILS):  # (several appended defaults: strip them one by one)
+            for tail in DEFAULT_TAILS:
+                stripped = stripped.replace(tail, ">(")
+            by_name.setdefault(stripped, []).append(v)
         for pat, repl in FLOAT_HEADS:
             if pat.search(k):
                 by_name.setdefault(pat.sub(repl, k, count=1), []).append(v)
