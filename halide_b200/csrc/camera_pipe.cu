@@ -31,7 +31,6 @@ constexpr int HW = TW / 2 + 3, HH = TH / 2 + 3;  // half-res sites needed by the
 constexpr int GW = HW + 2, GH = HH + 2;      // g_r / g_b tile (demosaic apron 1)
 constexpr int DW = 2 * GW, DH = 2 * GH;      // denoised tile (full-res)
 constexpr int RW = DW + 4, RH = DH + 4;      // raw tile (hot-pixel apron 2)
-constexpr int kMaxGridZ = 65535;             // grid z extent limit: larger bursts are walked by the blocks
 
 struct CPTables {
     i16 matrix[12];  // [y*4 + x]
@@ -134,10 +133,7 @@ __global__ void __launch_bounds__(256) camera_pipe_kernel(CPParams p) {
     // Frames n = blockIdx.z, + gridDim.z, ...: one launch serves any burst.  (No barrier is needed between frames: the
     // raw tile, the first array a frame writes, was last read before three of the previous frame's barriers.)
     for (int n = blockIdx.z; n < p.N; n += gridDim.z) {
-        // The thread index is read anew for every frame: otherwise the compiler keeps each stage's per-thread index
-        // arithmetic live across the frames, which takes the kernel to 57 registers (4 blocks per SM); read here, 32.
-        int tid;
-        asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
+        const int tid = hl::frame_tid();
         const u16 *in = p.in + (int64_t)n * p.in_sn;
         // raw tile: shifted(x,y) = input(x+16, y+12) (generator :412).  Coordinates the output never depends on may fall
         // outside the buffer at the frame's far edges of the last tiles; they are clamped (values unused).
@@ -368,7 +364,7 @@ int run_camera_pipe(hb::Arg *args, float color_temp, float gamma, float contrast
         HB_LAUNCH("cp_tables", cp_tables_kernel, 4, 256, 0, s, tab, m32p, (int64_t)m3200->dim[0].stride, (int64_t)m3200->dim[1].stride,
                   m70p, (int64_t)m7000->dim[0].stride, (int64_t)m7000->dim[1].stride, color_temp, gamma, contrast, sharpen_strength,
                   blackLevel, whiteLevel, inv_c_diff);
-        dim3 grid((W + TW - 1) / TW, (H + TH - 1) / TH, std::min(N, kMaxGridZ));
+        dim3 grid((W + TW - 1) / TW, (H + TH - 1) / TH, std::min(N, hb::kMaxGridZ));
         if (args[3].interleaved) HB_LAUNCH("camera_pipe_il", camera_pipe_kernel<true>, grid, 256, 0, s, p);
         else HB_LAUNCH("camera_pipe", camera_pipe_kernel<false>, grid, 256, 0, s, p);
     }

@@ -59,6 +59,8 @@ int resident_blocks(F *kernel, int threads, size_t smem) {
 }
 int sm_count();
 bool cooperative_launch();  // whether the device takes cudaLaunchCooperativeKernel
+// The largest grid z extent: kernels that index frames by blockIdx.z walk, or launch in groups, batches beyond it.
+constexpr int kMaxGridZ = 65535;
 
 // ---- device scratch (callee-owned intermediates; pooled, src/runtime/cuda.cpp:760-870 analogue) ---
 void *scratch_alloc(size_t bytes);  // returns nullptr on failure (caller maps to -16)

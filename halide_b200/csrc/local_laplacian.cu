@@ -75,10 +75,9 @@ LLFrame scalars_frame(const LLFrameT<T> &f) {
 }
 
 // Grids index frames by blockIdx.z; batches beyond its limit launch in groups of frames [n0, n0 + count).
-constexpr int kMaxGridZ = 65535;
 template<typename P, typename F>
 void for_frame_groups(const P &p, F launch) {
-    for (int n0 = 0; n0 < p.N; n0 += kMaxGridZ) launch(n0, std::min(kMaxGridZ, p.N - n0));
+    for (int n0 = 0; n0 < p.N; n0 += hb::kMaxGridZ) launch(n0, std::min(hb::kMaxGridZ, p.N - n0));
 }
 
 // The checks local_laplacian and its sharded and batch variants share, on args = {input, output}.  *done: return r now

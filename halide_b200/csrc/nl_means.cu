@@ -22,7 +22,8 @@
 // The batch and interleaved entry points run the same kernels too, with two more template parameters: IL (the frames are
 // pixel-interleaved: the tile fill reads them in memory order and the final store writes a pixel's channels side by side)
 // and FR (the grid's blocks walk the frames of a 4-D buffer, frame n = blockIdx.z, + gridDim.z, ...).  Only the fill of
-// sI and the final store differ; the phases, and so every float operation, are the planar one-frame kernels'.
+// sI and the final store differ, and both kernels share them (fill_tile, store_rows); the phases, and so every float
+// operation, are the planar one-frame kernels'.  Each kernel is one template; its parameter block is NLParamsOf<IL, FR>.
 #include <algorithm>
 #include <type_traits>
 
@@ -32,7 +33,6 @@
 namespace {
 
 constexpr int TX = 32, TY = 16;  // output tile per block; 256 threads, 2 rows per thread
-constexpr int kMaxGridZ = 65535;  // grid z extent limit: larger batches are walked by the blocks
 
 struct NLParams {
     const float *in;  // element at input mins (a uint8_t frame's for the <uint8_t> kernels; a batch's: of the input frame
@@ -56,41 +56,8 @@ struct NLVideoParams : NLParams {
     int in_px, out_px;      // pixel pitches (IL kernels, whose channel strides in_sc / out_sc are 1)
     int N;                  // frames (FR kernels)
 };
-
-// The IL tile fill: sI[c][v][u] (planes of npix = ih * iw floats) from an interleaved frame.  The warp's loads take the
-// tile's samples in memory order, channel innermost (32 consecutive samples of a pixel row per load), and a warp
-// shuffle hands each lane the three channels of one pixel, so that each store writes 32 consecutive floats of one plane:
-// storing the loaded samples directly would put the three channels of a pixel into one bank (npix is a multiple of 32
-// at patch 3 / search 7).  Channels clamp to the input's as in the planar fill.
-template<typename T>
-__device__ __forceinline__ void fill_tile_interleaved(float *sI, const NLVideoParams &q, const T *in, int tid, int ax0, int ay0,
-                                                      int iw, int npix) {
-    const int lane = tid & 31;
-    for (int p0 = (tid >> 5) * 32; p0 < npix; p0 += 256) {  // (warp-uniform: every lane takes the shuffles)
-        float smp[3];  // samples 3 * p0 + 32 * k + lane of the tile, pixel (that / 3), channel (that % 3)
-#pragma unroll
-        for (int k = 0; k < 3; k++) {
-            const int j = 3 * p0 + 32 * k + lane, pix = j / 3, c = j - 3 * pix;
-            smp[k] = 0.f;
-            if (pix < npix) {
-                const int v = pix / iw, u = pix - v * iw;
-                const int x = hl::clampi(ax0 + u, q.in_x0, q.in_x0 + q.in_w - 1) - q.in_x0;
-                const int y = hl::clampi(ay0 + v, q.in_y0, q.in_y0 + q.in_h - 1) - q.in_y0;
-                const int cc = hl::clampi(c, q.in_c0, q.in_c0 + q.in_c - 1) - q.in_c0;
-                smp[k] = hl::frame_to_f32(__ldg(in + (int64_t)y * q.in_sy + (int64_t)x * q.in_px + cc));
-            }
-        }
-#pragma unroll
-        for (int c = 0; c < 3; c++) {
-            // Lane p takes sample 3p + c, held in smp[(3p + c) / 32] of lane (3p + c) % 32.  This lane holds it for the one
-            // p with 3p + c == lane (mod 32), p = 11 (lane - c) mod 32 (3 * 11 == 1 mod 32), and sends that register.
-            const int p = ((lane - c) * 11) & 31, k = (3 * p + c) >> 5;
-            const float send = k == 0 ? smp[0] : (k == 1 ? smp[1] : smp[2]);
-            const float got = __shfl_sync(0xffffffffu, send, (3 * lane + c) & 31);
-            if (p0 + lane < npix) sI[c * npix + p0 + lane] = got;
-        }
-    }
-}
+template<bool IL, bool FR>
+using NLParamsOf = std::conditional_t<IL || FR, NLVideoParams, NLParams>;
 
 // Frame n's input (the element at the input's x/y/c mins) and output (at the output's mins), formed where they are used;
 // the one-frame kernels (FR false) read q.in and q.out there as they always did.
@@ -110,43 +77,90 @@ __device__ __forceinline__ int frames(const Q &q) {
     else return 1;
 }
 
-// The thread index, read anew for every frame of an FR kernel: read once, everything the phases derive from it is
-// invariant across the frame loop and the compiler keeps it live across the frames (the planar window kernels then take
-// 62-64 registers instead of 32, and the uint8 one at 3/7 spills).
-template<bool FR>
-__device__ __forceinline__ int thread_index() {
-    if constexpr (FR) {
-        int tid;
-        asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
-        return tid;
+// The tile fill of both kernels: sI[c][v][u], three planes of npix = ih * iw floats, tile (u, v) at absolute
+// (ax0 + u, ay0 + v), from frame n with every coordinate clamped to the input.  The window kernel passes constant
+// extents, the generic kernel q.iw and q.ih: by reference, so that its planar fill reads them from the parameters at
+// each use instead of holding them in registers across the loop (by value, its frame-walking instance compiles to
+// other code).
+// The IL fill's warp loads take the tile's samples in memory order, channel innermost (32 consecutive samples of a pixel
+// row per load), and a warp shuffle hands each lane the three channels of one pixel, so that each store writes 32
+// consecutive floats of one plane: storing the loaded samples directly would put the three channels of a pixel into one
+// bank (npix is a multiple of 32 at patch 3 / search 7).
+template<typename T, bool IL, bool FR, typename Q>
+__device__ __forceinline__ void fill_tile(float *sI, const Q &q, int n, int tid, int ax0, int ay0, const int &iw,
+                                          const int &ih) {
+    if constexpr (IL) {
+        const T *in = frame_in<T, FR>(q, n);
+        const int npix = ih * iw, lane = tid & 31;
+        for (int p0 = (tid >> 5) * 32; p0 < npix; p0 += 256) {  // (warp-uniform: every lane takes the shuffles)
+            float smp[3];  // samples 3 * p0 + 32 * k + lane of the tile, pixel (that / 3), channel (that % 3)
+#pragma unroll
+            for (int k = 0; k < 3; k++) {
+                const int j = 3 * p0 + 32 * k + lane, pix = j / 3, c = j - 3 * pix;
+                smp[k] = 0.f;
+                if (pix < npix) {
+                    const int v = pix / iw, u = pix - v * iw;
+                    const int x = hl::clampi(ax0 + u, q.in_x0, q.in_x0 + q.in_w - 1) - q.in_x0;
+                    const int y = hl::clampi(ay0 + v, q.in_y0, q.in_y0 + q.in_h - 1) - q.in_y0;
+                    const int cc = hl::clampi(c, q.in_c0, q.in_c0 + q.in_c - 1) - q.in_c0;
+                    smp[k] = hl::frame_to_f32(__ldg(in + (int64_t)y * q.in_sy + (int64_t)x * q.in_px + cc));
+                }
+            }
+#pragma unroll
+            for (int c = 0; c < 3; c++) {
+                // Lane p takes sample 3p + c, held in smp[(3p + c) / 32] of lane (3p + c) % 32.  This lane holds it for
+                // the one p with 3p + c == lane (mod 32), p = 11 (lane - c) mod 32 (3 * 11 == 1 mod 32), and sends that
+                // register.
+                const int p = ((lane - c) * 11) & 31, k = (3 * p + c) >> 5;
+                const float send = k == 0 ? smp[0] : (k == 1 ? smp[1] : smp[2]);
+                const float got = __shfl_sync(0xffffffffu, send, (3 * lane + c) & 31);
+                if (p0 + lane < npix) sI[c * npix + p0 + lane] = got;
+            }
+        }
     } else {
-        return threadIdx.x;
+        for (int t = tid; t < 3 * ih * iw; t += 256) {
+            const int c = t / (ih * iw), rem = t - c * ih * iw;
+            const int v = rem / iw, u = rem - v * iw;
+            const int x = hl::clampi(ax0 + u, q.in_x0, q.in_x0 + q.in_w - 1) - q.in_x0;
+            const int y = hl::clampi(ay0 + v, q.in_y0, q.in_y0 + q.in_h - 1) - q.in_y0;
+            const int cc = hl::clampi(c, q.in_c0, q.in_c0 + q.in_c - 1) - q.in_c0;
+            sI[t] = hl::frame_to_f32(__ldg(frame_in<T, FR>(q, n) + (int64_t)cc * q.in_sc + (int64_t)y * q.in_sy + x));
+        }
     }
 }
 
-// nl_means_kernel on frame n; Q = NLParams for the planar one-frame kernels (IL and FR false), else NLVideoParams.
+// The final store of both kernels: a thread's two output pixels of frame n (column tx, rows ty and ty + 8 of the block's
+// tile), each the four running sums acc[r] normalised and clamped.
+template<typename T, bool IL, bool FR, typename Q>
+__device__ __forceinline__ void store_rows(const Q &q, int n, const float (&acc)[2][4], int tx, int ty) {
+#pragma unroll
+    for (int r = 0; r < 2; r++) {
+        const int lx = blockIdx.x * TX + tx, ly = blockIdx.y * TY + ty + 8 * r;
+        if (lx < q.W && ly < q.H) {
+#pragma unroll
+            for (int c = 0; c < 3; c++) {
+                // (NaN -> 1: every weight is NaN when sigma^2 * patch^2 underflows and -1 / it is -inf)
+                const float v = hl::clamp01(__fdiv_rn(acc[r][c], acc[r][3]));
+                T *out = frame_out<T, FR>(q, n);
+                if constexpr (IL) out[(int64_t)ly * q.out_sy + (int64_t)lx * q.out_px + c] = hl::frame_from_f32<T>(v);
+                else out[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = hl::frame_from_f32<T>(v);
+            }
+        }
+    }
+}
+
+// nl_means_kernel on frame n.
 template<typename T, bool IL, bool FR, typename Q>
 __device__ __forceinline__ void nl_means_frame(const Q &q, int n) {
     extern __shared__ float smem[];
     float *sI = smem;                              // [3][ih][iw]
     float *sD = sI + 3 * q.ih * q.iw;              // [nd][dh][dw]
     float *sV = sD + q.nd * q.dh * q.dw;           // [nd][TY][dw]
-    const int tid = thread_index<FR>();
+    const int tid = FR ? hl::frame_tid() : (int)threadIdx.x;
     const int X0 = q.out_x0 + blockIdx.x * TX, Y0 = q.out_y0 + blockIdx.y * TY;
     // tile coordinate (u,v) <-> absolute (X0 + p_lo + s_lo + u, Y0 + p_lo + s_lo + v)
     const int ax0 = X0 + q.p_lo + q.s_lo, ay0 = Y0 + q.p_lo + q.s_lo;
-    if constexpr (IL) {
-        fill_tile_interleaved(sI, q, frame_in<T, FR>(q, n), tid, ax0, ay0, q.iw, q.ih * q.iw);
-    } else {
-        for (int t = tid; t < 3 * q.ih * q.iw; t += 256) {
-            int c = t / (q.ih * q.iw), rem = t - c * q.ih * q.iw;
-            int v = rem / q.iw, u = rem - v * q.iw;
-            int x = hl::clampi(ax0 + u, q.in_x0, q.in_x0 + q.in_w - 1) - q.in_x0;
-            int y = hl::clampi(ay0 + v, q.in_y0, q.in_y0 + q.in_h - 1) - q.in_y0;
-            int cc = hl::clampi(c, q.in_c0, q.in_c0 + q.in_c - 1) - q.in_c0;
-            sI[t] = hl::frame_to_f32(__ldg(frame_in<T, FR>(q, n) + (int64_t)cc * q.in_sc + (int64_t)y * q.in_sy + x));
-        }
-    }
+    fill_tile<T, IL, FR>(sI, q, n, tid, ax0, ay0, q.iw, q.ih);
     __syncthreads();
     const int plane = q.ih * q.iw;
     const int tx = tid & 31, ty = tid >> 5;  // rows ty and ty + 8
@@ -198,31 +212,19 @@ __device__ __forceinline__ void nl_means_frame(const Q &q, int n) {
             // enough between C and the next B, and the A->B barrier above provides it.
         }
     }
-#pragma unroll
-    for (int r = 0; r < 2; r++) {
-        int lx = blockIdx.x * TX + tx, ly = blockIdx.y * TY + ty + 8 * r;
-        if (lx < q.W && ly < q.H) {
-#pragma unroll
-            for (int c = 0; c < 3; c++) {
-                // (NaN -> 1: every weight is NaN when sigma^2 * patch^2 underflows and -1 / it is -inf)
-                float v = hl::clamp01(__fdiv_rn(acc[r][c], acc[r][3]));
-                T *out = frame_out<T, FR>(q, n);
-                if constexpr (IL) out[(int64_t)ly * q.out_sy + (int64_t)lx * q.out_px + c] = hl::frame_from_f32<T>(v);
-                else out[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = hl::frame_from_f32<T>(v);
-            }
-        }
-    }
+    store_rows<T, IL, FR>(q, n, acc, tx, ty);
 }
-template<typename T, bool IL = false, bool FR = false>
-__global__ void __launch_bounds__(256) nl_means_kernel(NLParams q) {
-    static_assert(!IL && !FR, "the IL and FR kernels take NLVideoParams");
-    nl_means_frame<T, false, false>(q, 0);
-}
+// (The planar one-frame instances call the frame body directly: through the one-iteration frame loop they compile to
+// longer code.)
 template<typename T, bool IL, bool FR>
-__global__ void __launch_bounds__(256) nl_means_kernel(NLVideoParams q) {
-    for (int n = FR ? blockIdx.z : 0; n < frames<FR>(q); n += FR ? gridDim.z : 1) {
-        if (n != (int)blockIdx.z) __syncthreads();  // the previous frame's last phase C may still read sI
-        nl_means_frame<T, IL, FR>(q, n);
+__global__ void __launch_bounds__(256) nl_means_kernel(NLParamsOf<IL, FR> q) {
+    if constexpr (!IL && !FR) {
+        nl_means_frame<T, false, false>(q, 0);
+    } else {
+        for (int n = FR ? blockIdx.z : 0; n < frames<FR>(q); n += FR ? gridDim.z : 1) {
+            if (n != (int)blockIdx.z) __syncthreads();  // the previous frame's last phase C may still read sI
+            nl_means_frame<T, IL, FR>(q, n);
+        }
     }
 }
 
@@ -245,21 +247,10 @@ __device__ __forceinline__ void nl_means_window_frame(const Q &q, int n) {
     extern __shared__ float smem[];
     float *sI = smem;             // [3][IH][IW]
     float *sV = sI + 3 * PLANE;   // [S][TY][DW]
-    const int tid = thread_index<FR>();
+    const int tid = FR ? hl::frame_tid() : (int)threadIdx.x;
     const int X0 = q.out_x0 + blockIdx.x * TX, Y0 = q.out_y0 + blockIdx.y * TY;
     const int ax0 = X0 + PLO + SLO, ay0 = Y0 + PLO + SLO;  // tile (u, v) <-> absolute (ax0 + u, ay0 + v)
-    if constexpr (IL) {
-        fill_tile_interleaved(sI, q, frame_in<T, FR>(q, n), tid, ax0, ay0, IW, PLANE);
-    } else {
-        for (int t = tid; t < 3 * PLANE; t += 256) {
-            const int c = t / PLANE, rem = t - c * PLANE;
-            const int v = rem / IW, u = rem - v * IW;
-            const int x = hl::clampi(ax0 + u, q.in_x0, q.in_x0 + q.in_w - 1) - q.in_x0;
-            const int y = hl::clampi(ay0 + v, q.in_y0, q.in_y0 + q.in_h - 1) - q.in_y0;
-            const int cc = hl::clampi(c, q.in_c0, q.in_c0 + q.in_c - 1) - q.in_c0;
-            sI[t] = hl::frame_to_f32(__ldg(frame_in<T, FR>(q, n) + (int64_t)cc * q.in_sc + (int64_t)y * q.in_sy + x));
-        }
-    }
+    fill_tile<T, IL, FR>(sI, q, n, tid, ax0, ay0, IW, IH);
     __syncthreads();
     const int tx = tid & 31, ty = tid >> 5;  // rows ty and ty + 8
     float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
@@ -305,37 +296,21 @@ __device__ __forceinline__ void nl_means_window_frame(const Q &q, int n) {
         }
         __syncthreads();  // (the next search row's phase 1 overwrites sV)
     }
-#pragma unroll
-    for (int r = 0; r < 2; r++) {
-        const int lx = blockIdx.x * TX + tx, ly = blockIdx.y * TY + ty + 8 * r;
-        if (lx < q.W && ly < q.H) {
-#pragma unroll
-            for (int c = 0; c < 3; c++) {
-                const float v = hl::clamp01(__fdiv_rn(acc[r][c], acc[r][3]));
-                T *out = frame_out<T, FR>(q, n);
-                if constexpr (IL) out[(int64_t)ly * q.out_sy + (int64_t)lx * q.out_px + c] = hl::frame_from_f32<T>(v);
-                else out[(int64_t)c * q.out_sc + (int64_t)ly * q.out_sy + lx] = hl::frame_from_f32<T>(v);
-            }
-        }
-    }
-}
-template<typename T, int P, int S, bool IL = false, bool FR = false>
-__global__ void __launch_bounds__(256) nl_means_window_kernel(NLParams q) {
-    static_assert(!IL && !FR, "the IL and FR kernels take NLVideoParams");
-    nl_means_window_frame<T, P, S, false, false>(q, 0);
+    store_rows<T, IL, FR>(q, n, acc, tx, ty);
 }
 // The uint8 IL kernels are held to 8 blocks per SM, which the planar kernels reach with 32 registers: left to itself the
 // compiler gives them 40, room for 6 blocks, and the interleaved call at 3/7 takes 1.08x the planar one's time at 4K
-// instead of 1.06x.  The same bound on the other kernels, which take 32 registers anyway, slows them by 2-3 %.
-template<typename T, bool IL>
-constexpr bool kHeldTo8 = IL && sizeof(T) == 1;
-template<typename T, int P, int S, bool IL, bool FR, std::enable_if_t<!kHeldTo8<T, IL>, int> = 0>
-__global__ void __launch_bounds__(256) nl_means_window_kernel(NLVideoParams q) {
-    for (int n = FR ? blockIdx.z : 0; n < frames<FR>(q); n += FR ? gridDim.z : 1) nl_means_window_frame<T, P, S, IL, FR>(q, n);
-}
-template<typename T, int P, int S, bool IL, bool FR, std::enable_if_t<kHeldTo8<T, IL>, int> = 0>
-__global__ void __launch_bounds__(256, 8) nl_means_window_kernel(NLVideoParams q) {
-    for (int n = FR ? blockIdx.z : 0; n < frames<FR>(q); n += FR ? gridDim.z : 1) nl_means_window_frame<T, P, S, IL, FR>(q, n);
+// instead of 1.06x.  The same bound on the other kernels, which take 32 registers anyway, slows them by 2-3 %; for them
+// the minimum of 0 blocks leaves the compiler free, as the one-argument form does.
+template<typename T, int P, int S, bool IL, bool FR>
+__global__ void __launch_bounds__(256, IL && sizeof(T) == 1 ? 8 : 0) nl_means_window_kernel(NLParamsOf<IL, FR> q) {
+    if constexpr (!IL && !FR) {
+        nl_means_window_frame<T, P, S, false, false>(q, 0);
+    } else {
+        for (int n = FR ? blockIdx.z : 0; n < frames<FR>(q); n += FR ? gridDim.z : 1) {
+            nl_means_window_frame<T, P, S, IL, FR>(q, n);
+        }
+    }
 }
 template<int P, int S>
 constexpr size_t nl_window_smem() {
@@ -374,19 +349,18 @@ const halide_filter_argument_t kU8BatchArgs[2] = {
 // the generic one), else the generic kernel.
 template<typename T, bool IL, bool FR>
 void launch(const NLVideoParams &v, dim3 grid, size_t smem, cudaStream_t s) {
-    using Q = std::conditional_t<IL || FR, NLVideoParams, NLParams>;
-    const Q &q = v;
+    const NLParamsOf<IL, FR> &q = v;
     const bool window = g_variant != 1;
     if (window && q.p == 3 && q.s == 7) {
         constexpr size_t sm = nl_window_smem<3, 7>();
         static_assert(sm <= 48 * 1024, "no opt-in needed");
-        HB_LAUNCH("nl_means_window", (static_cast<void (*)(Q)>(nl_means_window_kernel<T, 3, 7, IL, FR>)), grid, 256, sm, s, q);
+        HB_LAUNCH("nl_means_window", (nl_means_window_kernel<T, 3, 7, IL, FR>), grid, 256, sm, s, q);
     } else if (window && q.p == 7 && q.s == 7) {
         constexpr size_t sm = nl_window_smem<7, 7>();
         static_assert(sm <= 48 * 1024, "no opt-in needed");
-        HB_LAUNCH("nl_means_window", (static_cast<void (*)(Q)>(nl_means_window_kernel<T, 7, 7, IL, FR>)), grid, 256, sm, s, q);
+        HB_LAUNCH("nl_means_window", (nl_means_window_kernel<T, 7, 7, IL, FR>), grid, 256, sm, s, q);
     } else {
-        void (*kernel)(Q) = nl_means_kernel<T, IL, FR>;
+        auto kernel = nl_means_kernel<T, IL, FR>;
         hb::allow_smem(kernel, smem);
         HB_LAUNCH("nl_means", kernel, grid, 256, smem, s, q);
     }
@@ -471,7 +445,7 @@ int run_nl_means(hb::Arg *args, int32_t patch_size, int32_t search_area, float s
     cudaStream_t s = hb::stream();
     {
         hb::CallTimer timer(s);
-        dim3 grid((W + TX - 1) / TX, (H + TY - 1) / TY, std::min(N, kMaxGridZ));
+        dim3 grid((W + TX - 1) / TX, (H + TY - 1) / TY, std::min(N, hb::kMaxGridZ));
         if (il && batch) launch<T, true, true>(q, grid, smem, s);
         else if (il) launch<T, true, false>(q, grid, smem, s);
         else if (batch) launch<T, false, true>(q, grid, smem, s);

@@ -12,7 +12,7 @@ import pytest
 
 from halide_b200 import image_io
 from halide_b200.image_io import convert
-from util import kernels_run
+from util import kernels_run, nl_means_variant
 
 pytestmark = pytest.mark.gpu
 BG_KERNELS = {"bg_hist_blurz", "bg_blur_xy", "bg_slice"}
@@ -84,19 +84,6 @@ def assert_bg_kernels(ran):
 
 def assert_nl_kernel(ran, window):
     assert set(ran) == {"nl_means_window" if window else "nl_means"}, sorted(ran)
-
-
-class nl_variant:
-    """halide_b200_nl_means_variant(v) for the duration of a block (1 = the generic kernel for every size)."""
-
-    def __init__(self, hb, v):
-        self.l, self.v = hb.load_library(), v
-
-    def __enter__(self):
-        self.l.halide_b200_nl_means_variant(self.v)
-
-    def __exit__(self, *exc):
-        self.l.halide_b200_nl_means_variant(0)
 
 
 # ---- bilateral_grid: equality with the float path ------------------------------------------------------------------
@@ -185,7 +172,7 @@ def test_nl_sizes(hb, patch, search, variant, window, h, w, sigma):
     """patch / search 3/7 and 7/7 take the register-window kernels, 5/9 and 1/1 the generic one, and the variant hook
     routes 3/7 and 7/7 to the generic kernel as well."""
     img = u8_frame((3, h, w), h * w + patch * 10 + search)
-    with nl_variant(hb, variant):
+    with nl_means_variant(hb, variant):
         _, _, ran = check(hb, "nl", img, (patch, search, sigma))
     assert_nl_kernel(ran, window)
 
@@ -195,7 +182,7 @@ def test_nl_sizes(hb, patch, search, variant, window, h, w, sigma):
 def test_nl_channels(hb, channels, patch, search, variant, window):
     """A 1- or 4-channel input works as in the float path: channel accesses are clamped to the input's channels."""
     img = u8_frame((channels, 70, 90), channels)
-    with nl_variant(hb, variant):
+    with nl_means_variant(hb, variant):
         _, _, ran = check(hb, "nl", img, (patch, search, 0.12), (3, 70, 90))
     assert_nl_kernel(ran, window)
 
@@ -208,7 +195,7 @@ def test_nl_channels(hb, channels, patch, search, variant, window):
 @pytest.mark.parametrize("variant", [0, 1])
 def test_nl_crops(hb, in_shape, in_mins, out_shape, out_mins, variant):
     img = u8_frame(in_shape, sum(in_shape))
-    with nl_variant(hb, variant):
+    with nl_means_variant(hb, variant):
         _, _, ran = check(hb, "nl", img, (3, 7, 0.12), out_shape, in_mins, out_mins)
     assert_nl_kernel(ran, variant == 0)
 
@@ -235,7 +222,7 @@ def test_nl_4k(hb):
 def test_nl_against_the_oracle(hb, oracle, patch, search, sigma, in_shape, kw, variant):
     img = u8_frame(in_shape, patch + search)
     out_shape = kw.get("out_shape", in_shape)
-    with nl_variant(hb, variant):
+    with nl_means_variant(hb, variant):
         got, _, _ = check(hb, "nl", img, (patch, search, sigma), out_shape, kw.get("in_mins"), kw.get("out_mins"))
     want_f = oracle.nl_means(convert(img, np.float32), patch, search, sigma, **kw)
     assert_range(want_f, "oracle")

@@ -23,7 +23,7 @@ import pytest
 import conv_any_exact as cx
 from halide_b200.image_io import convert
 from test_dist_loopback_gpu import _RANK_THREADS, _settings, _single, FRAMES
-from util import CP_M3200, CP_M7000, cp_params, f32_frame, kernels_run, smooth_u16_frame, u16_frame
+from util import CP_M3200, CP_M7000, cp_params, f32_frame, kernels_run, nl_means_variant, smooth_u16_frame, u16_frame
 
 pytestmark = pytest.mark.gpu
 RTOL = 1e-4  # the float pipelines' tolerance, as in test_bilateral_grid_gpu.py / test_nl_means_gpu.py
@@ -346,15 +346,11 @@ def test_bilateral_grid(hb, oracle, in_lay, out_lay, s_sigma, variant):
 @pytest.mark.parametrize("in_lay,out_lay", pairs(["flip_c", "bcast_c", "flip_y", "xcy"], ["flip_y", "flip_c", "xcy"]))
 def test_nl_means(hb, oracle, in_lay, out_lay, kernel_variant, kernel, variant):
     """bcast_c: one grey plane read as 3 channels."""
-    l = hb.load_library()
     img = f32_frame((3, H, W), 9)
     call = lambda bi, bo: hb.filters.nl_means(bi, 3, 7, 0.12, bo)
-    l.halide_b200_nl_means_variant(kernel_variant)
-    try:
+    with nl_means_variant(hb, kernel_variant):
         (logical,), got, ran, _ = layout_call(hb, call, [img], [in_lay], (3, H, W), np.float32, out_lay, variant)
         dense = dense_call(hb, call, [logical], (3, H, W), np.float32)
-    finally:
-        l.halide_b200_nl_means_variant(0)
     assert list(ran) == [kernel], sorted(ran)
     close(got, oracle.nl_means(logical, 3, 7, 0.12), 1e-3, f"{in_lay} -> {out_lay}")
     same(got, dense, "against the dense call")

@@ -11,8 +11,8 @@ import pytest
 
 import nl_means_exact as E
 from halide_b200 import dist
-from test_param_extremes_gpu import nl_nd, nl_variant
-from util import kernels_run
+from test_param_extremes_gpu import nl_nd
+from util import kernels_run, nl_means_variant
 
 pytestmark = pytest.mark.gpu
 WINDOW = {(3, 7), (7, 7)}  # the (patch, search) pairs the default takes to the register-window kernel
@@ -26,7 +26,7 @@ def run(hb, inp, patch, search, sigma, variant, out_shape=None, in_mins=None, ou
     out = np.zeros((3,) + inp.shape[1:] if out_shape is None else out_shape, np.float32)
     bi = hb.HalideBuffer.from_numpy(inp, in_mins)
     bo = hb.HalideBuffer.from_numpy(out, out_mins, host_dirty=False)
-    with nl_variant(hb, variant), kernels_run(hb) as ran:
+    with nl_means_variant(hb, variant), kernels_run(hb) as ran:
         hb.filters.nl_means(bi, patch, search, sigma, bo)
     assert list(ran) == [kernel(patch, search, variant)], sorted(ran)
     bo.copy_to_host()

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 from nl_means_exact import sensitive_frame
-from util import f32_frame
+from util import f32_frame, nl_means_variant
 
 pytestmark = pytest.mark.gpu
 RTOL = 1e-4
@@ -85,9 +85,7 @@ def test_generic_and_window_kernels(hb, oracle, variant):
     """The generic kernel (variant 1, hook halide_b200_nl_means_variant) and the default, which takes the register-window
     kernel for patch 3 / 7 and search 7, against the oracle: ragged sizes, a crop with offsets, and a patch / search pair
     the window kernel does not cover (the default must fall back to the generic kernel by itself)."""
-    l = hb.load_library()
-    try:
-        l.halide_b200_nl_means_variant(variant)
+    with nl_means_variant(hb, variant):
         for h, w in ((1, 1), (16, 32), (33, 47), (70, 101)):
             inp = sensitive_frame(3, h, w, 0.12, 11 * variant + h + w)
             close(run(hb, inp, 3, 7, 0.12), oracle.nl_means(inp, 3, 7, 0.12))
@@ -98,5 +96,3 @@ def test_generic_and_window_kernels(hb, oracle, variant):
         kw = dict(out_shape=(3, 30, 41), in_mins=(-4, 2, 0), out_mins=(1, 6, 0))
         inp = sensitive_frame(3, 50, 70, 0.12, 5)
         close(run(hb, inp, 3, 7, 0.12, **kw), oracle.nl_means(inp, 3, 7, 0.12, **kw))
-    finally:
-        l.halide_b200_nl_means_variant(0)

@@ -11,7 +11,7 @@ import threading
 import numpy as np
 import pytest
 
-from util import kernels_run
+from util import kernels_run, nl_means_variant
 
 pytestmark = pytest.mark.gpu
 SIGMA = 0.12
@@ -74,19 +74,6 @@ def planar_frame(hb, inp, out_hw, args, in_mins=None, out_mins=None):
     return out
 
 
-class variant:
-    """halide_b200_nl_means_variant(v) for the duration of a block."""
-
-    def __init__(self, hb, v):
-        self.l, self.v = hb.load_library(), v
-
-    def __enter__(self):
-        self.l.halide_b200_nl_means_variant(self.v)
-
-    def __exit__(self, *exc):
-        self.l.halide_b200_nl_means_variant(0)
-
-
 def check_interleaved(hb, inp, args, out_pitch=3, out_hw=None, in_mins=None, out_mins=None, kernel=None):
     """The interleaved entry point on inp ([(n,) y, x, pitch] view) into channels [0, 3) of a guard-filled output of
     out_pitch samples per pixel, against the planar one-frame entry point frame by frame on planar copies.  Returns the
@@ -136,7 +123,7 @@ def test_interleaved_pitches_and_routes(hb, dtype, patch, search, hook, window, 
     """RGB, an RGBA input, an RGBA output whose alpha keeps its guard, a pitch above 4 on both sides, a 1-channel input
     of pitch 1; every kernel route."""
     img = frame((53, 71, in_pitch), dtype, in_pitch * 100 + patch * 10 + search)[..., :in_c]
-    with variant(hb, hook):
+    with nl_means_variant(hb, hook):
         check_interleaved(hb, img, (patch, search, SIGMA), out_pitch, kernel="nl_means_window" if window else "nl_means")
 
 
@@ -157,7 +144,7 @@ def test_rgba_input_alpha_is_never_read(hb, dtype):
 @pytest.mark.parametrize("hook", [0, 1])
 def test_interleaved_mins_crops_odd_widths_unaligned_bases(hb, dtype, hook):
     big = frame((120, 181, 4), dtype, 21 + hook)
-    with variant(hb, hook):
+    with nl_means_variant(hb, hook):
         # padded rows and an odd width, nonzero mins on both sides, input larger than the output
         check_interleaved(hb, big[7:107, 3:176, :3], (3, 7, SIGMA), in_mins=(-5, 3, 0), out_mins=(-2, 5, 0),
                           out_hw=(91, 167))
@@ -174,7 +161,7 @@ def test_interleaved_mins_crops_odd_widths_unaligned_bases(hb, dtype, hook):
 @pytest.mark.parametrize("patch,search,hook,window", ROUTES, ids=ROUTE_IDS)
 def test_interleaved_batches(hb, dtype, patch, search, hook, window):
     clip = frame((3, 37, 66, 4), dtype, patch + search + hook)
-    with variant(hb, hook):
+    with nl_means_variant(hb, hook):
         check_interleaved(hb, clip[..., :3], (patch, search, SIGMA), out_pitch=4,
                           kernel="nl_means_window" if window else "nl_means")
         # frame mins: output frames 0..1 read input frames 0..1 of an input whose frames start at -1 (indices 1..2)
@@ -193,7 +180,7 @@ def test_interleaved_batches(hb, dtype, patch, search, hook, window):
 @pytest.mark.parametrize("n", [1, 8])
 def test_batches(hb, dtype, patch, search, hook, window, n):
     clip = frame((n, 3, 45, 70), dtype, n * 10 + patch + search + hook)
-    with variant(hb, hook):
+    with nl_means_variant(hb, hook):
         check_batch(hb, clip, (patch, search, SIGMA), kernel="nl_means_window" if window else "nl_means")
 
 

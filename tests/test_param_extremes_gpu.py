@@ -5,13 +5,11 @@ nl_means' generic kernel batching a search row's dx offsets over several passes,
 inputs whose channels are not [0, 3); local_laplacian at 3..32 levels, negative alpha, and a sweep of alphas long
 enough to make the remap-table cache evict.  Where a host-side formula picks the branch, the test restates it and
 asserts which side the case falls on, so a retuned budget fails here instead of silently losing the coverage."""
-from contextlib import contextmanager
-
 import numpy as np
 import pytest
 
 from nl_means_exact import sensitive_frame
-from util import f32_frame, kernels_run, run_local_laplacian, smooth_u16_frame, u16_frame
+from util import f32_frame, kernels_run, nl_means_variant, run_local_laplacian, smooth_u16_frame, u16_frame
 
 pytestmark = pytest.mark.gpu
 RTOL = 1e-4  # the float pipelines' tolerance, as in test_bilateral_grid_gpu.py / test_nl_means_gpu.py
@@ -115,16 +113,6 @@ def nl_nd(patch, search):
     return nd, fixed + nd * per_dx
 
 
-@contextmanager
-def nl_variant(hb, v):
-    l = hb.load_library()
-    l.halide_b200_nl_means_variant(v)
-    try:
-        yield
-    finally:
-        l.halide_b200_nl_means_variant(0)
-
-
 def run_nl(hb, inp, patch, search, sigma, out_shape=None, in_mins=None, out_mins=None):
     out = np.zeros((3,) + inp.shape[1:] if out_shape is None else out_shape, np.float32)
     bi = hb.HalideBuffer.from_numpy(inp, in_mins)
@@ -136,7 +124,7 @@ def run_nl(hb, inp, patch, search, sigma, out_shape=None, in_mins=None, out_mins
 
 def nl_check(hb, oracle, inp, patch, search, sigma, kernel, variant=0, **kw):
     kw.setdefault("out_shape", (3,) + inp.shape[1:])
-    with nl_variant(hb, variant), kernels_run(hb) as ran:
+    with nl_means_variant(hb, variant), kernels_run(hb) as ran:
         got = run_nl(hb, inp, patch, search, sigma, **kw)
     assert list(ran) == [kernel], sorted(ran)
     want = oracle.nl_means(inp, patch, search, sigma, **kw)
@@ -189,10 +177,10 @@ def test_nl_means_window_kernel_bit_identical_to_generic(hb, patch, h, w):
     bit on ragged frames, not only each within tolerance of the oracle.  Content on which every offset carries weight
     (on uniform noise at sigma 0.12 only the centre does, and a shared mistake in an off-centre offset would not show)."""
     inp = sensitive_frame(3, h, w, 0.12, 1000 * patch + h + w)
-    with nl_variant(hb, 0), kernels_run(hb) as ran:
+    with nl_means_variant(hb, 0), kernels_run(hb) as ran:
         a = run_nl(hb, inp, patch, 7, 0.12)
     assert list(ran) == ["nl_means_window"], sorted(ran)
-    with nl_variant(hb, 1), kernels_run(hb) as ran:
+    with nl_means_variant(hb, 1), kernels_run(hb) as ran:
         b = run_nl(hb, inp, patch, 7, 0.12)
     assert list(ran) == ["nl_means"], sorted(ran)
     assert np.array_equal(a, b), f"{np.count_nonzero(a != b)} samples differ"

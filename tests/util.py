@@ -67,6 +67,18 @@ def kernels_run(hb):
         hb.lib.profile_reset()
 
 
+@contextmanager
+def nl_means_variant(hb, v):
+    """halide_b200_nl_means_variant(v) for the duration of the block (1 = nl_means's generic kernel for every patch /
+    search size), then the default (0) again."""
+    l = hb.load_library()
+    l.halide_b200_nl_means_variant(v)
+    try:
+        yield
+    finally:
+        l.halide_b200_nl_means_variant(0)
+
+
 # ---- camera_pipe ---------------------------------------------------------------------------------------------------
 # The harness's colour matrices (apps/camera_pipe/process.cpp:43-49), its scalar arguments, and each scalar at the
 # extremes the filter accepts, one at a time.  Left out everywhere: gamma = 0 and non-finite scalars.  1 / 0 = inf makes
