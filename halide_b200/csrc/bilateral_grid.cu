@@ -29,6 +29,7 @@
 // bg_slice take the frame's element type as a template parameter and convert at the load and the store
 // (hl::frame_to_f32 / hl::frame_from_f32), everything between them is the float path's.
 #include <algorithm>
+#include <type_traits>
 
 #include "hb_common.h"
 #include "hl_math.cuh"
@@ -51,14 +52,50 @@ struct BGParams {
     int gw, gh;    // stored cells
     float *grid_a, *grid_b;  // [gh][gw][nz][2]
 };
+// The parameters of the FR instances, which filter the frames of a clip, frame blockIdx.z of the launch each: BGParams
+// with in, out, grid_a and grid_b at the launch's first frame, and the strides from one frame to the next.  (A separate
+// type, so that the one-frame kernels keep their parameter block byte for byte: any field appended to it changes their
+// code.)
+struct BGBatchParams : BGParams {
+    int64_t in_sn, out_sn;  // frame strides of the input and the output, in elements (negative or, the input, zero too)
+    int64_t grid_sn;        // frame stride of grid_a and grid_b, in floats: one frame's grid
+};
+template<bool FR>
+using BGParamsOf = std::conditional_t<FR, BGBatchParams, BGParams>;
+
+// The input (T: its element type), output and grids a kernel body works on: in an FR instance frame blockIdx.z's, the
+// parameter block's pointers moved by that many frames; in a one-frame instance the parameter block's own.  The body reads
+// them where it used to read p.in, p.out, p.grid_a and p.grid_b, and the parameter block itself is never written: an FR
+// body that rewrote its pointers in place had every other parameter reloaded from the constant bank at each use (44
+// constant loads in bg_hist_blurz<uint8_t>, against 8).
+template<typename T, bool FR>
+__device__ __forceinline__ const T *frame_in(const BGParamsOf<FR> &p) {
+    if constexpr (FR) return reinterpret_cast<const T *>(p.in) + (int64_t)blockIdx.z * p.in_sn;
+    else return reinterpret_cast<const T *>(p.in);
+}
+template<typename T, bool FR>
+__device__ __forceinline__ T *frame_out(const BGParamsOf<FR> &p) {
+    if constexpr (FR) return reinterpret_cast<T *>(p.out) + (int64_t)blockIdx.z * p.out_sn;
+    else return reinterpret_cast<T *>(p.out);
+}
+template<bool FR>
+__device__ __forceinline__ float *frame_grid_a(const BGParamsOf<FR> &p) {
+    if constexpr (FR) return p.grid_a + (int64_t)blockIdx.z * p.grid_sn;
+    else return p.grid_a;
+}
+template<bool FR>
+__device__ __forceinline__ float *frame_grid_b(const BGParamsOf<FR> &p) {
+    if constexpr (FR) return p.grid_b + (int64_t)blockIdx.z * p.grid_sn;
+    else return p.grid_b;
+}
 
 // ---- K1: histogram + blurz --------------------------------------------------------------------------
 // One warp handles 16 horizontally adjacent cells (128 px): lane l covers columns 4l..4l+3 of the
 // strip for all 8 rows of the cell row.  Bins live in shared memory as [bin][channel][thread].
 // T: the frame's element type.  A float frame is read with float4 loads, an 8-bit one with uchar4 loads (4 bytes), each
 // sample converted to the float the float path sees for it (hl::frame_to_f32).
-template<typename T>
-__global__ void __launch_bounds__(128) bg_hist_blurz_kernel(BGParams p) {
+template<typename T, bool FR = false>
+__global__ void __launch_bounds__(128) bg_hist_blurz_kernel(BGParamsOf<FR> p) {
     extern __shared__ float s_bins[];  // (zmax+1) * 2 * 128
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nb = p.zmax + 1;
@@ -71,7 +108,7 @@ __global__ void __launch_bounds__(128) bg_hist_blurz_kernel(BGParams p) {
 #pragma unroll
     for (int ry = 0; ry < S; ry++) {
         int y = hl::clampi(gy * S + ry - S / 2, p.in_y0, p.in_y0 + p.in_h - 1) - p.in_y0;
-        const T *row = reinterpret_cast<const T *>(p.in) + (int64_t)y * p.in_sy;
+        const T *row = frame_in<T, FR>(p) + (int64_t)y * p.in_sy;
         float v[4];
         if (interior_x && ((reinterpret_cast<uintptr_t>(row + (px0 - p.in_x0)) & (4 * sizeof(T) - 1)) == 0)) {
             if constexpr (sizeof(T) == 1) {
@@ -107,7 +144,7 @@ __global__ void __launch_bounds__(128) bg_hist_blurz_kernel(BGParams p) {
         if (z < 0 || z > p.zmax) return 0.f;
         return s_bins[(z * 2 + ch) * 128 + ta] + s_bins[(z * 2 + ch) * 128 + tb];
     };
-    float *g = p.grid_a + ((size_t)cell_row * p.gw + cell) * p.nz * 2 + ch;
+    float *g = frame_grid_a<FR>(p) + ((size_t)cell_row * p.gw + cell) * p.nz * 2 + ch;
     float hm2 = 0.f, hm1 = 0.f, h0 = h(0), h1 = h(1), h2 = h(2);
     for (int z = 0; z < p.nz; z++) {
         // blurz = h(z-2) + 4 h(z-1) + 6 h(z) + 4 h(z+1) + h(z+2) (generator :33-37)
@@ -119,7 +156,8 @@ __global__ void __launch_bounds__(128) bg_hist_blurz_kernel(BGParams p) {
 // ---- K2: blurx + blury on the grid -------------------------------------------------------------------
 // blury is only needed on the interior (stored region shrunk by 2 cells on every side); the result is
 // written over the same extent with the border cells left untouched (never read by the slice).
-__global__ void __launch_bounds__(256) bg_blur_xy_kernel(BGParams p, int rows_per_block) {
+template<bool FR = false>
+__global__ void __launch_bounds__(256) bg_blur_xy_kernel(BGParamsOf<FR> p, int rows_per_block) {
     const int V = p.nz * 2;
     const int t = blockIdx.x * blockDim.x + threadIdx.x;  // (cell_x - 2) * V + v
     const int cx = t / V + 2;
@@ -135,7 +173,7 @@ __global__ void __launch_bounds__(256) bg_blur_xy_kernel(BGParams p, int rows_pe
         float t[5];
     };
     auto load_taps = [&](int cy) -> Taps {
-        const float *r = p.grid_a + ((size_t)cy * p.gw + cx) * V + v;
+        const float *r = frame_grid_a<FR>(p) + ((size_t)cy * p.gw + cx) * V + v;
         Taps k;
         k.t[0] = __ldg(r - 2 * V); k.t[1] = __ldg(r - V); k.t[2] = __ldg(r); k.t[3] = __ldg(r + V); k.t[4] = __ldg(r + 2 * V);
         return k;
@@ -153,11 +191,11 @@ __global__ void __launch_bounds__(256) bg_blur_xy_kernel(BGParams p, int rows_pe
         const Taps k0 = load_taps(cy + 2);
         const Taps k1 = load_taps(two ? cy + 3 : cy + 2);  // (rows up to y_end + 1 <= gh - 1 exist: the grid keeps a 2-cell border)
         float e = blurx(k0);
-        p.grid_b[((size_t)cy * p.gw + cx) * V + v] = (((a + b * 4.0f) + c * 6.0f) + d * 4.0f) + e;
+        frame_grid_b<FR>(p)[((size_t)cy * p.gw + cx) * V + v] = (((a + b * 4.0f) + c * 6.0f) + d * 4.0f) + e;
         a = b; b = c; c = d; d = e;
         if (two) {
             e = blurx(k1);
-            p.grid_b[((size_t)(cy + 1) * p.gw + cx) * V + v] = (((a + b * 4.0f) + c * 6.0f) + d * 4.0f) + e;
+            frame_grid_b<FR>(p)[((size_t)(cy + 1) * p.gw + cx) * V + v] = (((a + b * 4.0f) + c * 6.0f) + d * 4.0f) + e;
             a = b; b = c; c = d; d = e;
         }
     }
@@ -175,14 +213,16 @@ constexpr int kSliceW = 128, kSliceCells = 17, kSlicePitch = 24;
 
 // T: the frame's element type.  An 8-bit frame's 4 pixels move as one uchar4 in and one uchar4 out; the value sliced on is
 // hl::frame_to_f32 of the sample and the result is stored as hl::frame_from_f32<T>.
-template<typename T>
-__global__ void __launch_bounds__(256) bg_slice_kernel(BGParams p) {
+// The uint8 FR instance is held to 8 blocks per SM, which every other instance reaches with 32 registers: left to itself
+// the compiler gives it 40, room for 6.  (A minimum of 0 blocks leaves the compiler free, as the one-argument form does.)
+template<typename T, bool FR = false>
+__global__ void __launch_bounds__(256, FR && sizeof(T) == 1 ? 8 : 0) bg_slice_kernel(BGParamsOf<FR> p) {
     extern __shared__ float2 s_grid[];  // [nz][2][kSlicePitch]
     const int lane = threadIdx.x, row = threadIdx.y, tid = row * 32 + lane;
     const int X0 = (p.out_x0 & ~(S - 1)) + blockIdx.x * kSliceW, Y0 = (p.out_y0 & ~(S - 1)) + blockIdx.y * S;
     const int cx0 = (X0 >> 3) - p.gx0, cy0 = (Y0 >> 3) - p.gy0;  // first stored cell of the tile
     {
-        const float2 *g = reinterpret_cast<const float2 *>(p.grid_b);
+        const float2 *g = reinterpret_cast<const float2 *>(frame_grid_b<FR>(p));
         for (int it = tid; it < 2 * kSliceCells * p.nz; it += 256) {
             // (cell fastest: consecutive lanes store to consecutive banks; the planes of a cell are contiguous in HBM, so
             // the later planes of a cell hit the line the first one brought into L1)
@@ -195,8 +235,8 @@ __global__ void __launch_bounds__(256) bg_slice_kernel(BGParams p) {
     __syncthreads();
     const int y = Y0 + row, x = X0 + 8 * (lane & 15) + 4 * (lane >> 4);
     if (y < p.out_y0 || y >= p.out_y0 + p.H || x + 3 < p.out_x0 || x >= p.out_x0 + p.W) return;
-    const T *ip = reinterpret_cast<const T *>(p.in) + (int64_t)(y - p.in_y0) * p.in_sy + (x - p.in_x0);
-    T *op = reinterpret_cast<T *>(p.out) + (int64_t)(y - p.out_y0) * p.out_sy + (x - p.out_x0);
+    const T *ip = frame_in<T, FR>(p) + (int64_t)(y - p.in_y0) * p.in_sy + (x - p.in_x0);
+    T *op = frame_out<T, FR>(p) + (int64_t)(y - p.out_y0) * p.out_sy + (x - p.out_x0);
     const float2 *c00 = s_grid + (lane & 15);  // cell (xi, yi) of this thread's four pixels; xi + 1: +1, yi + 1: +kSlicePitch
     const float yf = __fmul_rn((float)(y & (S - 1)), 0.125f);
     auto px = [&](float raw, int xx) -> float {
@@ -281,7 +321,8 @@ __device__ __forceinline__ int floor_div_dev(int a, int b) {  // b > 0; per bloc
 // entry owned by one thread.  blurz then runs over (cell, z) items, so consecutive threads store consecutive float2 of the
 // grid (the block's cells are contiguous there).  (The minimum-blocks hint: without it ptxas held this kernel to 32
 // registers and spilled.)
-__global__ void __launch_bounds__(256, 1) bg_hist_blurz_s_kernel(BGParams p, BGSParams q) {
+template<bool FR = false>
+__global__ void __launch_bounds__(256, 1) bg_hist_blurz_s_kernel(BGParamsOf<FR> p, BGSParams q) {
     extern __shared__ float2 s_hist[];  // [cpb][nb] running sums, then [cpb][cell_stride] staged pixels
     const int tid = threadIdx.x, S = q.S, nb = p.zmax + 1, cpb = q.cpb;
     float2 *s_pix = s_hist + cpb * nb;
@@ -298,7 +339,7 @@ __global__ void __launch_bounds__(256, 1) bg_hist_blurz_s_kernel(BGParams p, BGS
         __syncthreads();  // the previous chunk is consumed (first chunk: the sums are cleared)
         for (int r = 0; r < nr; r++) {
             const int y = hl::clampi(gy * S + r0 + r - S / 2, p.in_y0, p.in_y0 + p.in_h - 1) - p.in_y0;
-            const float *row = p.in + (int64_t)y * p.in_sy;
+            const float *row = frame_in<float, FR>(p) + (int64_t)y * p.in_sy;
             for (int c = tid; c < cols; c += 256) {
                 const float val = hl::clamp01(__ldg(row + (hl::clampi(xb + c, xlo, xhi) - xlo)));
                 int zi = (int)__fadd_rn(__fmul_rn(val, p.inv_r), 0.5f);
@@ -324,7 +365,7 @@ __global__ void __launch_bounds__(256, 1) bg_hist_blurz_s_kernel(BGParams p, BGS
         }
     }
     __syncthreads();
-    float2 *g = reinterpret_cast<float2 *>(p.grid_a) + ((size_t)cell_row * p.gw + c0) * p.nz;
+    float2 *g = reinterpret_cast<float2 *>(frame_grid_a<FR>(p)) + ((size_t)cell_row * p.gw + c0) * p.nz;
     for (int it = tid; it < ncell * p.nz; it += 256) {
         const int cell = it / p.nz, z = it - cell * p.nz;
         const float2 *hc = s_hist + cell * nb;
@@ -341,16 +382,17 @@ __global__ void __launch_bounds__(256, 1) bg_hist_blurz_s_kernel(BGParams p, BGS
     }
 }
 
-// Histogram block shape for cell size S, nb bins and a grid of gw x gh cells: as many cell slots as 256 threads hold
-// (at most 4096 / S columns' worth), k cells per slot so a block reads at least 256 columns, running sums within 64 KB,
-// and fewer slots when the frame would not give two blocks per SM; staged rows fill up to 4096 pixels.
+// Histogram block shape for cell size S, nb bins and `frames` grids of gw x gh cells: as many cell slots as 256 threads
+// hold (at most 4096 / S columns' worth), k cells per slot so a block reads at least 256 columns, running sums within
+// 64 KB, and fewer slots when the frames would not give two blocks per SM; staged rows fill up to 4096 pixels.  (A clip's
+// launch counts all its frames: the block shape never changes a bin's sum, see bg_hist_blurz_s_kernel.)
 constexpr int kHistCols = 4096;
 
-void choose_hist_block(BGSParams &q, int nb, int gw, int gh) {
+void choose_hist_block(BGSParams &q, int nb, int gw, int gh, int frames) {
     const int S = q.S;
     int cslots = std::max(1, std::min(256 / nb, kHistCols / S));
     const int64_t min_blocks = 2 * (int64_t)hb::sm_count();
-    while (cslots > 1 && (int64_t)gh * ((gw + cslots - 1) / cslots) < min_blocks) cslots = (cslots + 1) / 2;
+    while (cslots > 1 && (int64_t)gh * frames * ((gw + cslots - 1) / cslots) < min_blocks) cslots = (cslots + 1) / 2;
     int k = std::max(1, (256 + cslots * S - 1) / (cslots * S));
     while (k > 1 && (cslots * k * S > kHistCols || (size_t)cslots * k * nb * sizeof(float2) > 64 * 1024)) k--;
     q.cslots = cslots;
@@ -371,14 +413,15 @@ size_t hist_s_bytes(const BGSParams &q, int nb) {
 // a per-pixel division.  Bank conflicts: lanes whose corners fall in one cell read one address when their planes agree
 // (a broadcast) and, with an odd plane stride, different banks when the planes differ by less than 16; lanes in
 // different cells can still collide when the data puts them on different planes.
-__global__ void __launch_bounds__(256) bg_slice_s_kernel(BGParams p, BGSParams q) {
+template<bool FR = false>
+__global__ void __launch_bounds__(256) bg_slice_s_kernel(BGParamsOf<FR> p, BGSParams q) {
     extern __shared__ float2 s_cells[];  // [nz][plane], plane >= ncy * ncx
     const int tid = threadIdx.x, S = q.S;
     const int X0 = (p.out_x0 & ~3) + blockIdx.y * (4 * q.tx), Y0 = p.out_y0 + blockIdx.x * q.th;
     const int cxl = floor_div_dev(X0, S), cyl = floor_div_dev(Y0, S);  // first cell of the tile (absolute)
     const int rx0 = X0 - cxl * S, ry0 = Y0 - cyl * S;                   // tile origin within that cell, [0, S)
     {
-        const float2 *g = reinterpret_cast<const float2 *>(p.grid_b);
+        const float2 *g = reinterpret_cast<const float2 *>(frame_grid_b<FR>(p));
         const int ncells = q.ncx * q.ncy;
         // plane fastest: a cell's planes are contiguous in HBM, and an odd plane stride spreads them over the banks
         for (int it = tid; it < ncells * p.nz; it += 256) {
@@ -407,8 +450,8 @@ __global__ void __launch_bounds__(256) bg_slice_s_kernel(BGParams p, BGSParams q
         const int yi = (int)((n * q.mag) >> kMagShift);
         const float yf = __fmul_rn((float)((int)n - yi * S), q.inv_s);
         const float2 *crow = s_cells + yi * q.ncx;  // cell row yi of plane 0
-        const float *ip = p.in + (int64_t)(y - p.in_y0) * p.in_sy + (x - p.in_x0);
-        float *op = p.out + (int64_t)(y - p.out_y0) * p.out_sy + (x - p.out_x0);
+        const float *ip = frame_in<float, FR>(p) + (int64_t)(y - p.in_y0) * p.in_sy + (x - p.in_x0);
+        float *op = frame_out<float, FR>(p) + (int64_t)(y - p.out_y0) * p.out_sy + (x - p.out_x0);
         auto px = [&](float raw, int i) -> float {
             const float val = hl::clamp01(raw);
             const float zv = __fmul_rn(val, p.inv_r);
@@ -491,27 +534,96 @@ const halide_filter_argument_t kU8Args[2] = {
     {"input", halide_argument_kind_input_buffer, 2, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
     {"bilateral_grid", halide_argument_kind_output_buffer, 2, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
 };
+// The batch entry points: the same buffers with a third dimension, the frame index n (float32, then uint8).
+const halide_filter_argument_t kBatchArgs[2] = {
+    {"input", halide_argument_kind_input_buffer, 3, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+    {"bilateral_grid", halide_argument_kind_output_buffer, 3, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+};
+const halide_filter_argument_t kU8BatchArgs[2] = {
+    {"input", halide_argument_kind_input_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+    {"bilateral_grid", halide_argument_kind_output_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+};
+
+// Scratch a clip's call may hold: its frames are filtered in groups whose two grids together fit in kGridBudget bytes
+// (at least one frame a group, however large its grids), and the groups reuse one pair of allocations.  The device pool
+// keeps freed blocks until they are released, so scratch sized to a whole clip would stay allocated after the call.  At
+// r_sigma 0.1 and s_sigma 8, 256 MiB holds the grids of 2 frames of 7680 x 4320 (101 MB each), 10 of 3840 x 2160 and
+// 40 of 1920 x 1080.
+constexpr size_t kGridBudget = size_t(256) << 20;
+// Frames so large that fewer than kMinGroup of them fit the budget run frame by frame through the one-frame kernels
+// instead, on one pair of grids: one such frame's launches already fill the GPU many times over, so a group gains no
+// occupancy, and the FR instances' frame offsets cost more than the group saves.  (4 x 7680 x 4320 uint8 at r_sigma 0.1,
+// H100 80GB HBM3 at 700 W: in groups of 2, 1.013 of the time of four one-frame calls; frame by frame, 1.000.  At r_sigma
+// 0.2, 4 frames a group: 0.987.)
+constexpr size_t kMinGroup = 3;
 
 inline int fdiv(int a, int b) {  // floor division, b > 0
     int q = a / b;
     return (a % b != 0 && a < 0) ? q - 1 : q;
 }
 
-// bilateral_grid with cell size s_sigma (the generator's GeneratorParam): the shipped S runs bg_hist_blurz, bg_blur_xy
-// and bg_slice; every other cell size runs bg_hist_blurz_s, bg_blur_xy and bg_slice_s.  T is the frames' element type and
-// rec their argument records: float (kArgs), or uint8_t (kU8Args), which runs S only.
+// The three launches of one group of `frames` frames (FR) or of one frame: bg_hist_blurz, bg_blur_xy and bg_slice at
+// the shipped S, the any-S kernels otherwise (q: their shapes, float frames only).  A clip's frame is blockIdx.z.
+template<typename T, bool FR>
+void launch(const BGParamsOf<FR> &p, const BGSParams &q, int s_sigma, int frames, cudaStream_t s) {
+    const size_t bins_bytes = (size_t)(p.zmax + 1) * 2 * 128 * sizeof(float);
+    if (s_sigma == S) {
+        auto kernel = bg_hist_blurz_kernel<T, FR>;
+        hb::allow_smem(kernel, bins_bytes);
+        dim3 g1((p.gw + 63) / 64, p.gh, frames);
+        HB_LAUNCH("bg_hist_blurz", kernel, g1, 128, bins_bytes, s, p);
+    } else if constexpr (std::is_same<T, float>::value) {
+        const size_t hist_bytes = hist_s_bytes(q, p.zmax + 1);
+        auto kernel = bg_hist_blurz_s_kernel<FR>;
+        hb::allow_smem(kernel, hist_bytes);
+        dim3 g1(p.gh, (p.gw + q.cpb - 1) / q.cpb, frames);
+        HB_LAUNCH("bg_hist_blurz_s", kernel, g1, 256, hist_bytes, s, p, q);
+    }
+    const int V = p.nz * 2;
+    const int cols = (p.gw - 4) * V;
+    const int64_t min_blocks = (int64_t)hb::sm_count() * 4;
+    int rows = 16;
+    while (rows > 2 && (int64_t)((cols + 255) / 256) * ((p.gh - 4 + rows - 1) / rows) < min_blocks) rows >>= 1;
+    dim3 g2((cols + 255) / 256, (p.gh - 4 + rows - 1) / rows, frames);
+    HB_LAUNCH("bg_blur_xy", bg_blur_xy_kernel<FR>, g2, 256, 0, s, p, rows);
+    const int ox = p.out_x0, oy = p.out_y0, W = p.W, H = p.H;
+    if (s_sigma == S) {
+        const int tx0 = ox & ~(S - 1), ty0 = oy & ~(S - 1);
+        dim3 g3((ox + W - tx0 + kSliceW - 1) / kSliceW, (oy + H - ty0 + S - 1) / S, frames);
+        const size_t slice_smem = (size_t)p.nz * 2 * kSlicePitch * sizeof(float2);
+        auto kernel = bg_slice_kernel<T, FR>;
+        hb::allow_smem(kernel, slice_smem);
+        HB_LAUNCH("bg_slice", kernel, g3, dim3(32, 8), slice_smem, s, p);
+    } else if constexpr (std::is_same<T, float>::value) {
+        const int tw = 4 * q.tx, tx0 = ox & ~3;
+        dim3 g3((H + q.th - 1) / q.th, (ox + W - tx0 + tw - 1) / tw, frames);
+        const size_t slice_smem = slice_s_bytes(q, p.nz);
+        auto kernel = bg_slice_s_kernel<FR>;
+        hb::allow_smem(kernel, slice_smem);
+        HB_LAUNCH("bg_slice_s", kernel, g3, 256, slice_smem, s, p, q);
+    }
+}
+
+// Every bilateral_grid entry point, with cell size s_sigma (the generator's GeneratorParam): the shipped S runs
+// bg_hist_blurz, bg_blur_xy and bg_slice; every other cell size runs bg_hist_blurz_s, bg_blur_xy and bg_slice_s.  T is
+// the frames' element type and in_rec / out_rec their argument records: float (kArgs, kBatchArgs), or uint8_t (kU8Args,
+// kU8BatchArgs), which runs S only.  2-D (x, y) records take one frame; 3-D (x, y, n) ones a clip, output frame n reading
+// input frame n, whose frames run in groups of up to G (see kGridBudget), three launches a group, or, frames too large
+// for kMinGroup of them to fit the budget, one frame at a time through the one-frame kernels.
 template<typename T>
 int run_bilateral_grid(halide_buffer_t *input, int s_sigma, float r_sigma, halide_buffer_t *output,
-                       const halide_filter_argument_t &in_rec, const halide_filter_argument_t &out_rec) {
+                       const halide_filter_argument_t &in_rec, const halide_filter_argument_t &out_rec, const char *what) {
     int r;
     hb::Arg args[2] = {{input, in_rec}, {output, out_rec}};
     if ((r = hb::check_args(args, 2))) return r;
-    // the slice reads input(x,y) unclamped (generator :50): the input must cover the output region
+    const bool batch = output->dimensions == 3;
+    // the slice reads input(x,y) unclamped (generator :50): the input must cover the output region, and a clip's output
+    // frame n reads input frame n, not clamped either: the input's frames must cover the output's (dimension 2)
     const hb::Region need[2] = {hb::region_of(output, true), hb::region_of(output, false)};
     if (hb::answer_bounds_query(args, need, 2)) return 0;
     if ((r = hb::check_shapes(args, 2)) || (r = hb::check_required(args, need, 2))) return r;
-    const int W = output->dim[0].extent, H = output->dim[1].extent;
-    if (W <= 0 || H <= 0) return 0;
+    const int W = output->dim[0].extent, H = output->dim[1].extent, N = batch ? output->dim[2].extent : 1;
+    if (W <= 0 || H <= 0 || N <= 0) return 0;
     if (s_sigma < 1 || s_sigma > 128) {
         return hb::fail(s_sigma < 1 ? halide_error_code_param_too_small : halide_error_code_param_too_large,
                         "Parameter s_sigma is %d but must be in [1, 128]", (int)s_sigma);
@@ -519,7 +631,7 @@ int run_bilateral_grid(halide_buffer_t *input, int s_sigma, float r_sigma, halid
     if (!(r_sigma > 0.0f)) {
         return hb::fail(halide_error_code_param_too_small, "Parameter r_sigma is %g but must be positive", (double)r_sigma);
     }
-    BGParams p;
+    BGBatchParams p;
     p.inv_r = 1.0f / r_sigma;
     p.zmax = (int)(1.0f * p.inv_r + 0.5f);
     p.nz = p.zmax + 2;
@@ -544,59 +656,52 @@ int run_bilateral_grid(halide_buffer_t *input, int s_sigma, float r_sigma, halid
     p.gy0 = fdiv(oy, s_sigma) - 2;
     p.gw = fdiv(ox + W - 1, s_sigma) + 1 + 2 - p.gx0 + 1;
     p.gh = fdiv(oy + H - 1, s_sigma) + 1 + 2 - p.gy0 + 1;
+    const size_t gelems = (size_t)p.gw * p.gh * p.nz * 2;  // one frame's grid
+    // G frames a group: G = min(N, kMaxGridZ, max(1, kGridBudget / (two grids of one frame))), or 1 frame at a time
+    // through the one-frame kernels when fewer than kMinGroup frames fit the budget
+    const size_t fit = std::max<size_t>(1, kGridBudget / (2 * gelems * sizeof(float)));
+    const bool groups = batch && fit >= kMinGroup;
+    const int G = groups ? (int)std::min<size_t>({(size_t)N, (size_t)hb::kMaxGridZ, fit}) : 1;
+    p.in_sn = batch ? input->dim[2].stride : 0;
+    p.out_sn = batch ? output->dim[2].stride : 0;
+    p.grid_sn = (int64_t)gelems;
+    if (batch) {  // the input frame output frame 0 reads
+        p.in = (const float *)((const T *)p.in + (int64_t)(output->dim[2].min - input->dim[2].min) * p.in_sn);
+    }
     hb::Scratch scratch;
-    const size_t gelems = (size_t)p.gw * p.gh * p.nz * 2;
-    p.grid_a = scratch.get<float>(gelems);
-    p.grid_b = scratch.get<float>(gelems);
+    p.grid_a = scratch.get<float>(gelems * G);
+    p.grid_b = scratch.get<float>(gelems * G);
     if (!p.grid_a || !p.grid_b) return hb::fail(halide_error_code_device_malloc_failed, "bilateral_grid: scratch allocation failed");
 
-    cudaStream_t s = hb::stream();
-    {
-        hb::CallTimer timer(s);
-        BGSParams q;  // (the any-S kernels' shapes)
-        if (s_sigma == S) {
-            hb::allow_smem(bg_hist_blurz_kernel<T>, bins_bytes);
-            dim3 g1((p.gw + 63) / 64, p.gh);
-            HB_LAUNCH("bg_hist_blurz", bg_hist_blurz_kernel<T>, g1, 128, bins_bytes, s, p);
-        } else if constexpr (std::is_same<T, float>::value) {
+    BGSParams q;  // (the any-S kernels' shapes)
+    if constexpr (std::is_same<T, float>::value) {
+        if (s_sigma != S) {
             q.S = s_sigma;
             q.inv_s = (float)(1.0 / (double)s_sigma);
             q.mag = (uint32_t)(((1u << kMagShift) + s_sigma - 1) / s_sigma);
             choose_slice_tile(q, p.nz);
-            choose_hist_block(q, p.zmax + 1, p.gw, p.gh);
-            const size_t hist_bytes = hist_s_bytes(q, p.zmax + 1);
-            hb::allow_smem(bg_hist_blurz_s_kernel, hist_bytes);
-            dim3 g1(p.gh, (p.gw + q.cpb - 1) / q.cpb);
-            HB_LAUNCH("bg_hist_blurz_s", bg_hist_blurz_s_kernel, g1, 256, hist_bytes, s, p, q);
-        }
-        const int V = p.nz * 2;
-        const int cols = (p.gw - 4) * V;
-        const int64_t min_blocks = (int64_t)hb::sm_count() * 4;
-        int rows = 16;
-        while (rows > 2 && (int64_t)((cols + 255) / 256) * ((p.gh - 4 + rows - 1) / rows) < min_blocks) rows >>= 1;
-        dim3 g2((cols + 255) / 256, (p.gh - 4 + rows - 1) / rows);
-        HB_LAUNCH("bg_blur_xy", bg_blur_xy_kernel, g2, 256, 0, s, p, rows);
-        if (s_sigma == S) {
-            const int tx0 = ox & ~(S - 1), ty0 = oy & ~(S - 1);
-            dim3 g3((ox + W - tx0 + kSliceW - 1) / kSliceW, (oy + H - ty0 + S - 1) / S);
-            const size_t slice_smem = (size_t)p.nz * 2 * kSlicePitch * sizeof(float2);
-            hb::allow_smem(bg_slice_kernel<T>, slice_smem);
-            HB_LAUNCH("bg_slice", bg_slice_kernel<T>, g3, dim3(32, 8), slice_smem, s, p);
-        } else if constexpr (std::is_same<T, float>::value) {
-            const int tw = 4 * q.tx, tx0 = ox & ~3;
-            dim3 g3((H + q.th - 1) / q.th, (ox + W - tx0 + tw - 1) / tw);
-            const size_t slice_smem = slice_s_bytes(q, p.nz);
-            hb::allow_smem(bg_slice_s_kernel, slice_smem);
-            HB_LAUNCH("bg_slice_s", bg_slice_s_kernel, g3, 256, slice_smem, s, p, q);
+            choose_hist_block(q, p.zmax + 1, p.gw, p.gh, G);
         }
     }
-    return hb::finish(args, 2, sizeof(T) == 1 ? "bilateral_grid_u8 launch" : "bilateral_grid launch");
+    cudaStream_t s = hb::stream();
+    {
+        hb::CallTimer timer(s);
+        const BGBatchParams first = p;
+        for (int n0 = 0; n0 < N; n0 += G) {  // group [n0, n0 + g): the grids' frames 0 .. g - 1
+            const int g = std::min(G, N - n0);
+            p.in = (const float *)((const T *)first.in + (int64_t)n0 * p.in_sn);
+            p.out = (float *)((T *)first.out + (int64_t)n0 * p.out_sn);
+            if (groups) launch<T, true>(p, q, s_sigma, g, s);
+            else launch<T, false>(p, q, s_sigma, 1, s);
+        }
+    }
+    return hb::finish(args, 2, what);
 }
 
 }  // namespace
 
 extern "C" int bilateral_grid(halide_buffer_t *input, float r_sigma, halide_buffer_t *output) {
-    return run_bilateral_grid<float>(input, S, r_sigma, output, kArgs[0], kArgs[2]);
+    return run_bilateral_grid<float>(input, S, r_sigma, output, kArgs[0], kArgs[2], "bilateral_grid launch");
 }
 HB_EXPORT_FILTER(bilateral_grid, kArgs)
 HB_EXPORT_AUTO_SCHEDULE(bilateral_grid, kArgs)
@@ -605,7 +710,7 @@ HB_EXPORT_AUTO_SCHEDULE(bilateral_grid, kArgs)
 // kernels (bit for bit).  Buffer rules, error codes and the bounds query are bilateral_grid's.
 extern "C" int halide_b200_bilateral_grid_s_sigma(halide_buffer_t *input, int32_t s_sigma, float r_sigma,
                                                   halide_buffer_t *output) {
-    return run_bilateral_grid<float>(input, s_sigma, r_sigma, output, kArgs[0], kArgs[2]);
+    return run_bilateral_grid<float>(input, s_sigma, r_sigma, output, kArgs[0], kArgs[2], "bilateral_grid launch");
 }
 
 // 8-bit entry point (library extension): out8 = to_u8(bilateral_grid(to_f32(in8), r_sigma)) bit for bit, with the
@@ -613,5 +718,21 @@ extern "C" int halide_b200_bilateral_grid_s_sigma(halide_buffer_t *input, int32_
 // bg_slice, the two kernels that read or write the frame.  Buffer rules, error codes and the bounds query are
 // bilateral_grid's.
 extern "C" int halide_b200_bilateral_grid_u8(halide_buffer_t *input, float r_sigma, halide_buffer_t *output) {
-    return run_bilateral_grid<uint8_t>(input, S, r_sigma, output, kU8Args[0], kU8Args[1]);
+    return run_bilateral_grid<uint8_t>(input, S, r_sigma, output, kU8Args[0], kU8Args[1], "bilateral_grid_u8 launch");
+}
+
+// Batch entry points (library extensions): bilateral_grid, halide_b200_bilateral_grid_u8 and
+// halide_b200_bilateral_grid_s_sigma on every frame of a 3-D (x, y, n) buffer, three launches per group of frames; output
+// frame n is, bit for bit, the one-frame entry point's result on input frame n.
+extern "C" int halide_b200_bilateral_grid_batch(halide_buffer_t *input, float r_sigma, halide_buffer_t *output) {
+    return run_bilateral_grid<float>(input, S, r_sigma, output, kBatchArgs[0], kBatchArgs[1], "bilateral_grid_batch launch");
+}
+extern "C" int halide_b200_bilateral_grid_u8_batch(halide_buffer_t *input, float r_sigma, halide_buffer_t *output) {
+    return run_bilateral_grid<uint8_t>(input, S, r_sigma, output, kU8BatchArgs[0], kU8BatchArgs[1],
+                                       "bilateral_grid_u8_batch launch");
+}
+extern "C" int halide_b200_bilateral_grid_s_sigma_batch(halide_buffer_t *input, int32_t s_sigma, float r_sigma,
+                                                        halide_buffer_t *output) {
+    return run_bilateral_grid<float>(input, s_sigma, r_sigma, output, kBatchArgs[0], kBatchArgs[1],
+                                     "bilateral_grid_s_sigma_batch launch");
 }

@@ -373,6 +373,24 @@ int halide_b200_bilateral_grid_u8(struct halide_buffer_t *input, float r_sigma, 
 int halide_b200_nl_means_u8(struct halide_buffer_t *input, int32_t patch_size, int32_t search_area, float sigma,
                             struct halide_buffer_t *output);
 
+/* bilateral_grid, halide_b200_bilateral_grid_u8 and halide_b200_bilateral_grid_s_sigma on video clips: 3-D (x, y, n)
+ * float32 (bilateral_grid_batch, _s_sigma_batch) or uint8 (_u8_batch) buffers, e.g. an (N, H, W) tensor.  Output frame n
+ * is, bit for bit, what the one-frame entry point gives on input frame n with the same arguments; frames are independent
+ * (nothing is clamped or shared across n).  The input must cover the output's x/y region and its frames (else
+ * halide_error_code_access_out_of_bounds, naming dimension 2 for the frames); output->dim[2].min selects the input frame
+ * each output frame reads.  A bounds query gives the input the output's (x, y, n) region with dense strides.  Strides: as
+ * halide_b200_nl_means_batch's (dim[0].stride == 1; rows may be padded, frames may be crops of a larger array, and frame
+ * strides may be negative or, on the input, zero).  The frames run in groups whose two scratch grids together stay within
+ * 256 MiB, three launches a group; frames so large that fewer than 3 fit (7680 x 4320 at r_sigma 0.1) run one at a time
+ * through the one-frame kernels, on one pair of grids.  Everything else follows the one-frame entry points:
+ * element types (the float entry points refuse uint8 and the reverse), the argument checks and their order, s_sigma in
+ * [1, 128], r_sigma > 0, the bins limit, size limits and error codes; an empty output (W, H or N of 0) returns 0 before
+ * any CUDA call.  _u8_batch runs s_sigma = 8, as _u8 does. */
+int halide_b200_bilateral_grid_batch(struct halide_buffer_t *input, float r_sigma, struct halide_buffer_t *output);
+int halide_b200_bilateral_grid_u8_batch(struct halide_buffer_t *input, float r_sigma, struct halide_buffer_t *output);
+int halide_b200_bilateral_grid_s_sigma_batch(struct halide_buffer_t *input, int32_t s_sigma, float r_sigma,
+                                             struct halide_buffer_t *output);
+
 /* nl_means and halide_b200_nl_means_u8 on video clips and pixel-interleaved frames, with nl_means' arguments:
  *   halide_b200_nl_means_batch / _u8_batch:                   4-D (x, y, c, n) float32 / uint8 buffers, planar;
  *   halide_b200_nl_means_interleaved / _u8_interleaved:       3-D (x, y, c), interleaved;

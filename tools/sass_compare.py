@@ -12,11 +12,14 @@ nl_means_kernel and nl_means_window_kernel, with the frame-walk parameter `bool 
 `int PI = 1, int PO = 1` (ll_up2_kernel) and the level set type `typename LS = LevelSet` (ll_coarse_fused_kernel).  A kernel that gained the frame element type as its
 first template parameter is also tried without it when that type is float: `f<float>(` as the plain function `f(` (the
 demangled name of a template instance also carries its return type, `void `), `f<float, 3, 7>(` as `f<3, 7>(`
-(bg_hist_blurz_kernel, bg_slice_kernel, nl_means_kernel, nl_means_window_kernel).  An old kernel with no new one of its
-name is also matched by name and template arguments alone, with the parameter list and a last template argument `0`
-dropped on both sides: the template arguments fix the parameter types however they are spelled (nl_means's kernels take
-theirs through an alias, which demangles as `std::conditional<...>::type`), and a std::enable_if choice between
-overloads adds that `0` (nl_means_window_kernel before it was one template).  Instruction addresses and padding are
+(bg_hist_blurz_kernel, bg_slice_kernel, nl_means_kernel, nl_means_window_kernel; the bilateral_grid kernels also gained
+the frame-walk parameter `bool FR = false` after it).  A plain kernel that became a template of one defaulted `bool`
+is tried without it: `f<false>(` as `f(` (bg_blur_xy_kernel, bg_hist_blurz_s_kernel, bg_slice_s_kernel).  An old kernel
+with no new one of its name is also matched by name and template arguments alone, with the parameter list and a last
+template argument `0` dropped on both sides (a plain function: by name alone): the template arguments fix the parameter
+types however they are spelled (nl_means's and bilateral_grid's kernels take theirs through an alias, which demangles as
+`std::conditional<...>::type`), and a std::enable_if choice between overloads adds that `0` (nl_means_window_kernel
+before it was one template).  Instruction addresses and padding are
 dropped before comparing; opcodes, operands and encodings must match.  Prints each old kernel that is missing or differs, then a count; exits 1 if any.
 """
 import re
@@ -26,10 +29,17 @@ import sys
 CUOBJDUMP = "/usr/local/cuda/bin/cuobjdump"
 # trailing template arguments that stand for the defaults of appended parameters
 DEFAULT_TAILS = [", 1, 1>(", ", false>(", ", llk::LevelSet>("]
-# a leading element type parameter: its float instance against the kernel before it had the parameter
-FLOAT_HEADS = [(re.compile(r"^void (.*)<float>\("), r"\1("), (re.compile(r"<float, "), "<")]
-# a name without its parameter list and an enable_if selector argument
+# a leading element type parameter: its float instance against the kernel before it had the parameter; and a plain
+# kernel's one appended `bool = false`
+HEADS = [(re.compile(r"^void (.*)<float>\("), r"\1("), (re.compile(r"<float, "), "<"), (re.compile(r"^void (.*)<false>\("), r"\1(")]
+# a name without its parameter list and an enable_if selector argument; a plain function's name without its parameter
+# list (the first parenthesis that follows a name character: "(anonymous namespace)" precedes none)
 BARE = re.compile(r"(, 0)?>\(.*\)$")
+PLAIN = re.compile(r"(?<=\w)\(.*\)$")
+
+
+def bare(name):
+    return BARE.sub(">", name) if BARE.search(name) else PLAIN.sub("", name)
 
 
 def kernels(obj):
@@ -63,15 +73,15 @@ def main():
             for tail in DEFAULT_TAILS:
                 stripped = stripped.replace(tail, ">(")
             by_name.setdefault(stripped, []).append(v)
-        for pat, repl in FLOAT_HEADS:
+        for pat, repl in HEADS:
             if pat.search(k):
                 by_name.setdefault(pat.sub(repl, k, count=1), []).append(v)
     by_bare = {}
     for k, vs in by_name.items():
-        by_bare.setdefault(BARE.sub(">", k), []).extend(vs)
+        by_bare.setdefault(bare(k), []).extend(vs)
     bad = 0
     for k, v in old.items():
-        cands = by_name.get(k) or by_bare.get(BARE.sub(">", k), [])
+        cands = by_name.get(k) or by_bare.get(bare(k), [])
         if not any(c == v for c in cands):
             print(("DIFFERS " if cands else "MISSING ") + k)
             bad += 1
