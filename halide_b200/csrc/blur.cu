@@ -15,6 +15,9 @@
 //     strips sized to fill the resident warps a whole number of times.
 //   * blur3x3_u16_kernel — any alignment: a lane owns 8 pixels, aligned 16-byte loads realigned by funnel shifts, the
 //     2-pixel horizontal apron from the neighbouring lane by shuffle.  Bound by the integer pipe.
+// halide_b200_blur_batch runs the same two kernels on every frame of a clip, in one launch (FR instances).
+#include <type_traits>
+
 #include "hb_common.h"
 
 namespace {
@@ -34,6 +37,35 @@ struct BlurArgs {
     // valid element range of the input allocation relative to `in`, for guarding vector loads
     int64_t in_lo, in_hi;
 };
+// The parameters of the FR instances, which filter the frames of a clip: BlurArgs at the clip's first frame (in_lo and
+// in_hi span the whole 3-D input allocation, relative to frame 0's `in`), the strides from one frame to the next and the
+// number of frames.  (A separate type, so that the one-frame kernels keep their parameter block byte for byte: any field
+// appended to it changes their code.)
+struct BlurBatchArgs : BlurArgs {
+    int64_t in_sn, out_sn;  // frame strides in elements (negative or, the input, zero too)
+    int n;                  // frames
+};
+template<bool FR>
+using BlurArgsOf = std::conditional_t<FR, BlurBatchArgs, BlurArgs>;
+
+// Frame n's input offset, relative to `in` (every input offset the kernels form stays relative to frame 0's `in`, so the
+// allocation span guards frame n unchanged), its output, and the number of frames.  They read the parameter block and
+// never write it; in a one-frame instance they give its own pointers and 1 frame.
+template<bool FR>
+__device__ __forceinline__ int64_t frame_in_off(const BlurArgsOf<FR> &a, int n) {
+    if constexpr (FR) return (int64_t)n * a.in_sn;
+    else return 0;
+}
+template<bool FR>
+__device__ __forceinline__ int frame_count(const BlurArgsOf<FR> &a) {
+    if constexpr (FR) return a.n;
+    else return 1;
+}
+template<bool FR>
+__device__ __forceinline__ uint16_t *frame_out(const BlurArgsOf<FR> &a, int n) {
+    if constexpr (FR) return a.out + (int64_t)n * a.out_sn;
+    else return a.out;
+}
 
 __device__ __forceinline__ uint4 load_chunk(const uint16_t *p, int64_t off, int64_t lo, int64_t hi) {
     // p+off is 16-byte aligned.  Fast path when the whole chunk is inside the allocation span.
@@ -113,7 +145,11 @@ __device__ __forceinline__ void blur_x_row(const RawRow &raw, int lane, uint32_t
     }
 }
 
-__global__ void __launch_bounds__(32 * kWarpsPerBlock) blur3x3_u16_kernel(BlurArgs a) {
+// FR: a clip, frames blockIdx.z, blockIdx.z + gridDim.z, ... (gridDim.z <= kMaxGridZ); the one-frame instance runs the
+// body once, for its frame.  (Written as one body rather than a frame loop around a device function: either of those
+// changed the one-frame instance's code.)
+template<bool FR = false>
+__global__ void __launch_bounds__(32 * kWarpsPerBlock) blur3x3_u16_kernel(BlurArgsOf<FR> a) {
     int lane = threadIdx.x & 31;
     int warp = threadIdx.x >> 5;
     int x0 = blockIdx.x * kStripW;
@@ -121,31 +157,36 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) blur3x3_u16_kernel(BlurAr
     if (y0 >= a.h) return;
     int y1 = min(y0 + a.rows_per_warp, a.h);
 
-    uint32_t r0[8], r1[8], r2[8];
-    blur_x_row(load_raw_row(a, (int64_t)y0 * a.in_stride_y, x0, lane), lane, r0);
-    blur_x_row(load_raw_row(a, (int64_t)(y0 + 1) * a.in_stride_y, x0, lane), lane, r1);
-    RawRow next = load_raw_row(a, (int64_t)(y0 + 2) * a.in_stride_y, x0, lane);
-    int xl = x0 + lane * kPxPerLane;
-    for (int y = y0; y < y1; y++) {
-        const RawRow cur = next;
-        if (y + 1 < y1) next = load_raw_row(a, (int64_t)(y + 3) * a.in_stride_y, x0, lane);
-        blur_x_row(cur, lane, r2);
-        uint32_t o[8];
+    int n = FR ? blockIdx.z : 0;
+    do {
+        const int64_t fo = frame_in_off<FR>(a, n);
+        uint32_t r0[8], r1[8], r2[8];
+        blur_x_row(load_raw_row(a, fo + (int64_t)y0 * a.in_stride_y, x0, lane), lane, r0);
+        blur_x_row(load_raw_row(a, fo + (int64_t)(y0 + 1) * a.in_stride_y, x0, lane), lane, r1);
+        RawRow next = load_raw_row(a, fo + (int64_t)(y0 + 2) * a.in_stride_y, x0, lane);
+        int xl = x0 + lane * kPxPerLane;
+        for (int y = y0; y < y1; y++) {
+            const RawRow cur = next;
+            if (y + 1 < y1) next = load_raw_row(a, fo + (int64_t)(y + 3) * a.in_stride_y, x0, lane);
+            blur_x_row(cur, lane, r2);
+            uint32_t o[8];
 #pragma unroll
-        for (int i = 0; i < 8; i++) o[i] = ((r0[i] + r1[i] + r2[i]) & 0xffffu) / 3u;
-        uint16_t *dst = a.out + (int64_t)y * a.out_stride_y + xl;
-        if (xl + 8 <= a.w && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-            uint4 pk = make_uint4(o[0] | (o[1] << 16), o[2] | (o[3] << 16), o[4] | (o[5] << 16), o[6] | (o[7] << 16));
-            *reinterpret_cast<uint4 *>(dst) = pk;
-        } else {
+            for (int i = 0; i < 8; i++) o[i] = ((r0[i] + r1[i] + r2[i]) & 0xffffu) / 3u;
+            uint16_t *dst = frame_out<FR>(a, n) + (int64_t)y * a.out_stride_y + xl;
+            if (xl + 8 <= a.w && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+                uint4 pk = make_uint4(o[0] | (o[1] << 16), o[2] | (o[3] << 16), o[4] | (o[5] << 16), o[6] | (o[7] << 16));
+                *reinterpret_cast<uint4 *>(dst) = pk;
+            } else {
 #pragma unroll
-            for (int i = 0; i < 8; i++) {
-                if (xl + i < a.w) dst[i] = (uint16_t)o[i];
+                for (int i = 0; i < 8; i++) {
+                    if (xl + i < a.w) dst[i] = (uint16_t)o[i];
+                }
             }
-        }
 #pragma unroll
-        for (int i = 0; i < 8; i++) { r0[i] = r1[i]; r1[i] = r2[i]; }
-    }
+            for (int i = 0; i < 8; i++) { r0[i] = r1[i]; r1[i] = r2[i]; }
+        }
+        if constexpr (FR) n += gridDim.z;
+    } while (FR && n < frame_count<FR>(a));
 }
 
 // ---- fast path: frames whose rows keep pixel pairs 4-byte aligned (even strides, aligned bases) ----------------------
@@ -243,10 +284,11 @@ struct QuadStrip {
 #pragma unroll
         for (int i = 0; i < 4; i++) { r0[i] = r1[i]; r1[i] = r2[i]; }
     }
-    __device__ __forceinline__ void run(int y0, int y1) {
+    // in, out: the frame's input (at the output origin) and output
+    __device__ __forceinline__ void run(const uint16_t *in, uint16_t *out, int y0, int y1) {
         last_in = y1 + 1;  // last input row read; y0 + 2 <= last_in
-        rin = a.in + ((int64_t)y0 * a.in_stride_y + x);
-        rout = a.out + ((int64_t)y0 * a.out_stride_y + x);
+        rin = in + ((int64_t)y0 * a.in_stride_y + x);
+        rout = out + ((int64_t)y0 * a.out_stride_y + x);
         const QuadRow t0 = fetch<false>(), t1 = fetch<false>();
         next_row = y0 + 2;
 #pragma unroll
@@ -270,12 +312,22 @@ struct QuadStrip {
     }
 };
 
-// a.rows_per_warp = strip height; strips are numbered x-fastest so the warps of a block read adjacent spans of a row
-template<int AHEAD>
-__global__ void __launch_bounds__(32 * kQuadWarps) blur3x3_u16_quad_kernel(BlurArgs a, int strips_x, int strips) {
+// a.rows_per_warp = strip height; strips are numbered x-fastest so the warps of a block read adjacent spans of a row.
+// FR: a clip's strips, frame by frame: strip t is strip t mod `strips` of frame t / `strips`.
+template<int AHEAD, bool FR = false>
+__global__ void __launch_bounds__(32 * kQuadWarps) blur3x3_u16_quad_kernel(BlurArgsOf<FR> a, int strips_x, int strips) {
     const int lane = threadIdx.x & 31;
-    const int t = blockIdx.x * kQuadWarps + (threadIdx.x >> 5);
-    if (t >= strips) return;
+    int t = blockIdx.x * kQuadWarps + (threadIdx.x >> 5);
+    int n = 0;
+    if constexpr (FR) {
+        if (t >= strips * a.n) return;
+        n = t / strips;
+        t -= n * strips;
+    } else {
+        if (t >= strips) return;
+    }
+    const uint16_t *in = a.in + frame_in_off<FR>(a, n);
+    uint16_t *out = frame_out<FR>(a, n);
     const int sx = t % strips_x, sy = t / strips_x;
     const int xw = sx * kQuadW, y0 = sy * a.rows_per_warp;
     const int y1 = min(y0 + a.rows_per_warp, a.h);
@@ -283,11 +335,11 @@ __global__ void __launch_bounds__(32 * kQuadWarps) blur3x3_u16_quad_kernel(BlurA
     if (xw + kQuadW <= a.w) {
         QuadStrip<false, AHEAD> st{a};
         st.x = xw + 4 * lane;
-        st.run(y0, y1);
+        st.run(in, out, y0, y1);
     } else {
         QuadStrip<true, AHEAD> st{a};
         st.x = xw + 4 * lane;
-        st.run(y0, y1);
+        st.run(in, out, y0, y1);
     }
 }
 
@@ -295,78 +347,116 @@ const halide_filter_argument_t kArgs[2] = {
     {"input", halide_argument_kind_input_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
     {"blur_y", halide_argument_kind_output_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
 };
+// The batch entry point: the same buffers with a third dimension, the frame index n.
+const halide_filter_argument_t kBatchArgs[2] = {
+    {"input", halide_argument_kind_input_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+    {"blur_y", halide_argument_kind_output_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+};
 
-}  // namespace
+// The one launch of a frame (FR false) or of a clip (FR): the pair kernel when `pair_ok`, the general one otherwise.
+template<bool FR>
+void launch(BlurArgsOf<FR> &a, bool pair_ok, int frames, cudaStream_t s) {
+    const int w = a.w, h = a.h;
+    if (pair_ok) {
+        // strips of 128 columns; height such that the strips of all frames fill the resident warps a whole number of times
+        const int sxq = (w + kQuadW - 1) / kQuadW;
+        auto kernel = blur3x3_u16_quad_kernel<6, FR>;
+        const int64_t slots = (int64_t)hb::resident_blocks(kernel, 32 * kQuadWarps, 0) * kQuadWarps;
+        int qrows = 8;
+        for (int m = 1; m <= 64; m++) {
+            const int64_t sy = m * slots / ((int64_t)sxq * frames);
+            if (sy < 1) continue;
+            const int rr = (int)((h + sy - 1) / sy);
+            if (rr <= 64 || m == 64) {
+                qrows = rr < 8 ? 8 : rr;
+                break;
+            }
+        }
+        if (g_force_general >= 8) qrows = g_force_general;
+        a.rows_per_warp = qrows;
+        const int strips_q = sxq * ((h + qrows - 1) / qrows);
+        const int nblk = (int)(((int64_t)strips_q * frames + kQuadWarps - 1) / kQuadWarps);
+        HB_LAUNCH("blur3x3_u16_quad", kernel, nblk, 32 * kQuadWarps, 0, s, a, sxq, strips_q);
+    } else {
+        // Enough warps to cover the SMs a few times over, but strips tall enough to amortise the two-row vertical apron.
+        int strips_x = (w + kStripW - 1) / kStripW;
+        int rows = 32;
+        const int64_t min_warps = (int64_t)hb::sm_count() * 8;
+        while (rows > 4 && (int64_t)strips_x * ((h + rows - 1) / rows) * frames < min_warps) rows >>= 1;
+        a.rows_per_warp = rows;
+        int warps_y = (h + rows - 1) / rows;
+        dim3 grid(strips_x, (warps_y + kWarpsPerBlock - 1) / kWarpsPerBlock, frames < hb::kMaxGridZ ? frames : hb::kMaxGridZ);
+        HB_LAUNCH("blur3x3_u16", blur3x3_u16_kernel<FR>, grid, 32 * kWarpsPerBlock, 0, s, a);
+    }
+}
 
-extern "C" int halide_blur(halide_buffer_t *input, halide_buffer_t *blur_y) {
+// Every blur entry point: 2-D (x, y) records take one frame; 3-D (x, y, n) ones a clip, output frame n reading input
+// frame n, all its frames in one launch.
+int run_blur(halide_buffer_t *input, halide_buffer_t *blur_y, const halide_filter_argument_t *rec, const char *what) {
     int r;
-    hb::Arg args[2] = {{input, kArgs[0]}, {blur_y, kArgs[1]}};
+    hb::Arg args[2] = {{input, rec[0]}, {blur_y, rec[1]}};
     if ((r = hb::check_args(args, 2))) return r;
-    // The input must cover the output region grown by the 3-tap footprints: [ox, ox+W+1] x [oy, oy+H+1].
+    const bool batch = blur_y->dimensions == 3;
+    // The input must cover the output region grown by the 3-tap footprints: [ox, ox+W+1] x [oy, oy+H+1]; a clip's output
+    // frame n reads input frame n, not clamped either: the input's frames must cover the output's (dimension 2).
     const int ox = blur_y->dim[0].min, oy = blur_y->dim[1].min;
     const int w = blur_y->dim[0].extent, h = blur_y->dim[1].extent;
-    const hb::Region need[2] = {{{ox, oy}, {w + 2, h + 2}, true}, hb::region_of(blur_y, false)};
+    const int on = batch ? blur_y->dim[2].min : 0, N = batch ? blur_y->dim[2].extent : 1;
+    const hb::Region need[2] = {{{ox, oy, on}, {w + 2, h + 2, N}, true}, hb::region_of(blur_y, false)};
     if (hb::answer_bounds_query(args, need, 2)) return 0;
     if ((r = hb::check_shapes(args, 2)) || (r = hb::check_required(args, need, 2))) return r;
-    if (w <= 0 || h <= 0) return 0;
+    if (w <= 0 || h <= 0 || N <= 0) return 0;
     if ((r = hb::acquire(args, 2))) return r;
 
-    BlurArgs a;
+    BlurBatchArgs a;
     const int64_t isy = input->dim[1].stride;
-    const int64_t origin = (int64_t)(ox - input->dim[0].min) + (int64_t)(oy - input->dim[1].min) * isy;
+    const int64_t isn = batch ? input->dim[2].stride : 0;
+    const int64_t origin = (int64_t)(ox - input->dim[0].min) + (int64_t)(oy - input->dim[1].min) * isy +
+                           (batch ? (int64_t)(on - input->dim[2].min) * isn : 0);
     a.in = (const uint16_t *)args[0].dev + origin;
     a.out = (uint16_t *)args[1].dev;
     a.in_stride_y = isy;
     a.out_stride_y = blur_y->dim[1].stride;
     a.w = w;
     a.h = h;
-    // allocation span of the input relative to a.in (dim0 stride is 1; dim1 stride may be negative)
-    int64_t reach1 = (int64_t)(input->dim[1].extent - 1) * isy;
-    int64_t lo = reach1 < 0 ? reach1 : 0, hi = (reach1 > 0 ? reach1 : 0) + input->dim[0].extent - 1;
+    a.in_sn = isn;
+    a.out_sn = batch ? blur_y->dim[2].stride : 0;
+    a.n = N;
+    // allocation span of the input relative to a.in (dim0 stride is 1; the dim1 and dim2 strides may be negative, and a
+    // clip's frame stride 0)
+    int64_t lo = 0, hi = input->dim[0].extent - 1;
+    for (int d = 1; d < input->dimensions; d++) {
+        const int64_t reach = (int64_t)(input->dim[d].extent - 1) * input->dim[d].stride;
+        (reach < 0 ? lo : hi) += reach;
+    }
     a.in_lo = lo - origin;
     a.in_hi = hi - origin;
 
-    // Enough warps to cover the SMs a few times over, but strips tall enough to amortise the two-row vertical apron.
-    int strips_x = (w + kStripW - 1) / kStripW;
-    int rows = 32;
-    const int64_t min_warps = (int64_t)hb::sm_count() * 8;
-    while (rows > 4 && (int64_t)strips_x * ((h + rows - 1) / rows) < min_warps) rows >>= 1;
-    a.rows_per_warp = rows;
-    int warps_y = (h + rows - 1) / rows;
-    dim3 grid(strips_x, (warps_y + kWarpsPerBlock - 1) / kWarpsPerBlock);
-
-    // pixel pairs 4-byte aligned on every row of both buffers -> the pair kernel; anything else -> the general kernel
+    // pixel pairs 4-byte aligned on every row of every frame of both buffers -> the pair kernel; anything else -> the
+    // general kernel
     const bool pair_ok = ((reinterpret_cast<uintptr_t>(a.in) | reinterpret_cast<uintptr_t>(a.out)) & 3) == 0 &&
-                         (a.in_stride_y & 1) == 0 && (a.out_stride_y & 1) == 0 && g_force_general != 1;
+                         ((a.in_stride_y | a.out_stride_y | a.in_sn | a.out_sn) & 1) == 0 && g_force_general != 1;
     cudaStream_t s = hb::stream();
     {
         hb::CallTimer timer(s);
-        if (pair_ok) {
-            // strips of 128 columns; height such that the strips fill the resident warps a whole number of times
-            const int sxq = (w + kQuadW - 1) / kQuadW;
-            const int64_t slots = (int64_t)hb::resident_blocks(blur3x3_u16_quad_kernel<6>, 32 * kQuadWarps, 0) * kQuadWarps;
-            int qrows = 8;
-            for (int m = 1; m <= 64; m++) {
-                const int64_t sy = m * slots / sxq;
-                if (sy < 1) continue;
-                const int rr = (int)((h + sy - 1) / sy);
-                if (rr <= 64 || m == 64) {
-                    qrows = rr < 8 ? 8 : rr;
-                    break;
-                }
-            }
-            if (g_force_general >= 8) qrows = g_force_general;
-            a.rows_per_warp = qrows;
-            const int strips_q = sxq * ((h + qrows - 1) / qrows);
-            const int nblk = (strips_q + kQuadWarps - 1) / kQuadWarps;
-            HB_LAUNCH("blur3x3_u16_quad", blur3x3_u16_quad_kernel<6>, nblk, 32 * kQuadWarps, 0, s, a, sxq, strips_q);
-        } else {
-            HB_LAUNCH("blur3x3_u16", blur3x3_u16_kernel, grid, 32 * kWarpsPerBlock, 0, s, a);
-        }
+        if (batch) launch<true>(a, pair_ok, N, s);
+        else launch<false>(a, pair_ok, 1, s);
     }
-    return hb::finish(args, 2, "halide_blur launch");
+    return hb::finish(args, 2, what);
+}
+
+}  // namespace
+
+extern "C" int halide_blur(halide_buffer_t *input, halide_buffer_t *blur_y) {
+    return run_blur(input, blur_y, kArgs, "halide_blur launch");
 }
 HB_EXPORT_FILTER(halide_blur, kArgs)
+
+// Batch entry point (library extension): halide_blur on every frame of a 3-D (x, y, n) buffer, in one launch; output
+// frame n is, bit for bit, halide_blur's result on input frame n.
+extern "C" int halide_b200_blur_batch(halide_buffer_t *input, halide_buffer_t *blur_y) {
+    return run_blur(input, blur_y, kBatchArgs, "halide_b200_blur_batch launch");
+}
 
 // Test hook: 1 = always take the general (any alignment) kernel, so both kernels stay covered by the parity tests;
 // >= 8 = the aligned kernel with strips of that many rows.

@@ -16,6 +16,12 @@
 // compulsory HBM traffic).  kFuse stages run per launch on a shared-memory tile with a 2*kFuse
 // apron (a chain whose length is not a multiple of kFuse ends with one shorter launch); the frame
 // itself (7.9 MB at the harness size) stays L2-resident between launches.
+//
+// halide_b200_stencil_chain_batch / _stencils_batch run the same launches on a clip: each launch takes a group of frames,
+// frame blockIdx.z each (FR instances).
+#include <algorithm>
+#include <type_traits>
+
 #include "hb_common.h"
 
 namespace {
@@ -36,6 +42,28 @@ struct Plane {
     int dst_w, dst_h;
     int src_words, dst_words;  // rows of src / dst keep pixel pairs 4-byte aligned (even stride, aligned base): 32-bit accesses
 };
+// The parameters of the FR instances, which run one launch's stages on a group of frames, frame blockIdx.z each: Plane
+// with src and dst at the group's first frame, and the strides from one frame to the next.  src_words / dst_words hold
+// for every frame of the group (an odd frame stride clears them).  (A separate type, so that the one-frame kernels keep
+// their parameter block byte for byte.)
+struct PlaneBatch : Plane {
+    int64_t src_sn, dst_sn;  // frame strides in elements (the pipeline input's may be negative or zero)
+};
+template<bool FR>
+using PlaneOf = std::conditional_t<FR, PlaneBatch, Plane>;
+
+// The source and destination of the block's frame: blockIdx.z's in an FR instance, the parameter block's own otherwise.
+// The parameter block is never written.
+template<bool FR>
+__device__ __forceinline__ const uint16_t *frame_src(const PlaneOf<FR> &p) {
+    if constexpr (FR) return p.src + (int64_t)blockIdx.z * p.src_sn;
+    else return p.src;
+}
+template<bool FR>
+__device__ __forceinline__ uint16_t *frame_dst(const PlaneOf<FR> &p) {
+    if constexpr (FR) return p.dst + (int64_t)blockIdx.z * p.dst_sn;
+    else return p.dst;
+}
 
 // ---- register-window kernel (kFuse stages per launch) -------------------------------------------------------------
 // The tile lives in shared memory as 32-bit words (two pixels), every edge length is a compile-time constant, and each
@@ -120,8 +148,8 @@ struct StencilStages<EDGE, 0> {
     static __device__ __forceinline__ const uint32_t *run(uint32_t *cur, uint32_t *, uint32_t *, int) { return cur; }
 };
 
-template<int FUSE>
-__global__ void __launch_bounds__(256) stencil_chain_window_kernel(Plane p) {
+template<int FUSE, bool FR = false>
+__global__ void __launch_bounds__(256) stencil_chain_window_kernel(PlaneOf<FR> p) {
     static_assert(FUSE >= 1 && FUSE <= kFuse, "the shared-memory tiles hold an input tile of kFuse stages at most");
     constexpr int IN = kTile + 4 * FUSE, INW = IN / 2;
     __shared__ uint32_t A[kTileIn * kPW];
@@ -138,10 +166,10 @@ __global__ void __launch_bounds__(256) stencil_chain_window_kernel(Plane p) {
         if (p.do_clamp) {
             const int cy = min(max(sy + p.clamp_y0, 0), p.clamp_h - 1);
             const int cx0 = min(max(sx + p.clamp_x0, 0), p.clamp_w - 1), cx1 = min(max(sx + 1 + p.clamp_x0, 0), p.clamp_w - 1);
-            const uint16_t *row = p.src + (int64_t)cy * p.src_sy;
+            const uint16_t *row = frame_src<FR>(p) + (int64_t)cy * p.src_sy;
             w = (uint32_t)row[cx0] | ((uint32_t)row[cx1] << 16);
         } else if (sy < p.src_h) {
-            const uint16_t *e = p.src + (int64_t)sy * p.src_sy + sx;
+            const uint16_t *e = frame_src<FR>(p) + (int64_t)sy * p.src_sy + sx;
             if (p.src_words && sx + 1 < p.src_w) {
                 w = *reinterpret_cast<const uint32_t *>(e);
             } else {
@@ -159,7 +187,7 @@ __global__ void __launch_bounds__(256) stencil_chain_window_kernel(Plane p) {
         const int dx = ox + 2 * lw, dy = oy + ly;
         if (dy >= p.dst_h || dx >= p.dst_w) continue;
         const uint32_t w = res[ly * kPW + lw];
-        uint16_t *e = p.dst + (int64_t)dy * p.dst_sy + dx;
+        uint16_t *e = frame_dst<FR>(p) + (int64_t)dy * p.dst_sy + dx;
         if (p.dst_words && dx + 1 < p.dst_w) {
             *reinterpret_cast<uint32_t *>(e) = w;
         } else {
@@ -175,34 +203,59 @@ const halide_filter_argument_t kArgs[2] = {
     {"input", halide_argument_kind_input_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
     {"output", halide_argument_kind_output_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
+// The batch entry points: the same buffers with a third dimension, the frame index n.
+const halide_filter_argument_t kBatchArgs[2] = {
+    {"input", halide_argument_kind_input_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+    {"output", halide_argument_kind_output_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
+};
 
-// One launch of `fuse` stages (1..kFuse).  Every depth is the same kernel and carries the same name.
-void launch_window(int fuse, const Plane &p, cudaStream_t s) {
-    const dim3 grid((p.dst_w + kTile - 1) / kTile, (p.dst_h + kTile - 1) / kTile);
+// Scratch a clip's call may hold: its frames run in groups whose intermediate planes together fit in kScratchBudget
+// bytes (at least one frame a group, however large its planes), and the groups reuse one allocation per plane.  The
+// device pool keeps freed blocks until they are released, so scratch sized to a whole clip would stay allocated after
+// the call.  At S = 32, 256 MiB holds the two planes of 1 frame of 7680 x 4320 (138 MB), 7 of 3840 x 2160 (36 MB
+// each), 27 of 1920 x 1080 and 150 of 640 x 480; chains of 4 stages or fewer need no scratch, so their groups hold up
+// to kMaxGridZ frames.  A group of one frame runs through the one-frame kernels.  No minimum group size is set: groups
+// of 2 or 3 frames were not measured against single calls (H100 80GB HBM3 at 700 W: 4 x 7680 x 4320 at S = 4, one
+// group of 4, took 0.991 of four one-frame calls; at S = 32 and 100, one frame a group, 1.000).
+constexpr size_t kScratchBudget = size_t(256) << 20;
+
+// One launch of `fuse` stages (1..kFuse) on `frames` frames (FR) or on one frame.  Every depth is the same kernel and
+// carries the same name.
+template<bool FR>
+void launch_window(int fuse, const PlaneOf<FR> &p, int frames, cudaStream_t s) {
+    const dim3 grid((p.dst_w + kTile - 1) / kTile, (p.dst_h + kTile - 1) / kTile, frames);
     switch (fuse) {
-    case 1: HB_LAUNCH("stencil_chain_window", stencil_chain_window_kernel<1>, grid, 256, 0, s, p); break;
-    case 2: HB_LAUNCH("stencil_chain_window", stencil_chain_window_kernel<2>, grid, 256, 0, s, p); break;
-    case 3: HB_LAUNCH("stencil_chain_window", stencil_chain_window_kernel<3>, grid, 256, 0, s, p); break;
-    default: HB_LAUNCH("stencil_chain_window", stencil_chain_window_kernel<kFuse>, grid, 256, 0, s, p); break;
+    case 1: HB_LAUNCH("stencil_chain_window", (stencil_chain_window_kernel<1, FR>), grid, 256, 0, s, p); break;
+    case 2: HB_LAUNCH("stencil_chain_window", (stencil_chain_window_kernel<2, FR>), grid, 256, 0, s, p); break;
+    case 3: HB_LAUNCH("stencil_chain_window", (stencil_chain_window_kernel<3, FR>), grid, 256, 0, s, p); break;
+    default: HB_LAUNCH("stencil_chain_window", (stencil_chain_window_kernel<kFuse, FR>), grid, 256, 0, s, p); break;
     }
 }
 
-// The chain of S = `stencils` stages.  Launch plan: floor(S / kFuse) launches of kFuse stages, then, when S mod kFuse
-// is not 0, one launch of the remaining stages.  Launch k reads the region grown by Rin = 2 * (stages not yet run) and
-// writes it grown by Rout = Rin - 2 * (its stages); the last launch writes the output itself.  Putting the short launch
-// last keeps every intermediate apron, and with it the scratch (largest at launch 0: 2 * (S - kFuse)), as small as the
-// order allows.  S = 32 is stencil_chain: 8 launches of 4 stages.
-int run_stencil_chain(halide_buffer_t *input, int32_t stencils, halide_buffer_t *output) {
+// Every stencil_chain entry point: the chain of S = `stencils` stages.  Launch plan: floor(S / kFuse) launches of kFuse
+// stages, then, when S mod kFuse is not 0, one launch of the remaining stages.  Launch k reads the region grown by
+// Rin = 2 * (stages not yet run) and writes it grown by Rout = Rin - 2 * (its stages); the last launch writes the output
+// itself.  Putting the short launch last keeps every intermediate apron, and with it the scratch (largest at launch 0:
+// 2 * (S - kFuse)), as small as the order allows.  S = 32 is stencil_chain: 8 launches of 4 stages.
+// 2-D (x, y) records take one frame; 3-D (x, y, n) ones a clip, output frame n reading input frame n (repeat_edge in x
+// and y within the frame, never across frames), whose frames run the launch plan in groups of up to G (see
+// kScratchBudget).
+int run_stencil_chain(halide_buffer_t *input, int32_t stencils, halide_buffer_t *output,
+                      const halide_filter_argument_t *rec, const char *what) {
     int r;
-    hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[1]}};
+    hb::Arg args[2] = {{input, rec[0]}, {output, rec[1]}};
     if ((r = hb::check_args(args, 2))) return r;
-    // every access to the input goes through repeat_edge: nothing beyond a non-empty buffer is
-    // required; a query is answered with the output region.
+    const bool batch = output->dimensions == 3;
+    // every access to the input goes through repeat_edge in x and y: nothing beyond a non-empty frame is required there;
+    // a clip's output frame n reads input frame n, not clamped: the input's frames must cover the output's (dimension 2).
+    // A query is answered with the output region.
+    const int on = batch ? output->dim[2].min : 0, N = batch ? output->dim[2].extent : 1;
     const hb::Region need[2] = {hb::region_of(output, false), hb::region_of(output, false)};
+    const hb::Region frames[1] = {{{0, 0, on}, {0, 0, N}, true}};  // (extents of 0: x and y are not checked)
     if (hb::answer_bounds_query(args, need, 2)) return 0;
-    if ((r = hb::check_shapes(args, 2))) return r;
+    if ((r = hb::check_shapes(args, 2)) || (r = hb::check_required(args, frames, 1))) return r;
     const int W = output->dim[0].extent, H = output->dim[1].extent;
-    if (W <= 0 || H <= 0) return 0;
+    if (W <= 0 || H <= 0 || N <= 0) return 0;
     if (input->dim[0].extent <= 0 || input->dim[1].extent <= 0) {
         return hb::fail(halide_error_code_access_out_of_bounds, "Input buffer input is empty");
     }
@@ -216,67 +269,95 @@ int run_stencil_chain(halide_buffer_t *input, int32_t stencils, halide_buffer_t 
     const int full = S / kFuse, rest = S % kFuse;
     const int groups = full + (rest ? 1 : 0);
 
-    // ping-pong buffers for the intermediate stages on their grown regions
+    // ping-pong buffers for the intermediate stages on their grown regions, G frames side by side in each
     const int maxR = groups > 1 ? 2 * (S - kFuse) : 0;
-    hb::Scratch scratch;
     const int64_t bw = (W + 2 * maxR + 1) & ~(int64_t)1, bh = H + 2 * maxR;  // (even pitch: intermediate rows keep pixel pairs word-aligned)
+    const int planes = groups > 2 ? 2 : groups > 1 ? 1 : 0;
+    const size_t frame_bytes = (size_t)planes * bw * bh * sizeof(uint16_t);
+    const size_t fit = frame_bytes ? std::max<size_t>(1, kScratchBudget / frame_bytes) : (size_t)hb::kMaxGridZ;
+    const int G = (int)std::min<size_t>({(size_t)N, (size_t)hb::kMaxGridZ, fit});
+    hb::Scratch scratch;
     uint16_t *buf[2] = {nullptr, nullptr};
     if (groups > 1) {
-        buf[0] = scratch.get<uint16_t>((size_t)bw * bh);
-        buf[1] = groups > 2 ? scratch.get<uint16_t>((size_t)bw * bh) : buf[0];
+        buf[0] = scratch.get<uint16_t>((size_t)bw * bh * G);
+        buf[1] = groups > 2 ? scratch.get<uint16_t>((size_t)bw * bh * G) : buf[0];
         if (!buf[0] || !buf[1]) return hb::fail(halide_error_code_device_malloc_failed, "stencil_chain: scratch allocation failed");
     }
+    // the input frame output frame 0 reads, and the frame strides
+    const int64_t in_sn = batch ? input->dim[2].stride : 0, out_sn = batch ? output->dim[2].stride : 0;
+    const uint16_t *in0 = (const uint16_t *)args[0].dev + (batch ? (int64_t)(on - input->dim[2].min) * in_sn : 0);
+    uint16_t *out0 = (uint16_t *)args[1].dev;
     cudaStream_t s = hb::stream();
     {
         hb::CallTimer timer(s);
-        for (int g = 0; g < groups; g++) {
-            const int F = g < full ? kFuse : rest;          // stages this launch runs
-            const int Rin = 2 * (S - g * kFuse);            // apron of the region this launch reads
-            const int Rout = Rin - 2 * F;                   // apron of the region it writes
-            Plane p;
-            p.dst_w = W + 2 * Rout;
-            p.dst_h = H + 2 * Rout;
-            p.src_w = W + 2 * Rin;
-            p.src_h = H + 2 * Rin;
-            if (g == 0) {
-                p.src = (const uint16_t *)args[0].dev;
-                p.src_sy = input->dim[1].stride;
-                p.do_clamp = 1;
-                // source-region local (0,0) is absolute (ox - Rin, oy - Rin); buffer-relative = minus input min
-                p.clamp_x0 = output->dim[0].min - Rin - input->dim[0].min;
-                p.clamp_y0 = output->dim[1].min - Rin - input->dim[1].min;
-                p.clamp_w = input->dim[0].extent;
-                p.clamp_h = input->dim[1].extent;
-            } else {
-                p.src = buf[(g - 1) & 1];
-                p.src_sy = bw;
-                p.do_clamp = 0;
-                p.clamp_x0 = p.clamp_y0 = p.clamp_w = p.clamp_h = 0;
+        for (int n0 = 0; n0 < N; n0 += G) {  // frames [n0, n0 + gn): scratch frames 0 .. gn - 1
+            const int gn = std::min(G, N - n0);
+            for (int g = 0; g < groups; g++) {
+                const int F = g < full ? kFuse : rest;          // stages this launch runs
+                const int Rin = 2 * (S - g * kFuse);            // apron of the region this launch reads
+                const int Rout = Rin - 2 * F;                   // apron of the region it writes
+                PlaneBatch p;
+                p.dst_w = W + 2 * Rout;
+                p.dst_h = H + 2 * Rout;
+                p.src_w = W + 2 * Rin;
+                p.src_h = H + 2 * Rin;
+                if (g == 0) {
+                    p.src = in0 + (int64_t)n0 * in_sn;
+                    p.src_sy = input->dim[1].stride;
+                    p.src_sn = in_sn;
+                    p.do_clamp = 1;
+                    // source-region local (0,0) is absolute (ox - Rin, oy - Rin); buffer-relative = minus input min
+                    p.clamp_x0 = output->dim[0].min - Rin - input->dim[0].min;
+                    p.clamp_y0 = output->dim[1].min - Rin - input->dim[1].min;
+                    p.clamp_w = input->dim[0].extent;
+                    p.clamp_h = input->dim[1].extent;
+                } else {
+                    p.src = buf[(g - 1) & 1];
+                    p.src_sy = bw;
+                    p.src_sn = bw * bh;
+                    p.do_clamp = 0;
+                    p.clamp_x0 = p.clamp_y0 = p.clamp_w = p.clamp_h = 0;
+                }
+                if (g == groups - 1) {
+                    p.dst = out0 + (int64_t)n0 * out_sn;
+                    p.dst_sy = output->dim[1].stride;
+                    p.dst_sn = out_sn;
+                } else {
+                    p.dst = buf[g & 1];
+                    p.dst_sy = bw;
+                    p.dst_sn = bw * bh;
+                }
+                // 32-bit accesses only where every frame of the group keeps pixel pairs 4-byte aligned
+                const int64_t src_sn = gn > 1 ? p.src_sn : 0, dst_sn = gn > 1 ? p.dst_sn : 0;
+                p.src_words = ((reinterpret_cast<uintptr_t>(p.src) & 3) == 0 && ((p.src_sy | src_sn) & 1) == 0) ? 1 : 0;
+                p.dst_words = ((reinterpret_cast<uintptr_t>(p.dst) & 3) == 0 && ((p.dst_sy | dst_sn) & 1) == 0) ? 1 : 0;
+                if (G > 1) launch_window<true>(F, p, gn, s);
+                else launch_window<false>(F, p, 1, s);
             }
-            if (g == groups - 1) {
-                p.dst = (uint16_t *)args[1].dev;
-                p.dst_sy = output->dim[1].stride;
-            } else {
-                p.dst = buf[g & 1];
-                p.dst_sy = bw;
-            }
-            p.src_words = ((reinterpret_cast<uintptr_t>(p.src) & 3) == 0 && (p.src_sy & 1) == 0) ? 1 : 0;
-            p.dst_words = ((reinterpret_cast<uintptr_t>(p.dst) & 3) == 0 && (p.dst_sy & 1) == 0) ? 1 : 0;
-            launch_window(F, p, s);
         }
     }
-    return hb::finish(args, 2, "stencil_chain launch");
+    return hb::finish(args, 2, what);
 }
 }  // namespace
 
 extern "C" int stencil_chain(halide_buffer_t *input, halide_buffer_t *output) {
-    return run_stencil_chain(input, kStages, output);
+    return run_stencil_chain(input, kStages, output, kArgs, "stencil_chain launch");
 }
 
 // stencil_chain with the stencils GeneratorParam as a run-time argument: what the generator built with stencils = S
 // computes, for S in [1, 100].  Buffer rules, error codes and the bounds query are stencil_chain's.
 extern "C" int halide_b200_stencil_chain_stencils(halide_buffer_t *input, int32_t stencils, halide_buffer_t *output) {
-    return run_stencil_chain(input, stencils, output);
+    return run_stencil_chain(input, stencils, output, kArgs, "stencil_chain launch");
 }
 HB_EXPORT_FILTER(stencil_chain, kArgs)
 HB_EXPORT_AUTO_SCHEDULE(stencil_chain, kArgs)
+
+// Batch entry points (library extensions): stencil_chain and halide_b200_stencil_chain_stencils on every frame of a 3-D
+// (x, y, n) buffer, the launch plan run once per group of frames; output frame n is, bit for bit, the one-frame entry
+// point's result on input frame n.
+extern "C" int halide_b200_stencil_chain_batch(halide_buffer_t *input, halide_buffer_t *output) {
+    return run_stencil_chain(input, kStages, output, kBatchArgs, "stencil_chain_batch launch");
+}
+extern "C" int halide_b200_stencil_chain_stencils_batch(halide_buffer_t *input, int32_t stencils, halide_buffer_t *output) {
+    return run_stencil_chain(input, stencils, output, kBatchArgs, "stencil_chain_batch launch");
+}

@@ -455,6 +455,24 @@ int halide_b200_ll_last_own_level(int32_t frame_w, int32_t frame_h, int32_t pyra
  * from S = 5 to 8, none below 5). */
 int halide_b200_stencil_chain_stencils(struct halide_buffer_t *input, int32_t stencils, struct halide_buffer_t *output);
 
+/* halide_blur, stencil_chain and halide_b200_stencil_chain_stencils on video clips: 3-D (x, y, n) uint16 buffers, e.g.
+ * an (N, H, W) tensor.  Output frame n is, bit for bit, what the one-frame entry point gives on input frame n with the
+ * same arguments; frames are independent (stencil_chain's repeat_edge applies in x and y within each frame, and nothing
+ * is clamped or shared across n).  output->dim[2].min selects the input frame each output frame reads, and the input's
+ * frames must cover the output's (else halide_error_code_access_out_of_bounds, naming dimension 2).  In x and y:
+ * blur_batch needs [ox, ox + W + 1] x [oy, oy + H + 1] of every output frame, as halide_blur does; the stencil_chain
+ * batches need a non-empty input, as stencil_chain does.  A bounds query gives the input that region (stencil_chain: the
+ * output's), extended by the output's frame range, with dense strides.  Strides: as halide_b200_bilateral_grid_batch's
+ * (dim[0].stride == 1; rows may be padded, frames may be crops of a larger array, and frame strides may be negative or,
+ * on the input, zero).  blur_batch is one launch for any N.  The stencil_chain batches run the launch plan once per group
+ * of frames, ceil(S / 4) launches a group; a group holds as many frames as their scratch planes fit in 256 MiB, at most
+ * 65 535, and a group of one frame runs the one-frame kernels.  Everything else follows the one-frame entry points: the
+ * argument checks and their order, stencils in [1, 100] with the same message, size limits and error codes; an empty
+ * output (W, H or N of 0) returns 0 before the parameter checks and any CUDA call.  stencil_chain_batch runs S = 32. */
+int halide_b200_blur_batch(struct halide_buffer_t *input, struct halide_buffer_t *blur_y);
+int halide_b200_stencil_chain_batch(struct halide_buffer_t *input, struct halide_buffer_t *output);
+int halide_b200_stencil_chain_stencils_batch(struct halide_buffer_t *input, int32_t stencils, struct halide_buffer_t *output);
+
 /* Host-only probe of the band geometry for tests: with level jr gathered, out[j*8..j*8+7] = {own.lo, own.hi, d.lo, d.hi,
  * u.lo, u.hi, S.lo, S.hi} per pyramid level j = 0..7 (rows owned in the gather partition / Gaussian-side rows computed and
  * held / outGPyramid rows needed / the level's rows on the whole frame), out[64..65] = input rows read. */
@@ -474,7 +492,8 @@ void halide_b200_ll_force_generic(int mask);
  * call does from its lookup to its last launch; taking builds the table if it is missing.  A held table is never evicted
  * from the cache.  0, or a negative halide_error_code_t (dropping a table that is not held: generic_error). */
 int halide_b200_ll_lut_hold(int32_t levels, float alpha, int32_t hold);
-/* halide_blur test hook: 1 = route 4-byte-aligned frames through the general (any alignment) kernel as well;
+/* halide_blur (and halide_b200_blur_batch) test hook: 1 = route 4-byte-aligned frames through the general (any alignment)
+ * kernel as well;
  * >= 8 = aligned kernel with strips of that many rows (0 restores the defaults). */
 void halide_b200_blur_force_general(int enable);
 /* nl_means test hook: 1 = generic kernel for every patch / search size, so it can be checked on the sizes the

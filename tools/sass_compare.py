@@ -14,7 +14,8 @@ first template parameter is also tried without it when that type is float: `f<fl
 demangled name of a template instance also carries its return type, `void `), `f<float, 3, 7>(` as `f<3, 7>(`
 (bg_hist_blurz_kernel, bg_slice_kernel, nl_means_kernel, nl_means_window_kernel; the bilateral_grid kernels also gained
 the frame-walk parameter `bool FR = false` after it).  A plain kernel that became a template of one defaulted `bool`
-is tried without it: `f<false>(` as `f(` (bg_blur_xy_kernel, bg_hist_blurz_s_kernel, bg_slice_s_kernel).  An old kernel
+is tried without it: `f<false>(` as `f(` (bg_blur_xy_kernel, bg_hist_blurz_s_kernel, bg_slice_s_kernel, blur3x3_u16_kernel;
+blur3x3_u16_quad_kernel<6> and stencil_chain_window_kernel<F> gained `bool FR = false` as a trailing default).  An old kernel
 with no new one of its name is also matched by name and template arguments alone, with the parameter list and a last
 template argument `0` dropped on both sides (a plain function: by name alone): the template arguments fix the parameter
 types however they are spelled (nl_means's and bilateral_grid's kernels take theirs through an alias, which demangles as
