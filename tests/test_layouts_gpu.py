@@ -55,7 +55,10 @@ def pitch(w, kind):
 
 def layout(shape, lay):
     """(memory shape, view(mem) -> (writable view, view of the logical shape)) for `lay` (a name or a (kind, axis)
-    pair).  A broadcast view is written through its writable view of extent 1 on the broadcast axis."""
+    pair, or a function of the shape giving that pair for a layout of the caller's own).  A broadcast view is written
+    through its writable view of extent 1 on the broadcast axis."""
+    if callable(lay):
+        return lay(tuple(shape))
     kind, axis = NAMED[lay] if isinstance(lay, str) else lay
     shape = tuple(shape)
     p = pitch(shape[-1], kind)
