@@ -530,19 +530,10 @@ const halide_filter_argument_t kArgs[3] = {
     {"bilateral_grid", halide_argument_kind_output_buffer, 2, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
 // halide_b200_bilateral_grid_u8: the same buffers in uint8.
-const halide_filter_argument_t kU8Args[2] = {
-    {"input", halide_argument_kind_input_buffer, 2, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-    {"bilateral_grid", halide_argument_kind_output_buffer, 2, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-};
+const halide_filter_argument_t kU8Args[2] = {hb::variant(kArgs[0], 0, hb::kU8), hb::variant(kArgs[2], 0, hb::kU8)};
 // The batch entry points: the same buffers with a third dimension, the frame index n (float32, then uint8).
-const halide_filter_argument_t kBatchArgs[2] = {
-    {"input", halide_argument_kind_input_buffer, 3, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-    {"bilateral_grid", halide_argument_kind_output_buffer, 3, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-};
-const halide_filter_argument_t kU8BatchArgs[2] = {
-    {"input", halide_argument_kind_input_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-    {"bilateral_grid", halide_argument_kind_output_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-};
+const halide_filter_argument_t kBatchArgs[2] = {hb::variant(kArgs[0], 1), hb::variant(kArgs[2], 1)};
+const halide_filter_argument_t kU8BatchArgs[2] = {hb::variant(kArgs[0], 1, hb::kU8), hb::variant(kArgs[2], 1, hb::kU8)};
 
 // Scratch a clip's call may hold: its frames are filtered in groups whose two grids together fit in kGridBudget bytes
 // (at least one frame a group, however large its grids), and the groups reuse one pair of allocations.  The device pool
@@ -616,13 +607,13 @@ int run_bilateral_grid(halide_buffer_t *input, int s_sigma, float r_sigma, halid
     int r;
     hb::Arg args[2] = {{input, in_rec}, {output, out_rec}};
     if ((r = hb::check_args(args, 2))) return r;
-    const bool batch = output->dimensions == 3;
+    const hb::Clip c = hb::clip_of(args[0], args[1], 2);
     // the slice reads input(x,y) unclamped (generator :50): the input must cover the output region, and a clip's output
     // frame n reads input frame n, not clamped either: the input's frames must cover the output's (dimension 2)
     const hb::Region need[2] = {hb::region_of(output, true), hb::region_of(output, false)};
     if (hb::answer_bounds_query(args, need, 2)) return 0;
     if ((r = hb::check_shapes(args, 2)) || (r = hb::check_required(args, need, 2))) return r;
-    const int W = output->dim[0].extent, H = output->dim[1].extent, N = batch ? output->dim[2].extent : 1;
+    const int W = output->dim[0].extent, H = output->dim[1].extent, N = c.N;
     if (W <= 0 || H <= 0 || N <= 0) return 0;
     if (s_sigma < 1 || s_sigma > 128) {
         return hb::fail(s_sigma < 1 ? halide_error_code_param_too_small : halide_error_code_param_too_large,
@@ -644,7 +635,7 @@ int run_bilateral_grid(halide_buffer_t *input, int s_sigma, float r_sigma, halid
     if ((r = hb::acquire(args, 2))) return r;
 
     const int ox = output->dim[0].min, oy = output->dim[1].min;
-    p.in = (const float *)args[0].dev;
+    p.in = (const float *)((const T *)args[0].dev + c.in_off);  // the input frame output frame 0 reads
     p.in_sy = input->dim[1].stride;
     p.in_x0 = input->dim[0].min; p.in_y0 = input->dim[1].min;
     p.in_w = input->dim[0].extent; p.in_h = input->dim[1].extent;
@@ -660,14 +651,11 @@ int run_bilateral_grid(halide_buffer_t *input, int s_sigma, float r_sigma, halid
     // G frames a group: G = min(N, kMaxGridZ, max(1, kGridBudget / (two grids of one frame))), or 1 frame at a time
     // through the one-frame kernels when fewer than kMinGroup frames fit the budget
     const size_t fit = std::max<size_t>(1, kGridBudget / (2 * gelems * sizeof(float)));
-    const bool groups = batch && fit >= kMinGroup;
+    const bool groups = c.clip && fit >= kMinGroup;
     const int G = groups ? (int)std::min<size_t>({(size_t)N, (size_t)hb::kMaxGridZ, fit}) : 1;
-    p.in_sn = batch ? input->dim[2].stride : 0;
-    p.out_sn = batch ? output->dim[2].stride : 0;
+    p.in_sn = c.in_sn;
+    p.out_sn = c.out_sn;
     p.grid_sn = (int64_t)gelems;
-    if (batch) {  // the input frame output frame 0 reads
-        p.in = (const float *)((const T *)p.in + (int64_t)(output->dim[2].min - input->dim[2].min) * p.in_sn);
-    }
     hb::Scratch scratch;
     p.grid_a = scratch.get<float>(gelems * G);
     p.grid_b = scratch.get<float>(gelems * G);

@@ -348,10 +348,7 @@ const halide_filter_argument_t kArgs[2] = {
     {"blur_y", halide_argument_kind_output_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
 };
 // The batch entry point: the same buffers with a third dimension, the frame index n.
-const halide_filter_argument_t kBatchArgs[2] = {
-    {"input", halide_argument_kind_input_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-    {"blur_y", halide_argument_kind_output_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-};
+const halide_filter_argument_t kBatchArgs[2] = {hb::variant(kArgs[0], 1), hb::variant(kArgs[1], 1)};
 
 // The one launch of a frame (FR false) or of a clip (FR): the pair kernel when `pair_ok`, the general one otherwise.
 template<bool FR>
@@ -396,13 +393,12 @@ int run_blur(halide_buffer_t *input, halide_buffer_t *blur_y, const halide_filte
     int r;
     hb::Arg args[2] = {{input, rec[0]}, {blur_y, rec[1]}};
     if ((r = hb::check_args(args, 2))) return r;
-    const bool batch = blur_y->dimensions == 3;
+    const hb::Clip c = hb::clip_of(args[0], args[1], 2);
     // The input must cover the output region grown by the 3-tap footprints: [ox, ox+W+1] x [oy, oy+H+1]; a clip's output
     // frame n reads input frame n, not clamped either: the input's frames must cover the output's (dimension 2).
     const int ox = blur_y->dim[0].min, oy = blur_y->dim[1].min;
-    const int w = blur_y->dim[0].extent, h = blur_y->dim[1].extent;
-    const int on = batch ? blur_y->dim[2].min : 0, N = batch ? blur_y->dim[2].extent : 1;
-    const hb::Region need[2] = {{{ox, oy, on}, {w + 2, h + 2, N}, true}, hb::region_of(blur_y, false)};
+    const int w = blur_y->dim[0].extent, h = blur_y->dim[1].extent, N = c.N;
+    const hb::Region need[2] = {c.with_frames({{ox, oy}, {w + 2, h + 2}, true}), hb::region_of(blur_y, false)};
     if (hb::answer_bounds_query(args, need, 2)) return 0;
     if ((r = hb::check_shapes(args, 2)) || (r = hb::check_required(args, need, 2))) return r;
     if (w <= 0 || h <= 0 || N <= 0) return 0;
@@ -410,25 +406,20 @@ int run_blur(halide_buffer_t *input, halide_buffer_t *blur_y, const halide_filte
 
     BlurBatchArgs a;
     const int64_t isy = input->dim[1].stride;
-    const int64_t isn = batch ? input->dim[2].stride : 0;
-    const int64_t origin = (int64_t)(ox - input->dim[0].min) + (int64_t)(oy - input->dim[1].min) * isy +
-                           (batch ? (int64_t)(on - input->dim[2].min) * isn : 0);
+    const int64_t origin = (int64_t)(ox - input->dim[0].min) + (int64_t)(oy - input->dim[1].min) * isy + c.in_off;
     a.in = (const uint16_t *)args[0].dev + origin;
     a.out = (uint16_t *)args[1].dev;
     a.in_stride_y = isy;
     a.out_stride_y = blur_y->dim[1].stride;
     a.w = w;
     a.h = h;
-    a.in_sn = isn;
-    a.out_sn = batch ? blur_y->dim[2].stride : 0;
+    a.in_sn = c.in_sn;
+    a.out_sn = c.out_sn;
     a.n = N;
-    // allocation span of the input relative to a.in (dim0 stride is 1; the dim1 and dim2 strides may be negative, and a
-    // clip's frame stride 0)
-    int64_t lo = 0, hi = input->dim[0].extent - 1;
-    for (int d = 1; d < input->dimensions; d++) {
-        const int64_t reach = (int64_t)(input->dim[d].extent - 1) * input->dim[d].stride;
-        (reach < 0 ? lo : hi) += reach;
-    }
+    // allocation span of the input relative to a.in (the dim1 and dim2 strides may be negative, and a clip's frame
+    // stride 0)
+    int64_t lo, hi;
+    hb::span_elems(input, &lo, &hi);
     a.in_lo = lo - origin;
     a.in_hi = hi - origin;
 
@@ -439,7 +430,7 @@ int run_blur(halide_buffer_t *input, halide_buffer_t *blur_y, const halide_filte
     cudaStream_t s = hb::stream();
     {
         hb::CallTimer timer(s);
-        if (batch) launch<true>(a, pair_ok, N, s);
+        if (c.clip) launch<true>(a, pair_ok, N, s);
         else launch<false>(a, pair_ok, 1, s);
     }
     return hb::finish(args, 2, what);

@@ -289,10 +289,7 @@ const halide_filter_argument_t kArgs[10] = {
     {"processed", halide_argument_kind_output_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, est_out_p},
 };
 // The burst entry points: the same buffers with a frame dimension n, input (x, y, n) and output (x, y, c, n).
-const halide_filter_argument_t kBatchArgs[2] = {
-    {"input", halide_argument_kind_input_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-    {"processed", halide_argument_kind_output_buffer, 4, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-};
+const halide_filter_argument_t kBatchArgs[2] = {hb::variant(kArgs[0], 1), hb::variant(kArgs[9], 1)};
 
 inline int fdiv(int a, int b) {
     int q = a / b;
@@ -317,15 +314,10 @@ int run_camera_pipe(hb::Arg *args, float color_temp, float gamma, float contrast
     int r;
     if ((r = hb::check_args(args, 4))) return r;
     halide_buffer_t *input = args[0].b, *m3200 = args[1].b, *m7000 = args[2].b, *out = args[3].b;
-    const bool batch = out->dimensions == 4;
-    const int ox = out->dim[0].min, oy = out->dim[1].min, W = out->dim[0].extent, H = out->dim[1].extent;
-    const int N = batch ? out->dim[3].extent : 1;
+    const hb::Clip c = hb::clip_of(args[0], args[3], 3);  // (output frame n reads input frame n)
+    const int ox = out->dim[0].min, oy = out->dim[1].min, W = out->dim[0].extent, H = out->dim[1].extent, N = c.N;
     const hb::Region matrix = {{0, 0}, {4, 3}, true};
-    hb::Region need[4] = {raw_region(ox, oy, W, H), matrix, matrix, hb::region_of(out, false)};
-    if (batch) {  // output frame n reads input frame n
-        need[0].min[2] = out->dim[3].min;
-        need[0].extent[2] = N;
-    }
+    const hb::Region need[4] = {c.with_frames(raw_region(ox, oy, W, H)), matrix, matrix, hb::region_of(out, false)};
     if (hb::answer_bounds_query(args, need, 4)) return 0;
     if ((r = hb::check_shapes(args, 4))) return r;
     if (W <= 0 || H <= 0 || out->dim[2].extent <= 0 || N <= 0) return 0;
@@ -340,15 +332,14 @@ int run_camera_pipe(hb::Arg *args, float color_temp, float gamma, float contrast
     if (!tab) return hb::fail(halide_error_code_device_malloc_failed, "camera_pipe: scratch allocation failed");
 
     CPParams p;
-    p.in = (const u16 *)args[0].dev;
+    p.in = (const u16 *)args[0].dev + c.in_off;  // the input frame output frame 0 reads
     p.in_sy = input->dim[1].stride;
-    p.in_sn = batch ? input->dim[2].stride : 0;
-    if (batch) p.in += (int64_t)(out->dim[3].min - input->dim[2].min) * p.in_sn;  // the input frame of the output's first
+    p.in_sn = c.in_sn;
     p.in_x0 = input->dim[0].min; p.in_y0 = input->dim[1].min;
     p.in_w = input->dim[0].extent; p.in_h = input->dim[1].extent;
     p.out = (u8 *)args[3].dev;
     p.out_sy = out->dim[1].stride; p.out_sc = out->dim[2].stride;
-    p.out_sn = batch ? out->dim[3].stride : 0;
+    p.out_sn = c.out_sn;
     p.out_px = out->dim[0].stride;
     p.out_x0 = ox; p.out_y0 = oy; p.W = W; p.H = H; p.C = out->dim[2].extent; p.out_c0 = out->dim[2].min; p.N = N;
     p.tab = tab;

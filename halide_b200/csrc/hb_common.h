@@ -126,6 +126,36 @@ int acquire(Arg *a, int n);
 // device-dirty.
 int finish(const Arg *a, int n, const char *what);
 
+// A clip entry point takes a filter's buffers with one more dimension, the last of each: the frame index n.  Output frame
+// n reads input frame n, and the input's frames must cover the output's.  clip_of describes the frames of an {input,
+// output} pair that passed check_args, whose output has `frame_dims` dimensions per frame; a one-frame call is N = 1 with
+// zero strides and offset 0.
+struct Clip {
+    bool clip;              // the buffers have the frame dimension
+    int in_dim;             // the input's frame dimension
+    int n_min, N;           // the output's frames [n_min, n_min + N)
+    int64_t in_sn, out_sn;  // frame strides, in elements
+    int64_t in_off;         // elements from the input's mins to the input frame output frame 0 reads
+    // r with the output's frames in the input's frame dimension (a one-frame call: r): the input's region for the bounds
+    // query and, must_cover, for check_required.
+    Region with_frames(Region r) const {
+        if (clip) r.min[in_dim] = n_min, r.extent[in_dim] = N;
+        return r;
+    }
+};
+Clip clip_of(const Arg &in, const Arg &out, int frame_dims);
+
+// The argument record of a library-extension entry point: the generator's record g with `more_dims` more dimensions (a
+// clip's frame index) and element type t, without estimates.  hb::Arg::meta refers to it, so it is kept in a
+// namespace-scope constant.
+constexpr halide_type_t kU8 = {halide_type_uint, 8, 0};
+inline halide_filter_argument_t variant(const halide_filter_argument_t &g, int more_dims, halide_type_t t) {
+    return {g.name, g.kind, g.dimensions + more_dims, t, nullptr, nullptr, nullptr, nullptr, nullptr};
+}
+inline halide_filter_argument_t variant(const halide_filter_argument_t &g, int more_dims) {
+    return variant(g, more_dims, g.type);
+}
+
 // Metadata default of a scalar argument: all 8 bytes zero but the member set.
 halide_scalar_value_t scalar_i32(int32_t v);
 halide_scalar_value_t scalar_f32(float v);
@@ -148,6 +178,8 @@ int call_argv(int (*f)(A...), void **args) {
 inline size_t elem_bytes(const halide_buffer_t *b) {
     return (b->type.bits + 7) / 8;
 }
+// Span of a buffer in elements relative to the element at the mins: [lo, hi] (empty dimensions add nothing).
+void span_elems(const halide_buffer_t *b, int64_t *lo, int64_t *hi);
 
 }  // namespace hb
 

@@ -158,18 +158,6 @@ KernelLimits &allow_smem_locked(const void *kernel, int dev, size_t bytes) {
     return k;
 }
 
-// Span of a buffer in elements relative to the element at the mins: [lo, hi].
-void span_elems(const halide_buffer_t *b, int64_t *lo, int64_t *hi) {
-    int64_t l = 0, h = 0;
-    for (int d = 0; d < b->dimensions; d++) {
-        int64_t reach = (int64_t)(b->dim[d].extent - 1) * b->dim[d].stride;
-        if (b->dim[d].extent <= 0) continue;
-        if (reach < 0) l += reach; else h += reach;
-    }
-    *lo = l;
-    *hi = h;
-}
-
 bool any_empty(const halide_buffer_t *b) {
     for (int d = 0; d < b->dimensions; d++) {
         if (b->dim[d].extent <= 0) return true;
@@ -190,7 +178,7 @@ int if_device_malloc(void *uc, halide_buffer_t *buf, const halide_device_interfa
         return 0;
     }
     int64_t lo, hi;
-    span_elems(buf, &lo, &hi);
+    hb::span_elems(buf, &lo, &hi);
     size_t bytes = (size_t)(hi - lo + 1) * hb::elem_bytes(buf);
     void *p = pool().alloc(bytes);
     if (!p) {
@@ -204,7 +192,7 @@ int if_device_malloc(void *uc, halide_buffer_t *buf, const halide_device_interfa
 
 void *alloc_base(const halide_buffer_t *buf) {
     int64_t lo, hi;
-    span_elems(buf, &lo, &hi);
+    hb::span_elems(buf, &lo, &hi);
     return (uint8_t *)buf->device + lo * (int64_t)hb::elem_bytes(buf);
 }
 
@@ -354,7 +342,7 @@ int if_copy_to_device(void *uc, halide_buffer_t *buf, const halide_device_interf
 
 int if_device_and_host_malloc(void *uc, halide_buffer_t *buf, const halide_device_interface_t *iface) {
     int64_t lo, hi;
-    span_elems(buf, &lo, &hi);
+    hb::span_elems(buf, &lo, &hi);
     size_t eb = hb::elem_bytes(buf);
     size_t bytes = (size_t)(hi - lo + 1) * eb;
     void *h = nullptr;
@@ -374,7 +362,7 @@ int if_device_and_host_malloc(void *uc, halide_buffer_t *buf, const halide_devic
 int if_device_and_host_free(void *uc, halide_buffer_t *buf) {
     if (buf->host) {
         int64_t lo, hi;
-        span_elems(buf, &lo, &hi);
+        hb::span_elems(buf, &lo, &hi);
         cudaFreeHost(buf->host + lo * (int64_t)hb::elem_bytes(buf));
         buf->host = nullptr;
     }
@@ -630,6 +618,22 @@ int check_args(const Arg *a, int n) {
     return 0;
 }
 
+Clip clip_of(const Arg &in, const Arg &out, int frame_dims) {
+    Clip c = {};
+    c.N = 1;
+    if (out.b->dimensions > frame_dims) {
+        c.clip = true;
+        c.in_dim = in.b->dimensions - 1;
+        const halide_dimension_t &i = in.b->dim[c.in_dim], &o = out.b->dim[out.b->dimensions - 1];
+        c.n_min = o.min;
+        c.N = o.extent;
+        c.in_sn = i.stride;
+        c.out_sn = o.stride;
+        c.in_off = ((int64_t)o.min - i.min) * i.stride;
+    }
+    return c;
+}
+
 bool answer_bounds_query(Arg *a, const Region *need, int n) {
     bool query = false;
     for (int i = 0; i < n; i++) {
@@ -756,6 +760,17 @@ int finish(const Arg *a, int n, const char *what) {
         a[i].b->flags |= halide_buffer_flag_device_dirty;
     }
     return 0;
+}
+
+void span_elems(const halide_buffer_t *b, int64_t *lo, int64_t *hi) {
+    int64_t l = 0, h = 0;
+    for (int d = 0; d < b->dimensions; d++) {
+        int64_t reach = (int64_t)(b->dim[d].extent - 1) * b->dim[d].stride;
+        if (b->dim[d].extent <= 0) continue;
+        if (reach < 0) l += reach; else h += reach;
+    }
+    *lo = l;
+    *hi = h;
 }
 
 halide_scalar_value_t scalar_i32(int32_t v) {

@@ -32,19 +32,10 @@ const halide_filter_argument_t kArgs[5] = {
     {"output", halide_argument_kind_output_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
 // halide_b200_local_laplacian_batch: the same buffers with a fourth dimension, the frame index n.
-const halide_filter_argument_t kBatchArgs[2] = {
-    {"input", halide_argument_kind_input_buffer, 4, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-    {"output", halide_argument_kind_output_buffer, 4, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-};
+const halide_filter_argument_t kBatchArgs[2] = {hb::variant(kArgs[0], 1), hb::variant(kArgs[4], 1)};
 // halide_b200_local_laplacian_u8 / _u8_batch: uint8 buffers of 3 / 4 dimensions.
-const halide_filter_argument_t kU8Args[2] = {
-    {"input", halide_argument_kind_input_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-    {"output", halide_argument_kind_output_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-};
-const halide_filter_argument_t kU8BatchArgs[2] = {
-    {"input", halide_argument_kind_input_buffer, 4, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-    {"output", halide_argument_kind_output_buffer, 4, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-};
+const halide_filter_argument_t kU8Args[2] = {hb::variant(kArgs[0], 0, hb::kU8), hb::variant(kArgs[4], 0, hb::kU8)};
+const halide_filter_argument_t kU8BatchArgs[2] = {hb::variant(kArgs[0], 1, hb::kU8), hb::variant(kArgs[4], 1, hb::kU8)};
 
 // Everything one call needs on the device: frame description + per-level buffers, for N frames of one geometry.
 // T = the frame's element type (uint16_t, or uint8_t for the 8-bit entry points).
@@ -111,8 +102,9 @@ int check_and_query(hb::Arg *args, int levels, bool *done, int J = ll::kMaxJ) {
 template<typename T>
 void fill_frame(PlanT<T> &p, const hb::Arg *args, int levels, float alpha, float beta) {
     const halide_buffer_t *input = args[0].b, *output = args[1].b;
+    const hb::Clip c = hb::clip_of(args[0], args[1], 3);
     LLFrameT<T> &f = p.f;
-    f.in = (const T *)args[0].dev;
+    f.in = (const T *)args[0].dev + c.in_off;  // output frame n reads input frame n
     f.in_sy = input->dim[1].stride; f.in_sc = input->dim[2].stride;
     f.in_x0 = input->dim[0].min; f.in_y0 = input->dim[1].min; f.in_c0 = input->dim[2].min;
     f.in_w = input->dim[0].extent; f.in_h = input->dim[1].extent; f.in_c = input->dim[2].extent;
@@ -128,16 +120,10 @@ void fill_frame(PlanT<T> &p, const hb::Arg *args, int levels, float alpha, float
     p.il = args[0].interleaved;
     p.fs.px_in = p.il ? input->dim[0].stride : 1;
     p.fs.px_out = p.il ? output->dim[0].stride : 1;
-    p.N = 1;
-    if (output->dimensions == 4) {
-        // output frame n reads input frame n: the output's first frame is (out n min - in n min) input frames past the
-        // input's mins
-        f.in += (int64_t)(output->dim[3].min - input->dim[3].min) * input->dim[3].stride;
-        p.N = output->dim[3].extent;
-        if (p.N > 1) {  // (one frame keeps stride 0: the same layout checks, hence kernels, as the 3-D call)
-            p.fs.in = input->dim[3].stride;
-            p.fs.out = output->dim[3].stride;
-        }
+    p.N = c.N;
+    if (p.N > 1) {  // (one frame keeps stride 0: the same layout checks, hence kernels, as the 3-D call)
+        p.fs.in = c.in_sn;
+        p.fs.out = c.out_sn;
     }
     f.levels = levels;
     f.beta = beta;

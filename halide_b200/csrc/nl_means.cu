@@ -330,20 +330,11 @@ const halide_filter_argument_t kArgs[5] = {
     {"non_local_means", halide_argument_kind_output_buffer, 3, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
 // halide_b200_nl_means_u8: the same buffers in uint8.
-const halide_filter_argument_t kU8Args[2] = {
-    {"input", halide_argument_kind_input_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-    {"non_local_means", halide_argument_kind_output_buffer, 3, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-};
+const halide_filter_argument_t kU8Args[2] = {hb::variant(kArgs[0], 0, hb::kU8), hb::variant(kArgs[4], 0, hb::kU8)};
 // The batch entry points: the same buffers with a fourth dimension, the frame index n (float32, then uint8).  The
 // interleaved entry points use these records and the ones above with hb::Arg::interleaved set.
-const halide_filter_argument_t kBatchArgs[2] = {
-    {"input", halide_argument_kind_input_buffer, 4, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-    {"non_local_means", halide_argument_kind_output_buffer, 4, {halide_type_float, 32, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-};
-const halide_filter_argument_t kU8BatchArgs[2] = {
-    {"input", halide_argument_kind_input_buffer, 4, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-    {"non_local_means", halide_argument_kind_output_buffer, 4, {halide_type_uint, 8, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-};
+const halide_filter_argument_t kBatchArgs[2] = {hb::variant(kArgs[0], 1), hb::variant(kArgs[4], 1)};
+const halide_filter_argument_t kU8BatchArgs[2] = {hb::variant(kArgs[0], 1, hb::kU8), hb::variant(kArgs[4], 1, hb::kU8)};
 
 // The one launch of a call: the register-window kernel at patch / search 3/7 and 7/7 (unless the variant hook asks for
 // the generic one), else the generic kernel.
@@ -373,14 +364,12 @@ int run_nl_means(hb::Arg *args, int32_t patch_size, int32_t search_area, float s
     int r;
     if ((r = hb::check_args(args, 2))) return r;
     halide_buffer_t *input = args[0].b, *output = args[1].b;
-    const bool batch = output->dimensions == 4, il = args[0].interleaved;
+    const hb::Clip c = hb::clip_of(args[0], args[1], 3);
+    const bool il = args[0].interleaved;
     // every input access is clamped in x, y and c: a query is answered with the output's x/y region, 3 channels and (a
     // batch) the output's frames
-    hb::Region region = {{output->dim[0].min, output->dim[1].min, 0}, {output->dim[0].extent, output->dim[1].extent, 3}, false};
-    if (batch) {
-        region.min[3] = output->dim[3].min;
-        region.extent[3] = output->dim[3].extent;
-    }
+    const hb::Region region =
+        c.with_frames({{output->dim[0].min, output->dim[1].min, 0}, {output->dim[0].extent, output->dim[1].extent, 3}, false});
     const hb::Region need[2] = {region, region};
     if (hb::answer_bounds_query(args, need, 2)) return 0;
     if ((r = hb::check_shapes(args, 2))) return r;
@@ -390,20 +379,14 @@ int run_nl_means(hb::Arg *args, int32_t patch_size, int32_t search_area, float s
                         "Constraint violated: non_local_means.min.2 (%d) == 0 and non_local_means.extent.2 (%d) == 3",
                         output->dim[2].min, output->dim[2].extent);
     }
-    const int W = output->dim[0].extent, H = output->dim[1].extent, N = batch ? output->dim[3].extent : 1;
+    const int W = output->dim[0].extent, H = output->dim[1].extent, N = c.N;
     if (W <= 0 || H <= 0 || N <= 0) return 0;
     if (input->dim[0].extent <= 0 || input->dim[1].extent <= 0 || input->dim[2].extent <= 0) {
         return hb::fail(halide_error_code_access_out_of_bounds, "Input buffer input is empty");
     }
     // output frame n reads input frame n, which is not clamped: the input's frames must cover the output's
-    if (batch) {
-        const int n0 = output->dim[3].min, n1 = n0 + N - 1, have0 = input->dim[3].min, have1 = have0 + input->dim[3].extent - 1;
-        if (n0 < have0 || n1 > have1) {
-            return hb::fail(halide_error_code_access_out_of_bounds,
-                            "Input buffer input is accessed at %d, which is %s the %s (%d) in dimension 3", n0 < have0 ? n0 : n1,
-                            n0 < have0 ? "before" : "beyond", n0 < have0 ? "min" : "max", n0 < have0 ? have0 : have1);
-        }
-    }
+    const hb::Region frames = c.with_frames({{}, {}, true});  // (extents of 0: x, y and c are not checked)
+    if ((r = hb::check_required(args, &frames, 1))) return r;
     if (patch_size < 1 || search_area < 1 || patch_size > 31 || search_area > 63) {
         return hb::fail(patch_size < 1 || search_area < 1 ? halide_error_code_param_too_small : halide_error_code_param_too_large,
                         "nl_means: patch_size %d / search_area %d outside the supported range [1,31] / [1,63]", patch_size,
@@ -412,7 +395,7 @@ int run_nl_means(hb::Arg *args, int32_t patch_size, int32_t search_area, float s
     if ((r = hb::acquire(args, 2))) return r;
 
     NLVideoParams q;
-    q.in = (const float *)args[0].dev;
+    q.in = (const float *)((const T *)args[0].dev + c.in_off);  // the input frame output frame 0 reads
     q.in_sy = input->dim[1].stride; q.in_sc = input->dim[2].stride;
     q.in_x0 = input->dim[0].min; q.in_y0 = input->dim[1].min; q.in_c0 = input->dim[2].min;
     q.in_w = input->dim[0].extent; q.in_h = input->dim[1].extent; q.in_c = input->dim[2].extent;
@@ -426,12 +409,9 @@ int run_nl_means(hb::Arg *args, int32_t patch_size, int32_t search_area, float s
     q.iw = TX + patch_size + search_area - 2; q.ih = TY + patch_size + search_area - 2;
     q.dw = TX + patch_size - 1; q.dh = TY + patch_size - 1;
     q.in_px = input->dim[0].stride; q.out_px = output->dim[0].stride;
-    q.in_sn = batch ? input->dim[3].stride : 0;
-    q.out_sn = batch ? output->dim[3].stride : 0;
+    q.in_sn = c.in_sn;
+    q.out_sn = c.out_sn;
     q.N = N;
-    if (batch) {  // the input frame output frame 0 reads
-        q.in = (const float *)((const T *)q.in + (int64_t)(output->dim[3].min - input->dim[3].min) * q.in_sn);
-    }
     const size_t fixed = (size_t)3 * q.iw * q.ih * sizeof(float);
     const size_t per_dx = (size_t)(q.dh + TY) * q.dw * sizeof(float);
     const size_t budget = 100 * 1024;
@@ -446,9 +426,9 @@ int run_nl_means(hb::Arg *args, int32_t patch_size, int32_t search_area, float s
     {
         hb::CallTimer timer(s);
         dim3 grid((W + TX - 1) / TX, (H + TY - 1) / TY, std::min(N, hb::kMaxGridZ));
-        if (il && batch) launch<T, true, true>(q, grid, smem, s);
+        if (il && c.clip) launch<T, true, true>(q, grid, smem, s);
         else if (il) launch<T, true, false>(q, grid, smem, s);
-        else if (batch) launch<T, false, true>(q, grid, smem, s);
+        else if (c.clip) launch<T, false, true>(q, grid, smem, s);
         else launch<T, false, false>(q, grid, smem, s);
     }
     return hb::finish(args, 2, what);

@@ -204,10 +204,7 @@ const halide_filter_argument_t kArgs[2] = {
     {"output", halide_argument_kind_output_buffer, 2, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, est_ptrs},
 };
 // The batch entry points: the same buffers with a third dimension, the frame index n.
-const halide_filter_argument_t kBatchArgs[2] = {
-    {"input", halide_argument_kind_input_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-    {"output", halide_argument_kind_output_buffer, 3, {halide_type_uint, 16, 0}, nullptr, nullptr, nullptr, nullptr, nullptr},
-};
+const halide_filter_argument_t kBatchArgs[2] = {hb::variant(kArgs[0], 1), hb::variant(kArgs[1], 1)};
 
 // Scratch a clip's call may hold: its frames run in groups whose intermediate planes together fit in kScratchBudget
 // bytes (at least one frame a group, however large its planes), and the groups reuse one allocation per plane.  The
@@ -245,15 +242,15 @@ int run_stencil_chain(halide_buffer_t *input, int32_t stencils, halide_buffer_t 
     int r;
     hb::Arg args[2] = {{input, rec[0]}, {output, rec[1]}};
     if ((r = hb::check_args(args, 2))) return r;
-    const bool batch = output->dimensions == 3;
+    const hb::Clip c = hb::clip_of(args[0], args[1], 2);
     // every access to the input goes through repeat_edge in x and y: nothing beyond a non-empty frame is required there;
     // a clip's output frame n reads input frame n, not clamped: the input's frames must cover the output's (dimension 2).
     // A query is answered with the output region.
-    const int on = batch ? output->dim[2].min : 0, N = batch ? output->dim[2].extent : 1;
+    const int N = c.N;
     const hb::Region need[2] = {hb::region_of(output, false), hb::region_of(output, false)};
-    const hb::Region frames[1] = {{{0, 0, on}, {0, 0, N}, true}};  // (extents of 0: x and y are not checked)
+    const hb::Region frames = c.with_frames({{}, {}, true});  // (extents of 0: x and y are not checked)
     if (hb::answer_bounds_query(args, need, 2)) return 0;
-    if ((r = hb::check_shapes(args, 2)) || (r = hb::check_required(args, frames, 1))) return r;
+    if ((r = hb::check_shapes(args, 2)) || (r = hb::check_required(args, &frames, 1))) return r;
     const int W = output->dim[0].extent, H = output->dim[1].extent;
     if (W <= 0 || H <= 0 || N <= 0) return 0;
     if (input->dim[0].extent <= 0 || input->dim[1].extent <= 0) {
@@ -283,9 +280,7 @@ int run_stencil_chain(halide_buffer_t *input, int32_t stencils, halide_buffer_t 
         buf[1] = groups > 2 ? scratch.get<uint16_t>((size_t)bw * bh * G) : buf[0];
         if (!buf[0] || !buf[1]) return hb::fail(halide_error_code_device_malloc_failed, "stencil_chain: scratch allocation failed");
     }
-    // the input frame output frame 0 reads, and the frame strides
-    const int64_t in_sn = batch ? input->dim[2].stride : 0, out_sn = batch ? output->dim[2].stride : 0;
-    const uint16_t *in0 = (const uint16_t *)args[0].dev + (batch ? (int64_t)(on - input->dim[2].min) * in_sn : 0);
+    const uint16_t *in0 = (const uint16_t *)args[0].dev + c.in_off;  // the input frame output frame 0 reads
     uint16_t *out0 = (uint16_t *)args[1].dev;
     cudaStream_t s = hb::stream();
     {
@@ -302,9 +297,9 @@ int run_stencil_chain(halide_buffer_t *input, int32_t stencils, halide_buffer_t 
                 p.src_w = W + 2 * Rin;
                 p.src_h = H + 2 * Rin;
                 if (g == 0) {
-                    p.src = in0 + (int64_t)n0 * in_sn;
+                    p.src = in0 + (int64_t)n0 * c.in_sn;
                     p.src_sy = input->dim[1].stride;
-                    p.src_sn = in_sn;
+                    p.src_sn = c.in_sn;
                     p.do_clamp = 1;
                     // source-region local (0,0) is absolute (ox - Rin, oy - Rin); buffer-relative = minus input min
                     p.clamp_x0 = output->dim[0].min - Rin - input->dim[0].min;
@@ -319,9 +314,9 @@ int run_stencil_chain(halide_buffer_t *input, int32_t stencils, halide_buffer_t 
                     p.clamp_x0 = p.clamp_y0 = p.clamp_w = p.clamp_h = 0;
                 }
                 if (g == groups - 1) {
-                    p.dst = out0 + (int64_t)n0 * out_sn;
+                    p.dst = out0 + (int64_t)n0 * c.out_sn;
                     p.dst_sy = output->dim[1].stride;
-                    p.dst_sn = out_sn;
+                    p.dst_sn = c.out_sn;
                 } else {
                     p.dst = buf[g & 1];
                     p.dst_sy = bw;
