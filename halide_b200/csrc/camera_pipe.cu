@@ -394,3 +394,31 @@ extern "C" int halide_b200_camera_pipe_interleaved_batch(halide_buffer_t *input,
     return run_camera_pipe(args, color_temp, gamma, contrast, sharpen_strength, blackLevel, whiteLevel,
                            "camera_pipe_interleaved_batch launch");
 }
+
+// Test hook: the tables of n scalar sets, one cp_tables launch each with the filter's own arguments (the curve is where
+// halide_pow meets the caller's scalars, so a test can sweep them without running the image kernel).
+extern "C" int halide_b200_camera_pipe_tables(const float *m3200, const float *m7000, const float *scalars, const int32_t *levels,
+                                              int n, int16_t *matrix, uint8_t *curve, uint8_t *s32) {
+    if (n <= 0) return 0;
+    if (!m3200 || !m7000 || !scalars || !levels || !matrix || !curve || !s32) {
+        return hb::fail(halide_error_code_generic_error, "halide_b200_camera_pipe_tables: null argument");
+    }
+    hb::Scratch scratch;
+    CPTables *tab = scratch.get<CPTables>(n);
+    if (!tab) return hb::fail(halide_error_code_device_malloc_failed, "camera_pipe_tables: scratch allocation failed");
+    const float c_diff = 1.0f / 7000 - 1.0f / 3200;
+    const float inv_c_diff = (float)(1.0 / (double)c_diff);
+    cudaStream_t s = hb::stream();
+    for (int i = 0; i < n; i++) {
+        const float *p = scalars + 4 * (size_t)i;
+        HB_LAUNCH("cp_tables", cp_tables_kernel, 4, 256, 0, s, tab + i, m3200, (int64_t)1, (int64_t)4, m7000, (int64_t)1, (int64_t)4,
+                  p[0], p[1], p[2], p[3], levels[2 * i], levels[2 * i + 1], inv_c_diff);
+    }
+    const size_t pitch = sizeof(CPTables);
+    cudaError_t e = cudaMemcpy2DAsync(matrix, sizeof(CPTables::matrix), tab->matrix, pitch, sizeof(CPTables::matrix), n,
+                                      cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpy2DAsync(curve, 1024, tab->curve, pitch, 1024, n, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpy2DAsync(s32, 1, &tab->s32, pitch, 1, n, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return hb::check_cuda(e, "halide_b200_camera_pipe_tables", halide_error_code_device_run_failed);
+}

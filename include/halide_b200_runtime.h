@@ -501,6 +501,25 @@ void halide_b200_blur_force_general(int enable);
 void halide_b200_nl_means_variant(int variant);
 /* Device self-test of the fast kernels' arithmetic shortcuts; returns mismatches vs div.rn / cvt, or -1. */
 long long halide_b200_selftest_arith(unsigned long long n, unsigned long long seed);
+/* Device evaluation of one scalar primitive of the float pipelines (hl_math.cuh) over n elements of device arrays,
+ * out[i] = f(a[i] [, b ...]); returns 0 or a negative halide_error_code_t.  fn, with the element types of a, b and out:
+ *   0 halide_exp, 1 halide_log, 2 fast_exp, 3 clamp01        a float, out float
+ *   4 halide_pow(a[i], b[i])                                a, b float, out float
+ *   5 clampf(a[i], b[2i], b[2i+1]), 6 lerpf(a[i], b[2i], b[2i+1])  a float, b float pairs, out float
+ *   7, 8, 9 evaluate_polynomial with 8, 10 and 7 coefficients (halide_exp's, halide_log's, and an odd-count set)
+ *   10 frame_to_f32<uint8_t>                                a uint8, out float
+ *   11 frame_from_f32<uint8_t>                              a float, out uint8
+ *   12 frame_val<uint8_t> (u8 -> u16 value, as float)        a uint8, out float
+ *   13 frame_narrow<uint8_t> (u16 -> u8)                    a uint16, out uint8
+ *   14 pair_u16<uint8_t> (two u8 -> two u16 in one word)    a uint16, out uint32
+ * The CPU oracle's oracle_math_vec takes the same numbers 0 .. 9. */
+int halide_b200_selftest_math(int fn, const void *a, const void *b, void *out, long long n);
+/* camera_pipe's per-call tables for n scalar sets, as its tables kernel computes them: m3200 / m7000 are dense 3x4 float
+ * matrices on the device (x fastest); scalars holds n host records {color_temp, gamma, contrast, sharpen_strength} and
+ * levels n host records {blackLevel, whiteLevel}.  Writes, on the device, matrix[n][12] (int16 Q8.8, x fastest),
+ * curve[n][1024] (uint8) and s32[n] (uint8 sharpen strength x 32).  0 or a negative halide_error_code_t. */
+int halide_b200_camera_pipe_tables(const float *m3200, const float *m7000, const float *scalars, const int32_t *levels, int n,
+                                   int16_t *matrix, uint8_t *curve, uint8_t *s32);
 
 #ifdef __cplusplus
 }

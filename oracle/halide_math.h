@@ -95,13 +95,21 @@ static inline float evaluate_polynomial(float x, const float *coeff, int n) {
     return odd_terms * x + even_terms;
 }
 
+// k = floor(x / ln 2) as an int: NaN -> 0, anything else clamped to [-256, 256] (past the ends the result is +inf or 0
+// either way).  Halide leaves the plain conversion undefined for NaN and values outside int32 (x86 gives INT_MIN, the
+// GPU's cvt.rzi saturates, NaN -> 0) and k + 127 could overflow; hl_math.cuh: exp_k converts the same way.
+static inline int32_t exp_k(float k_real) {
+    if (k_real != k_real) return 0;
+    return (int32_t)clampf(k_real, -256.0f, 256.0f);
+}
+
 static inline float halide_exp(float x_full) {
     const float ln2_part1 = 0.6931457519f;
     const float ln2_part2 = 1.4286067653e-6f;
     const float one_over_ln2 = 1.0f / logf(2.0f);
     float scaled = x_full * one_over_ln2;
     float k_real = floorf(scaled);
-    int32_t k = (int32_t)k_real;
+    int32_t k = exp_k(k_real);
     float x = x_full - k_real * ln2_part1;
     x = x - k_real * ln2_part2;
     static const float coeff[] = {0.00031965933071842413f, 0.00119156835564003744f, 0.00848988645943932717f,
@@ -156,12 +164,12 @@ static inline float fast_exp(float x_full) {
     const float ln2 = logf(2.0f);
     float scaled = div_const(x_full, ln2);
     float k_real = floorf(scaled);
-    int32_t k = (int32_t)k_real;
+    int32_t k = exp_k(k_real);
     float x = x_full - k_real * ln2;
     static const float coeff[] = {0.01314350012789660196f, 0.03668965196652099192f, 0.16873890085469545053f,
                                   0.49970514590562437052f, 1.0f, 1.0f};
     float result = evaluate_polynomial(x, coeff, 6);
-    int32_t biased = clampi(k + 127, 0, 255);
+    int32_t biased = clampi(k, -127, 128) + 127;  // clamp(k + 127, 0, 255)
     float two_to_the_n = as_float((int32_t)((uint32_t)biased << 23));
     return result * two_to_the_n;
 }

@@ -28,13 +28,20 @@ class Field:
         return self.arr[yi[:, None], xi[None, :]]
 
 
+def exp_k(k_real):
+    """floor(x / ln 2) as int32 the way halide_math.h's exp_k converts it: NaN -> 0, everything else clamped to
+    [-256, 256]."""
+    with np.errstate(invalid="ignore"):
+        return np.where(np.isnan(k_real), 0, np.clip(k_real, -256, 256)).astype(np.int32)
+
+
 def halide_exp(x_full):
     x_full = x_full.astype(F)
     ln2_part1, ln2_part2 = F(0.6931457519), F(1.4286067653e-6)
     one_over_ln2 = F(1.0) / np.log(F(2.0), dtype=F)
     scaled = x_full * one_over_ln2
     k_real = np.floor(scaled)
-    k = k_real.astype(np.int32)
+    k = exp_k(k_real)
     x = x_full - k_real * ln2_part1
     x = x - k_real * ln2_part2
     c = [F(v) for v in (0.00031965933071842413, 0.00119156835564003744, 0.00848988645943932717, 0.04160188091348320655,
@@ -277,7 +284,7 @@ def fast_exp(x_full):
     ln2 = np.log(F(2.0), dtype=F)                 # logf(2.0)
     scaled = x_full * F(1.0 / float(ln2))         # x / const -> x * fold(1 / const), folded in double
     k_real = np.floor(scaled)
-    k = k_real.astype(np.int32)
+    k = exp_k(k_real)
     x = x_full - k_real * ln2
     c = [F(v) for v in (0.01314350012789660196, 0.03668965196652099192, 0.16873890085469545053, 0.49970514590562437052, 1.0, 1.0)]
     x2 = x * x

@@ -34,6 +34,8 @@ def _load():
     l.oracle_halide_pow.restype = ctypes.c_float
     l.oracle_halide_pow.argtypes = [ctypes.c_float, ctypes.c_float]
     l.oracle_ll_remap.restype = ctypes.c_float
+    l.oracle_math_vec.restype = ctypes.c_int
+    l.oracle_math_vec.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong]
     l.oracle_ll_remap.argtypes = [ctypes.c_int, ctypes.c_float]
     return l
 
@@ -95,6 +97,31 @@ def local_laplacian(inp, levels, alpha, beta, out_shape=None, in_mins=None, out_
                                      ctypes.c_int(pyramid_levels))
     if r != 0:
         raise RuntimeError(f"oracle_local_laplacian returned {r}")
+    return out
+
+
+# oracle_math_vec's case numbers (the device hook halide_b200_selftest_math uses the same); the three-operand cases take
+# b as (n, 2) pairs: clampf(a, lo, hi) and lerpf(a, one_val, w)
+MATH_FN = {"halide_exp": 0, "halide_log": 1, "fast_exp": 2, "clamp01": 3, "halide_pow": 4, "clampf": 5, "lerpf": 6,
+           "poly8": 7, "poly10": 8, "poly7": 9}
+
+
+def math_vec(fn, a, b=None, out=None):
+    """The oracle's primitive `fn` (a MATH_FN key) element by element over float32 arrays, on all OpenMP threads."""
+    a = np.ascontiguousarray(a, np.float32)
+    if out is None:
+        out = np.empty(a.shape, np.float32)
+    bp = None
+    if b is not None:
+        b = np.ascontiguousarray(b, np.float32)
+        assert b.size == a.size * (2 if MATH_FN[fn] in (5, 6) else 1)
+        bp = b.ctypes.data
+    elif MATH_FN[fn] in (4, 5, 6):
+        raise ValueError(f"{fn} needs a second operand")
+    assert out.dtype == np.float32 and out.shape == a.shape and out.flags.c_contiguous
+    r = lib().oracle_math_vec(MATH_FN[fn], a.ctypes.data, bp, out.ctypes.data, a.size)
+    if r != 0:
+        raise RuntimeError(f"oracle_math_vec returned {r}")
     return out
 
 

@@ -116,3 +116,68 @@ def test_strict_float_switch_builds_and_stays_close():
     assert r == 0
     diff = np.abs(out.astype(np.int64) - want.astype(np.int64))
     assert diff.max() <= 1 and (diff != 0).mean() < 0.02
+
+
+def _math_vec_inputs(n=1 << 15, seed=9):
+    """Random bit patterns of every class, values near the primitives' working ranges, and the specials."""
+    rng = np.random.default_rng(seed)
+    bits = rng.integers(0, 1 << 32, n, dtype=np.uint64).astype(np.uint32).view(np.float32)
+    near = rng.uniform(-120, 120, n).astype(np.float32)
+    specials = np.array([0.0, -0.0, np.inf, -np.inf, np.nan, 1.0, -1.0, 2.0, 0.5, -2.5, 1e-45, 3.4028235e38, 88.72, 1e10,
+                         -1e10, 2.0 ** 31, -(2.0 ** 31)], np.float32)
+    # through float64, as ctypes passes a float to the scalar exports: that quiets signalling NaNs, whose payload
+    # halide_log's bit manipulation would otherwise see
+    with np.errstate(invalid="ignore"):
+        return np.concatenate([bits, near, specials]).astype(np.float64).astype(np.float32)
+
+
+def _same(got, want):
+    return np.array_equal(got.view(np.uint32), want.view(np.uint32)) or \
+        bool(np.all((got.view(np.uint32) == want.view(np.uint32)) | (np.isnan(got) & np.isnan(want))))
+
+
+@pytest.mark.parametrize("fn", ["halide_exp", "halide_log", "fast_exp"])
+def test_math_vec_equals_scalar_exports(oracle, fn):
+    """oracle_math_vec (vectorised, OpenMP) computes what the scalar exports compute, input by input."""
+    a = _math_vec_inputs()
+    got = oracle.math_vec(fn, a)
+    f = getattr(oracle.lib(), f"oracle_{fn}")
+    want = np.array([f(float(v)) for v in a], np.float32)
+    assert _same(got, want)
+
+
+def test_math_vec_pow_equals_scalar_export(oracle):
+    a = _math_vec_inputs(1 << 13, 1)
+    b = _math_vec_inputs(1 << 13, 2)
+    b[: b.size // 2] = np.floor(b[: b.size // 2])  # integer exponents, for negative bases
+    got = oracle.math_vec("halide_pow", a, b)
+    want = np.array([oracle.lib().oracle_halide_pow(float(x), float(y)) for x, y in zip(a, b)], np.float32)
+    assert _same(got, want)
+
+
+def test_math_vec_clamp_lerp_poly_restated(oracle):
+    """The vector export's clamp, lerp and polynomial cases against their float32 expressions restated in numpy (select-based
+    min / max, no contraction)."""
+    a = _math_vec_inputs()
+    rng = np.random.default_rng(4)
+    b = np.stack([rng.permutation(a), rng.permutation(a)], axis=1).astype(np.float32)
+    f = np.float32
+    with np.errstate(all="ignore"):
+        m = np.where(a < f(1), a, f(1))
+        assert _same(oracle.math_vec("clamp01", a), np.where(m > f(0), m, f(0)))
+        m = np.where(a < b[:, 1], a, b[:, 1])
+        assert _same(oracle.math_vec("clampf", a, b), np.where(m > b[:, 0], m, b[:, 0]))
+        assert _same(oracle.math_vec("lerpf", a, b), a * (f(1) - b[:, 1]) + b[:, 0] * b[:, 1])
+        for fn, coeff in (("poly7", [0.25, -0.5, 0.0, 1.5, -2.0, 0.125, 3.0]),):
+            c = np.array(coeff, np.float32)
+            x2 = a * a
+            even, odd = np.full_like(a, c[0]), np.full_like(a, c[1])
+            for i in range(2, c.size):
+                if i % 2 == 0:
+                    even = even * x2 if c[i] == 0 else even * x2 + c[i]
+                else:
+                    odd = odd * x2 if c[i] == 0 else odd * x2 + c[i]
+            want = even * a + odd if c.size % 2 == 0 else odd * a + even
+            assert _same(oracle.math_vec(fn, a), want)
+    with pytest.raises(ValueError):
+        oracle.math_vec("halide_pow", a)

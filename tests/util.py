@@ -81,9 +81,11 @@ def nl_means_variant(hb, v):
 
 # ---- camera_pipe ---------------------------------------------------------------------------------------------------
 # The harness's colour matrices (apps/camera_pipe/process.cpp:43-49), its scalar arguments, and each scalar at the
-# extremes the filter accepts, one at a time.  Left out everywhere: gamma = 0 and non-finite scalars.  1 / 0 = inf makes
-# halide_pow compute log(1) * inf = NaN and convert floor(NaN) to int, which Halide leaves undefined (the GPU gives 0,
-# x86 INT_MIN), so the oracle and the kernel may both be right and still disagree.
+# extremes the filter accepts, one at a time.  Left out: a zero or non-finite color_temp, whose matrix entries convert inf
+# or NaN to int16, which Halide leaves undefined (the GPU saturates, x86 gives INT_MIN), so the oracle and the kernel may
+# both be right and still disagree.  Zero and non-finite gamma, contrast and sharpen_strength are defined in both copies
+# (halide_exp's exponent goes through exp_k, NaN -> 0 and clamped) and test_hl_math_gpu.py checks their tables bit for
+# bit; they stay out of this list because the float64 formulas of test_camera_pipe_tables.py mean nothing there.
 CP_M3200 = np.array([[1.6697, -0.2693, -0.4004, -42.4346], [-0.3576, 1.0615, 1.5949, -37.1158],
                      [-0.2175, -1.8751, 6.9640, -26.6970]], np.float32)
 CP_M7000 = np.array([[2.2997, -0.4478, 0.1706, -39.0923], [-0.3826, 1.5906, -0.2080, -25.4311],
