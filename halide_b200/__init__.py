@@ -16,5 +16,6 @@ from . import nl_means_video  # noqa: F401  (batch and interleaved nl_means)
 from . import bilateral_grid_video  # noqa: F401  (batch bilateral_grid)
 from . import blur_video  # noqa: F401  (batch halide_blur)
 from . import stencil_chain_video  # noqa: F401  (batch stencil_chain)
+from . import local_laplacian_depth  # noqa: F401  (local_laplacian at any pyramid depth on batch / 8-bit / interleaved frames)
 from .pipeline import FramePipeline  # noqa: F401
 from . import image_io  # noqa: F401  (host-side: file formats + the reference's type-conversion rules)

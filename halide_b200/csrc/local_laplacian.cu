@@ -43,9 +43,10 @@ template<typename T>
 struct PlanT {
     LLFrameT<T> f;
     LevelSetDeep ls{};  // levels 1 .. J-1 (level 0 is never stored: its slot stays zero)
-    int J = ll::kMaxJ;  // pyramid levels (8 but for halide_b200_local_laplacian_pyramid_levels, whose frames have N == 1)
+    int J = ll::kMaxJ;  // pyramid levels (8 but for the pyramid_levels entry points)
     int N;  // frames (1 but for a batch)
-    FrameStrides fs;  // all zero when N == 1 (but the pixel pitches)
+    FrameStrides fs;  // all zero when N == 1 (but the pixel pitches); level slots: levels 0 .. 7
+    LevelStridesDeep deep{};  // the level strides of every level (all zero when N == 1): those of levels past 7 live only here
     float alpha;
     bool il = false;  // interleaved frames (the kernels' IL instantiations)
 };
@@ -252,7 +253,10 @@ int alloc_levels(P &p, const ll::Geom &geom, hb::Scratch &scratch) {
         b.gp = scratch.get<float>((size_t)gp_sn * p.N);
         b.ing = scratch.get<float>((size_t)ing_sn * p.N);
         b.outg = with_outg ? scratch.get<float>((size_t)outg_sn * p.N) : nullptr;
-        if (p.N > 1) p.fs.gp[j] = gp_sn, p.fs.ing[j] = ing_sn, p.fs.outg[j] = outg_sn;  // (N > 1: J == 8)
+        if (p.N > 1) {
+            p.deep.gp[j] = gp_sn, p.deep.ing[j] = ing_sn, p.deep.outg[j] = outg_sn;
+            if (j < ll::kMaxJ) p.fs.gp[j] = gp_sn, p.fs.ing[j] = ing_sn, p.fs.outg[j] = outg_sn;
+        }
         if (!b.gp || !b.ing || (with_outg && !b.outg)) {
             return hb::fail(halide_error_code_device_malloc_failed, "local_laplacian: scratch allocation failed");
         }
@@ -331,12 +335,23 @@ void launch_level12(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2, cudaS
     else launch_level12_il<false>(p, f, cy1, cy2, s);
 }
 
-// Index of level j's entries in FrameStrides, whose arrays have ll::kMaxJ slots (a kernel reads those of j - 1 .. j + 1).
-// A batch has J == 8: j itself.  A deeper pyramid (J > 8) is a single frame, whose level strides are all zero: its
-// levels from 7 on, whose neighbours could reach slot 8, take slot 6 (neighbours 5 .. 7) — every read stays inside the
-// arrays and still sees a zero stride.
+// The strides a launch that produces level j reads, and the index that stands for level j in them (*js).  FrameStrides'
+// level arrays have ll::kMaxJ slots, and such a launch reads those of levels j - 1 .. j + 1: up to J == 8 the plan's own
+// strides at j itself.  In a deeper pyramid the levels from 7 on, whose neighbours could reach slot 8, get a copy whose
+// slots 5 .. 7 hold the strides of levels j - 1 .. j + 1 and j is slot 6 (a single frame's are all zero, as the copy's).
 template<typename P>
-int fs_slot(const P &p, int j) { return p.J <= ll::kMaxJ ? j : std::min(j, ll::kMaxJ - 2); }
+FrameStrides level_strides(const P &p, int j, int *js) {
+    *js = p.J <= ll::kMaxJ ? j : std::min(j, ll::kMaxJ - 2);
+    if (*js == j) return p.fs;
+    FrameStrides w = p.fs;
+    for (int k = 0; k < 3; k++) {
+        const int lv = j - 1 + k;  // (level J, the top's neighbour above, does not exist: stride 0)
+        w.gp[*js - 1 + k] = lv < p.J ? p.deep.gp[lv] : 0;
+        w.ing[*js - 1 + k] = lv < p.J ? p.deep.ing[lv] : 0;
+        w.outg[*js - 1 + k] = lv < p.J ? p.deep.outg[lv] : 0;
+    }
+    return w;
+}
 
 template<typename T>
 void launch_down(PlanT<T> &p, int j, cudaStream_t s) {  // produce level j (j >= 1) rows cy
@@ -352,7 +367,9 @@ void launch_down(PlanT<T> &p, int j, cudaStream_t s) {  // produce level j (j >=
             const int slots = hb::resident_blocks(kern, 256, 0);
             long long g = (tasks + 7) / 8;
             if (g > slots) g = slots;
-            HB_LAUNCH("ll_down_rows", kern, (int)g, 256, 0, s, lb[j - 1], lb[j], ns, ng, p.N, fs_slot(p, j), p.fs);
+            int js;
+            const FrameStrides fs = level_strides(p, j, &js);
+            HB_LAUNCH("ll_down_rows", kern, (int)g, 256, 0, s, lb[j - 1], lb[j], ns, ng, p.N, js, fs);
         }
     } else if (lb[j].cy.n() <= 0) {
         return;
@@ -364,12 +381,13 @@ void launch_down(PlanT<T> &p, int j, cudaStream_t s) {  // produce level j (j >=
                       p.fs);
         });
     } else {
-        const int js = fs_slot(p, j);
+        int js;
+        const FrameStrides fs = level_strides(p, j, &js);
         for_frame_groups(p, [&](int n0, int nf) {
             dim3 g = grid_for(lb[j].sx.n(), lb[j].cy.n());
             g.z = nf;
-            HB_LAUNCH("ll_down", ll_down_naive_kernel, g, kBlk, 0, s, at_frame(lb[j - 1], js - 1, p.fs, n0), at_frame(lb[j], js, p.fs, n0), p.f.levels, js,
-                      p.fs);
+            HB_LAUNCH("ll_down", ll_down_naive_kernel, g, kBlk, 0, s, at_frame(lb[j - 1], js - 1, fs, n0), at_frame(lb[j], js, fs, n0), p.f.levels, js,
+                      fs);
         });
     }
 }
@@ -384,19 +402,20 @@ void launch_up(P &p, int j, cudaStream_t s) {  // produce outGPyramid[j] (1 <= j
     if (lb[j].coy.n() <= 0) return;
     const bool fast_up = p.f.levels == 8 && !(g_force_naive & 2);
     const bool top = j == p.J - 1;
-    const int js = fs_slot(p, j);
+    int js;
+    const FrameStrides fs = level_strides(p, j, &js);
     for_frame_groups(p, [&](int n0, int nf) {
         if (fast_up && !top) {
             static const CUtensorMap no_map = {};
             HB_LAUNCH("ll_up2", (nf > 1 ? ll_up2_kernel<false, false, true, false, true> : ll_up2_kernel<false, false, true, false, false>), up_grid(lb[j].ox.lo, lb[j].ox.hi, lb[j].coy.lo, lb[j].coy.hi, nf),
-                      256, up2_smem_bytes(false, false), s, scalars_frame(at_frame(p.f, p.fs, n0)), at_frame(lb[j], js, p.fs, n0),
-                      at_frame(lb[j + 1], js + 1, p.fs, n0), no_map, js, p.fs);
+                      256, up2_smem_bytes(false, false), s, scalars_frame(at_frame(p.f, fs, n0)), at_frame(lb[j], js, fs, n0),
+                      at_frame(lb[j + 1], js + 1, fs, n0), no_map, js, fs);
         } else {
             dim3 g = grid_for(lb[j].ox.n(), lb[j].coy.n());
             g.z = nf;
             const int jc = top ? j : j + 1;
-            HB_LAUNCH("ll_up", ll_up_naive_kernel, g, kBlk, 0, s, at_frame(lb[j], js, p.fs, n0), at_frame(lb[jc], top ? js : js + 1, p.fs, n0),
-                      p.f.flm1, p.f.levels, top ? 1 : 0, js, p.fs);
+            HB_LAUNCH("ll_up", ll_up_naive_kernel, g, kBlk, 0, s, at_frame(lb[j], js, fs, n0), at_frame(lb[jc], top ? js : js + 1, fs, n0),
+                      p.f.flm1, p.f.levels, top ? 1 : 0, js, fs);
         }
     });
 }
@@ -500,16 +519,19 @@ void launch_final(PlanT<T> &p, cudaStream_t s) {
 template<typename P>
 bool launch_coarse_fused(P &p, int j0, cudaStream_t s) {
     if (!hb::cooperative_launch()) return false;
-    // J <= 8: the LevelSet instantiations, on the first 8 slots; a deeper pyramid (one frame) takes all of LevelSetDeep
+    // J <= 8: the LevelSet instantiations, on the first 8 slots; a deeper pyramid takes all of LevelSetDeep, and a deeper
+    // batch the strides of every level too
     LevelSet ls8;
     memcpy(ls8.lv, p.ls.lv, sizeof ls8.lv);
-    const bool deep = p.J > ll::kMaxJ;
-    const void *kern = deep ? (const void *)ll_coarse_fused_kernel<false, LevelSetDeep>
-                            : (p.N > 1 ? (const void *)ll_coarse_fused_kernel<true> : (const void *)ll_coarse_fused_kernel<false>);
+    const bool deep = p.J > ll::kMaxJ, frames = p.N > 1;
+    const void *kern = deep ? (frames ? (const void *)ll_coarse_fused_kernel<true, LevelSetDeep, LevelStridesDeep>
+                                      : (const void *)ll_coarse_fused_kernel<false, LevelSetDeep>)
+                            : (frames ? (const void *)ll_coarse_fused_kernel<true> : (const void *)ll_coarse_fused_kernel<false>);
     const int max_blocks = std::min(hb::resident_blocks(kern, 256, 0), 2 * hb::sm_count());
     int J = p.J, K = p.f.levels, levels = p.f.levels, jd = fast_down(p) && j0 < 2 ? 2 : j0, nf = p.N;
     float flm1 = p.f.flm1;
-    void *args[] = {deep ? (void *)&p.ls : (void *)&ls8, &J, &j0, &jd, &K, &flm1, &levels, &nf, &p.fs};
+    void *args[] = {deep ? (void *)&p.ls : (void *)&ls8, &J, &j0, &jd, &K, &flm1, &levels, &nf,
+                    deep && frames ? (void *)&p.deep : (void *)&p.fs};
     hb::count_launch("ll_coarse_fused", s);
     cudaError_t e = cudaLaunchCooperativeKernel((void *)kern, dim3(max_blocks), dim3(256), args, 0, s);
     hb::after_launch(s);
@@ -551,25 +573,71 @@ void run_coarse_sweep(P &p, int from_level, cudaStream_t s) {
     for (int j = j0; j > from_level && j >= first_up_level(p); j--) launch_up(p, j, s);
 }
 
-// J = 1: the whole filter is the pointwise tone kernel over the output region (ll_tone_kernel).  Its aligned form needs
-// every plane row it reads and writes to start on 16 bytes at the output's first column.
-void launch_tone(Plan &p, cudaStream_t s) {
-    const LLFrame &f = p.f;
+// J = 1: the whole filter is the pointwise tone kernel over the output region (ll_tone_kernel), one launch per group of
+// frames.  Its aligned forms move a unit of kTonePx pixels as whole words, so every byte offset from a unit's first
+// sample to another's (rows, planes, frames) and the first unit's address are multiples of the word size: planar frames,
+// one word per plane row of kTonePx samples (16 bytes of uint16, 8 of uint8); interleaved RGB / RGBA frames of channels
+// [0, 3), the unit's run of 8 * pitch samples (16-byte words, 8-byte ones for uint8 RGB), and for an RGBA output the word
+// of a pixel's R and G (an RGBA input must describe its fourth channel: the run covers whole pixels).
+template<typename T>
+void launch_tone(PlanT<T> &p, cudaStream_t s) {
+    const LLFrameT<T> &f = p.f;
     const int upr = (f.W + kTonePx - 1) / kTonePx;
     const long long units = (long long)upr * f.H;
-    auto a16 = [](int64_t bytes) { return (bytes & 15) == 0; };
-    const uint16_t *in0 = f.in + (int64_t)(f.out_y0 - f.in_y0) * f.in_sy + (f.out_x0 - f.in_x0);
-    const bool vec = a16((int64_t)(uintptr_t)in0) && a16(f.in_sy * 2) && a16(f.in_sc * 2) && a16((int64_t)(uintptr_t)f.out) &&
-                     a16(f.out_sy * 2) && a16(f.out_sc * 2) && !(g_force_naive & 16);
+    const int pin = p.fs.px_in, pout = p.fs.px_out;
+    const int64_t eb = sizeof(T);
+    auto al = [](int64_t bytes, int64_t a) { return bytes % a == 0; };
+    const T *in0 = f.in + (int64_t)(f.out_y0 - f.in_y0) * f.in_sy + (int64_t)(f.out_x0 - f.in_x0) * pin;
+    const int64_t in_b = (int64_t)(uintptr_t)in0, out_b = (int64_t)(uintptr_t)f.out;
+    const int64_t a = kTonePx * eb;
+    const bool vec = !p.il && al(in_b, a) && al(f.in_sy * eb, a) && al(f.in_sc * eb, a) && al(p.fs.in * eb, a) && al(out_b, a) &&
+                     al(f.out_sy * eb, a) && al(f.out_sc * eb, a) && al(p.fs.out * eb, a) && !(g_force_naive & 16);
+    auto run_word = [&](int pitch) -> int64_t { return kTonePx * pitch * eb % 16 == 0 ? 16 : 8; };
+    const int64_t ai = run_word(pin), ao = pout == 3 ? run_word(3) : 2 * eb;
+    const bool il_vec = p.il && f.C == 3 && f.in_c0 == 0 && f.out_c0 == 0 && f.in_c == pin &&
+                        ((pin == 3 && pout == 3) || (pin == 4 && (pout == 3 || pout == 4))) && al(in_b, ai) && al(f.in_sy * eb, ai) &&
+                        al(p.fs.in * eb, ai) && al(out_b, ao) && al(f.out_sy * eb, ao) && al(p.fs.out * eb, ao) && !(g_force_naive & 16);
     const size_t smem = (size_t)(2 * f.lut_half + 1) * sizeof(float);
-    auto kern = vec ? ll_tone_kernel<true> : ll_tone_kernel<false>;
-    const int slots = hb::resident_blocks(kern, 256, smem);  // (smem is above 48 KB for levels > 24)
-    const int g = (int)std::min<long long>(slots, (units + 255) / 256);
-    HB_LAUNCH("ll_tone", kern, g, 256, smem, s, f, upr, units);
+    // the planar uint16 single-frame form: units counted in 64 bits, one launch
+    auto launch1 = [&](auto kern) {
+        const int slots = hb::resident_blocks(kern, 256, smem);  // (smem is above 48 KB for levels > 24)
+        const int g = (int)std::min<long long>(slots, (units + 255) / 256);
+        HB_LAUNCH("ll_tone", kern, g, 256, smem, s, f, upr, units, p.fs);
+    };
+    // the others: frame blockIdx.z of each group, the resident blocks shared out over the group's frames; their unit index
+    // is 32-bit, so a frame of 2^31 units or more runs in bands of rows
+    auto launch = [&](auto kern) {
+        const int slots = hb::resident_blocks(kern, 256, smem);
+        const int band = (int)std::min<long long>(f.H, INT32_MAX / upr);
+        for_frame_groups(p, [&](int n0, int nf) {
+            for (int y0 = 0; y0 < f.H; y0 += band) {
+                LLFrameT<T> fb = at_frame(f, p.fs, n0);
+                fb.out += (int64_t)y0 * f.out_sy;
+                fb.out_y0 += y0;
+                fb.H = std::min(band, f.H - y0);
+                const long long bu = (long long)upr * fb.H;
+                const dim3 g((unsigned)std::max<long long>(1, std::min<long long>((bu + 255) / 256, (slots + nf - 1) / nf)), 1, nf);
+                HB_LAUNCH("ll_tone", kern, g, 256, smem, s, fb, upr, bu, p.fs);
+            }
+        });
+    };
+    if constexpr (std::is_same<T, uint16_t>::value) {
+        if (!p.il && p.N == 1) {
+            if (vec) launch1(ll_tone_kernel<true>);
+            else launch1(ll_tone_kernel<false>);
+            return;
+        }
+    }
+    if (il_vec && pin == 3) launch(ll_tone_kernel<true, T, 3, 3, true>);
+    else if (il_vec && pout == 3) launch(ll_tone_kernel<true, T, 4, 3, true>);
+    else if (il_vec) launch(ll_tone_kernel<true, T, 4, 4, true>);
+    else if (p.il) launch(ll_tone_kernel<false, T, 0, 0, true>);
+    else if (vec) launch(ll_tone_kernel<true, T, 1, 1, true>);
+    else launch(ll_tone_kernel<false, T, 1, 1, true>);
 }
 
 // One GPU, args = {input, output} of 3 dimensions (one frame) or 4 (a batch of frames along dimension 3), elements T;
-// J = pyramid levels (8 but for halide_b200_local_laplacian_pyramid_levels: uint16, one frame).
+// J = pyramid levels (8 but for the pyramid_levels entry points).
 template<typename T>
 int run_local_laplacian(hb::Arg *args, int levels, float alpha, float beta, int J, const char *what) {
     int r;
@@ -591,10 +659,9 @@ int run_local_laplacian(hb::Arg *args, int levels, float alpha, float beta, int 
     if ((r = get_lut(p, s, lut))) return r;
     {
         hb::CallTimer timer(s);
-        if constexpr (std::is_same<T, uint16_t>::value) {
-            if (J == 1) launch_tone(p, s);
-        }
-        if (J > 1) {
+        if (J == 1) {
+            launch_tone(p, s);
+        } else {
             run_coarse_sweep(p, 0, s);
             launch_final(p, s);
         }
@@ -664,6 +731,49 @@ extern "C" int halide_b200_local_laplacian_pyramid_levels(halide_buffer_t *input
                                                           float beta, halide_buffer_t *output) {
     hb::Arg args[2] = {{input, kArgs[0]}, {output, kArgs[4]}};
     return run_local_laplacian<uint16_t>(args, levels, alpha, beta, pyramid_levels, "local_laplacian_pyramid_levels launch");
+}
+
+// halide_b200_local_laplacian_pyramid_levels on the buffers of the batch, 8-bit and interleaved entry points above: each
+// is its fixed-depth counterpart with J chosen per call (J = 8: the same launches), and on every frame bit for bit what
+// halide_b200_local_laplacian_pyramid_levels gives on a planar uint16 copy (converted as the 8-bit entry points convert).
+extern "C" int halide_b200_local_laplacian_pyramid_levels_batch(halide_buffer_t *input, int32_t pyramid_levels, int32_t levels, float alpha,
+                                                                float beta, halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kBatchArgs[0]}, {output, kBatchArgs[1]}};
+    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, pyramid_levels, "local_laplacian_pyramid_levels_batch launch");
+}
+extern "C" int halide_b200_local_laplacian_pyramid_levels_u8(halide_buffer_t *input, int32_t pyramid_levels, int32_t levels, float alpha,
+                                                             float beta, halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kU8Args[0]}, {output, kU8Args[1]}};
+    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, pyramid_levels, "local_laplacian_pyramid_levels_u8 launch");
+}
+extern "C" int halide_b200_local_laplacian_pyramid_levels_u8_batch(halide_buffer_t *input, int32_t pyramid_levels, int32_t levels,
+                                                                   float alpha, float beta, halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kU8BatchArgs[0]}, {output, kU8BatchArgs[1]}};
+    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, pyramid_levels, "local_laplacian_pyramid_levels_u8_batch launch");
+}
+extern "C" int halide_b200_local_laplacian_pyramid_levels_interleaved(halide_buffer_t *input, int32_t pyramid_levels, int32_t levels,
+                                                                      float alpha, float beta, halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kArgs[0], nullptr, true}, {output, kArgs[4], nullptr, true}};
+    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, pyramid_levels, "local_laplacian_pyramid_levels_interleaved launch");
+}
+extern "C" int halide_b200_local_laplacian_pyramid_levels_interleaved_batch(halide_buffer_t *input, int32_t pyramid_levels,
+                                                                            int32_t levels, float alpha, float beta,
+                                                                            halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kBatchArgs[0], nullptr, true}, {output, kBatchArgs[1], nullptr, true}};
+    return run_local_laplacian<uint16_t>(args, levels, alpha, beta, pyramid_levels,
+                                         "local_laplacian_pyramid_levels_interleaved_batch launch");
+}
+extern "C" int halide_b200_local_laplacian_pyramid_levels_u8_interleaved(halide_buffer_t *input, int32_t pyramid_levels, int32_t levels,
+                                                                         float alpha, float beta, halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kU8Args[0], nullptr, true}, {output, kU8Args[1], nullptr, true}};
+    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, pyramid_levels, "local_laplacian_pyramid_levels_u8_interleaved launch");
+}
+extern "C" int halide_b200_local_laplacian_pyramid_levels_u8_interleaved_batch(halide_buffer_t *input, int32_t pyramid_levels,
+                                                                               int32_t levels, float alpha, float beta,
+                                                                               halide_buffer_t *output) {
+    hb::Arg args[2] = {{input, kU8BatchArgs[0], nullptr, true}, {output, kU8BatchArgs[1], nullptr, true}};
+    return run_local_laplacian<uint8_t>(args, levels, alpha, beta, pyramid_levels,
+                                        "local_laplacian_pyramid_levels_u8_interleaved_batch launch");
 }
 
 namespace {

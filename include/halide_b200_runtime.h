@@ -323,6 +323,29 @@ int halide_b200_local_laplacian_u8_interleaved(struct halide_buffer_t *input, in
 int halide_b200_local_laplacian_u8_interleaved_batch(struct halide_buffer_t *input, int32_t levels, float alpha, float beta,
                                                      struct halide_buffer_t *output);
 
+/* The seven entry points above (batch, 8-bit and interleaved, in every combination) with the pyramid_levels J of
+ * halide_b200_local_laplacian_pyramid_levels (below) as an argument, 1 <= J <= 20.  Buffers, layout rules, error codes
+ * and the bounds query are those of the fixed-depth entry point of the same suffix, and J is checked as
+ * halide_b200_local_laplacian_pyramid_levels checks it.  Frame n of the output is, bit for bit,
+ * halide_b200_local_laplacian_pyramid_levels(J) on a planar uint16 copy of input frame n (8-bit frames converted as
+ * halide_b200_local_laplacian_u8 converts them); at J == 8 each is its fixed-depth counterpart, with the same launches. */
+int halide_b200_local_laplacian_pyramid_levels_batch(struct halide_buffer_t *input, int32_t pyramid_levels, int32_t levels,
+                                                     float alpha, float beta, struct halide_buffer_t *output);
+int halide_b200_local_laplacian_pyramid_levels_u8(struct halide_buffer_t *input, int32_t pyramid_levels, int32_t levels, float alpha,
+                                                  float beta, struct halide_buffer_t *output);
+int halide_b200_local_laplacian_pyramid_levels_u8_batch(struct halide_buffer_t *input, int32_t pyramid_levels, int32_t levels,
+                                                        float alpha, float beta, struct halide_buffer_t *output);
+int halide_b200_local_laplacian_pyramid_levels_interleaved(struct halide_buffer_t *input, int32_t pyramid_levels, int32_t levels,
+                                                           float alpha, float beta, struct halide_buffer_t *output);
+int halide_b200_local_laplacian_pyramid_levels_interleaved_batch(struct halide_buffer_t *input, int32_t pyramid_levels,
+                                                                 int32_t levels, float alpha, float beta,
+                                                                 struct halide_buffer_t *output);
+int halide_b200_local_laplacian_pyramid_levels_u8_interleaved(struct halide_buffer_t *input, int32_t pyramid_levels, int32_t levels,
+                                                              float alpha, float beta, struct halide_buffer_t *output);
+int halide_b200_local_laplacian_pyramid_levels_u8_interleaved_batch(struct halide_buffer_t *input, int32_t pyramid_levels,
+                                                                    int32_t levels, float alpha, float beta,
+                                                                    struct halide_buffer_t *output);
+
 /* camera_pipe on raw bursts and into pixel-interleaved RGB.  Matrices and scalars are camera_pipe's, in the same order,
  * and shared by every frame; the tables they give are computed once per call, and every frame runs in one launch.
  *   halide_b200_camera_pipe_batch:             input uint16 (x, y, n), processed uint8 (x, y, c, n), planar;

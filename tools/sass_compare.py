@@ -9,7 +9,9 @@ Kernels are matched by demangled name.  A template parameter that a change appen
 mangled name of every existing instantiation without changing its code, so the new object's names are also tried with
 such trailing defaults removed, one after another: the interleaved-layout parameters `bool IL = false` (ll_level1_kernel;
 nl_means_kernel and nl_means_window_kernel, with the frame-walk parameter `bool FR = false` after it),
-`int PI = 1, int PO = 1` (ll_up2_kernel) and the level set type `typename LS = LevelSet` (ll_coarse_fused_kernel).  A kernel that gained the frame element type as its
+`int PI = 1, int PO = 1` (ll_up2_kernel), the level set type `typename LS = LevelSet` and after it the stride set type
+`typename FS = FrameStrides` (ll_coarse_fused_kernel), and ll_tone_kernel's `typename T = uint16_t, int PI = 1, int PO = 1,
+bool FRAMES = false` (its element type, `unsigned short`, is trailing once the others are stripped).  A kernel that gained the frame element type as its
 first template parameter is also tried without it when that type is float: `f<float>(` as the plain function `f(` (the
 demangled name of a template instance also carries its return type, `void `), `f<float, 3, 7>(` as `f<3, 7>(`
 (bg_hist_blurz_kernel, bg_slice_kernel, nl_means_kernel, nl_means_window_kernel; the bilateral_grid kernels also gained
@@ -29,7 +31,7 @@ import sys
 
 CUOBJDUMP = "/usr/local/cuda/bin/cuobjdump"
 # trailing template arguments that stand for the defaults of appended parameters
-DEFAULT_TAILS = [", 1, 1>(", ", false>(", ", llk::LevelSet>("]
+DEFAULT_TAILS = [", 1, 1>(", ", false>(", ", llk::LevelSet>(", ", llk::FrameStrides>(", ", unsigned short>("]
 # a leading element type parameter: its float instance against the kernel before it had the parameter; and a plain
 # kernel's one appended `bool = false`
 HEADS = [(re.compile(r"^void (.*)<float>\("), r"\1("), (re.compile(r"<float, "), "<"), (re.compile(r"^void (.*)<false>\("), r"\1(")]
