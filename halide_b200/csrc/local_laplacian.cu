@@ -266,7 +266,34 @@ int alloc_levels(P &p, const ll::Geom &geom, hb::Scratch &scratch) {
 
 // ---- launch helpers ------------------------------------------------------------------------------------
 const dim3 kBlk(32, 8);
-dim3 grid_for(int w, int h) { return dim3((w + 31) / 32, (h + 7) / 8); }
+dim3 grid_for(int w, int h, int nf) { return dim3((w + 31) / 32, (h + 7) / 8, nf); }  // z = frames
+
+// Returns f(std::bool_constant<b>{}...) for the run-time flags b...: each becomes a template argument of the kernel f picks.
+template<typename F>
+auto with_flags(F &&f) { return f(); }
+template<typename F, typename... B>
+auto with_flags(F &&f, bool b, B... bs) {
+    if (b) return with_flags([&](auto... c) { return f(std::true_type{}, c...); }, bs...);
+    return with_flags([&](auto... c) { return f(std::false_type{}, c...); }, bs...);
+}
+
+// Whether each address, and each offset or stride in bytes, is a multiple of n bytes.
+template<typename... B>
+bool multiples_of(int64_t n, B... bytes) { return (((int64_t)(uintptr_t)bytes % n == 0) && ...); }
+
+// The layouts the final and tone kernels have forms for: any planar or interleaved frame (General, GeneralIL), aligned
+// planar words (Aligned; AlignedTma: with the final kernel's frame tile by TMA) and the frames il_form names.
+enum class Form { General, GeneralIL, Aligned, AlignedTma, Rgb, RgbaToRgb, Rgba };
+
+// An interleaved frame's aligned form, if its layout has one: channels [0, 3) of RGB -> RGB, RGBA -> RGB and RGBA -> RGBA
+// frames, where an RGBA input must describe its fourth channel (the aligned forms read whole pixels).
+template<typename T>
+Form il_form(const PlanT<T> &p) {
+    const int pin = p.fs.px_in, pout = p.fs.px_out;
+    const bool rgb = p.f.C == 3 && p.f.in_c0 == 0 && p.f.out_c0 == 0 && p.f.in_c == pin &&
+                     ((pin == 3 && pout == 3) || (pin == 4 && (pout == 3 || pout == 4)));
+    return !rgb ? Form::GeneralIL : pin == 3 ? Form::Rgb : pout == 3 ? Form::RgbaToRgb : Form::Rgba;
+}
 
 // Levels 1 and 2 from the frame (K == 8): stores level-1 rows cy1 and level-2 rows cy2, reading the frame through f
 // (the row-sharded path narrows both spans, and hides the halo rows from the launch that runs before they arrive).
@@ -310,9 +337,7 @@ void launch_level12_kernel(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2
     // aligned 4-byte words (a column pair of uint16, the pairs of two lanes of uint8): every byte offset between the
     // frame's first element and a staged word is a multiple of 4; 32-bit element offsets from the frame's first element
     const int64_t eb = sizeof(T);
-    auto w4 = [](int64_t bytes) { return (bytes & 3) == 0; };
-    const int wide = w4((int64_t)(uintptr_t)f.in) && w4(f.in_sy * eb) && w4(f.in_sc * eb) && w4(p.fs.in * eb) && w4(f.in_x0 * eb) &&
-                     w4((int64_t)(uintptr_t)f.halo_top) && w4((int64_t)(uintptr_t)f.halo_bot) && w4(f.halo_pitch * eb);
+    const int wide = multiples_of(4, f.in, f.in_sy * eb, f.in_sc * eb, p.fs.in * eb, f.in_x0 * eb, f.halo_top, f.halo_bot, f.halo_pitch * eb);
     // (an interleaved frame's columns are px_in elements apart: its last sample is up to in_w * px_in further)
     const int idx32 = f.in_sy > 0 && f.in_sc > 0 &&
                       (int64_t)f.in_h * f.in_sy + (int64_t)f.in_c * f.in_sc + (IL ? (int64_t)f.in_w * p.fs.px_in : 0) < (1ll << 31);
@@ -320,19 +345,10 @@ void launch_level12_kernel(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2
               p.N, p.fs);
 }
 
-template<bool IL, typename T>
-void launch_level12_il(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2, cudaStream_t s) {
-    const bool beta1 = p.f.beta == 1.0f, frames = p.N > 1;
-    if (beta1 && frames) launch_level12_kernel<true, true, IL>(p, f, cy1, cy2, s);
-    else if (beta1) launch_level12_kernel<true, false, IL>(p, f, cy1, cy2, s);
-    else if (frames) launch_level12_kernel<false, true, IL>(p, f, cy1, cy2, s);
-    else launch_level12_kernel<false, false, IL>(p, f, cy1, cy2, s);
-}
-
 template<typename T>
 void launch_level12(PlanT<T> &p, const LLFrameT<T> &f, Span cy1, Span cy2, cudaStream_t s) {
-    if (p.il) launch_level12_il<true>(p, f, cy1, cy2, s);
-    else launch_level12_il<false>(p, f, cy1, cy2, s);
+    with_flags([&](auto beta1, auto frames, auto il) { launch_level12_kernel<beta1, frames, il>(p, f, cy1, cy2, s); },
+               p.f.beta == 1.0f, p.N > 1, p.il);
 }
 
 // The strides a launch that produces level j reads, and the index that stands for level j in them (*js).  FrameStrides'
@@ -363,31 +379,25 @@ void launch_down(PlanT<T> &p, int j, cudaStream_t s) {  // produce level j (j >=
             // stored levels: load-bound row-group kernel
             const int ns = (lb[j].sx.n() + kRCols - 1) / kRCols, ng = (lb[j].cy.n() + kRG - 1) / kRG;
             const long long tasks = (long long)ns * ng * 5 * p.N;
-            auto kern = p.N > 1 ? ll_down_rows_kernel<true> : ll_down_rows_kernel<false>;
-            const int slots = hb::resident_blocks(kern, 256, 0);
-            long long g = (tasks + 7) / 8;
-            if (g > slots) g = slots;
             int js;
             const FrameStrides fs = level_strides(p, j, &js);
-            HB_LAUNCH("ll_down_rows", kern, (int)g, 256, 0, s, lb[j - 1], lb[j], ns, ng, p.N, js, fs);
+            const auto kern = with_flags([](auto frames) { return ll_down_rows_kernel<frames>; }, p.N > 1);
+            const int slots = hb::resident_blocks(kern, 256, 0);
+            HB_LAUNCH("ll_down_rows", kern, (int)std::min<long long>(slots, (tasks + 7) / 8), 256, 0, s, lb[j - 1], lb[j], ns, ng, p.N, js, fs);
         }
     } else if (lb[j].cy.n() <= 0) {
         return;
     } else if (j == 1) {
         for_frame_groups(p, [&](int n0, int nf) {
-            dim3 g = grid_for(lb[1].sx.n(), lb[1].cy.n());
-            g.z = nf;
-            HB_LAUNCH("ll_level1_generic", ll_level1_naive_kernel<T>, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0),
-                      p.fs);
+            HB_LAUNCH("ll_level1_generic", ll_level1_naive_kernel<T>, grid_for(lb[1].sx.n(), lb[1].cy.n(), nf), kBlk, 0, s, at_frame(p.f, p.fs, n0),
+                      at_frame(lb[1], 1, p.fs, n0), p.fs);
         });
     } else {
         int js;
         const FrameStrides fs = level_strides(p, j, &js);
         for_frame_groups(p, [&](int n0, int nf) {
-            dim3 g = grid_for(lb[j].sx.n(), lb[j].cy.n());
-            g.z = nf;
-            HB_LAUNCH("ll_down", ll_down_naive_kernel, g, kBlk, 0, s, at_frame(lb[j - 1], js - 1, fs, n0), at_frame(lb[j], js, fs, n0), p.f.levels, js,
-                      fs);
+            HB_LAUNCH("ll_down", ll_down_naive_kernel, grid_for(lb[j].sx.n(), lb[j].cy.n(), nf), kBlk, 0, s, at_frame(lb[j - 1], js - 1, fs, n0),
+                      at_frame(lb[j], js, fs, n0), p.f.levels, js, fs);
         });
     }
 }
@@ -407,112 +417,95 @@ void launch_up(P &p, int j, cudaStream_t s) {  // produce outGPyramid[j] (1 <= j
     for_frame_groups(p, [&](int n0, int nf) {
         if (fast_up && !top) {
             static const CUtensorMap no_map = {};
-            HB_LAUNCH("ll_up2", (nf > 1 ? ll_up2_kernel<false, false, true, false, true> : ll_up2_kernel<false, false, true, false, false>), up_grid(lb[j].ox.lo, lb[j].ox.hi, lb[j].coy.lo, lb[j].coy.hi, nf),
-                      256, up2_smem_bytes(false, false), s, scalars_frame(at_frame(p.f, fs, n0)), at_frame(lb[j], js, fs, n0),
-                      at_frame(lb[j + 1], js + 1, fs, n0), no_map, js, fs);
+            const auto kern = with_flags([](auto frames) { return ll_up2_kernel<false, false, true, false, frames>; }, nf > 1);
+            HB_LAUNCH("ll_up2", kern, up_grid(lb[j].ox.lo, lb[j].ox.hi, lb[j].coy.lo, lb[j].coy.hi, nf), 256, up2_smem_bytes(false, false), s,
+                      scalars_frame(at_frame(p.f, fs, n0)), at_frame(lb[j], js, fs, n0), at_frame(lb[j + 1], js + 1, fs, n0), no_map, js, fs);
         } else {
-            dim3 g = grid_for(lb[j].ox.n(), lb[j].coy.n());
-            g.z = nf;
             const int jc = top ? j : j + 1;
-            HB_LAUNCH("ll_up", ll_up_naive_kernel, g, kBlk, 0, s, at_frame(lb[j], js, fs, n0), at_frame(lb[jc], top ? js : js + 1, fs, n0),
-                      p.f.flm1, p.f.levels, top ? 1 : 0, js, fs);
+            HB_LAUNCH("ll_up", ll_up_naive_kernel, grid_for(lb[j].ox.n(), lb[j].coy.n(), nf), kBlk, 0, s, at_frame(lb[j], js, fs, n0),
+                      at_frame(lb[jc], top ? js : js + 1, fs, n0), p.f.flm1, p.f.levels, top ? 1 : 0, js, fs);
         }
     });
+}
+
+// The fast final kernel's form for a call (the forms from AlignedTma on also need the frame tile's map, per group of
+// frames).  Its ALIGNED path (32-bit addressing) moves one aligned word of two pixels per thread and channel, wb bytes, so
+// every pointer and element offset to such a word is a multiple of wb bytes.  Interleaved frames take it with fixed pitches:
+// the frame tile by TMA, and a pixel pair's output samples stored together as wb-byte words (so the output's base, row and
+// frame strides in bytes are multiples of wb, and both its columns and the input's start even).
+template<typename T>
+Form final_form(const PlanT<T> &p) {
+    const bool general = g_force_naive & 16, tile_tma = !(g_force_naive & 64);
+    const LLFrameT<T> &f = p.f;
+    const int64_t eb = sizeof(T), wb = 2 * eb;
+    if (p.il) {
+        const bool pairs = f.W % 2 == 0 && f.out_x0 % 2 == 0 && f.in_x0 % 2 == 0 && f.out_sy > 0 &&
+                           multiples_of(wb, f.out, f.out_sy * eb, p.fs.out * eb);
+        return pairs && !general && tile_tma ? il_form(p) : Form::GeneralIL;
+    }
+    const int64_t in_span = (int64_t)f.in_h * f.in_sy + 3 * f.in_sc, out_span = (int64_t)f.H * f.out_sy + 3 * f.out_sc;
+    const bool aligned = f.C == 3 && f.in_c0 == 0 && f.out_c0 == 0 && f.in_c >= 3 && f.in_sy > 0 && f.in_sc > 0 && f.out_sy > 0 &&
+                         f.out_sc > 0 && in_span < (1ll << 31) && out_span < (1ll << 31) &&
+                         multiples_of(wb, f.W * eb, f.out_x0 * eb, f.in_x0 * eb, f.in, f.out, f.in_sy * eb, f.in_sc * eb,
+                                      f.out_sy * eb, f.out_sc * eb, p.fs.in * eb, p.fs.out * eb);
+    return !aligned || general ? Form::General : tile_tma ? Form::AlignedTma : Form::Aligned;
+}
+
+// The final kernel's frame tile by TMA for the nf frames from `in`: false if the buffer breaks TMA's rules (16-byte aligned
+// base and strides) or a tile's first column would not start on a 16-byte boundary.  The map describes the input buffer
+// itself, (x, y, c), or (x, y) with x over an interleaved RGB frame's samples or an RGBA frame's 4-sample pixels, and the
+// group's frames as one more dimension if there are several: a tile reaching past it reads zeros, for pixels never stored.
+template<typename T>
+bool frame_tile_map(const PlanT<T> &p, const T *in, int nf, CUtensorMap *map) {
+    const LLFrameT<T> &f = p.f;
+    const int64_t eb = sizeof(T);
+    const int xs = p.il && p.fs.px_in == 3 ? 3 : 1;
+    uint64_t dims[4] = {(uint64_t)xs * f.in_w, (uint64_t)f.in_h};
+    uint32_t box[4] = {(uint32_t)(xs * up_in_w<T>()), kUpTH};
+    int64_t strides[3] = {f.in_sy * eb};
+    int rank = 2;
+    if (!p.il) dims[rank] = f.in_c, box[rank] = 3, strides[rank - 1] = f.in_sc * eb, rank++;
+    if (nf > 1) dims[rank] = nf, box[rank] = 1, strides[rank - 1] = p.fs.in * eb, rank++;
+    const CUtensorMapDataType dt = p.il && p.fs.px_in == 4 ? (eb == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_UINT64)
+                                                          : (eb == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16);
+    return tma::strides_ok(in, strides, rank - 1) && multiples_of(16, ((f.out_x0 & ~1) - f.in_x0) * eb) &&
+           tma::encode(map, dt, rank, (void *)in, dims, strides, box);
 }
 
 template<typename T>
 void launch_final(PlanT<T> &p, cudaStream_t s) {
     LevelBuf *lb = p.ls.lv;
-    if (fast_final(p)) {
-        const LLFrameT<T> &f = p.f;
-        // the common layout takes the kernel's ALIGNED path (32-bit addressing, one aligned word of two pixels per thread
-        // and channel: wb bytes, so every pointer and element offset to such a word is a multiple of wb bytes)
-        const int64_t eb = sizeof(T), wb = 2 * eb;
-        auto aw = [&](int64_t bytes) { return bytes % wb == 0; };
-        const int64_t in_span = (int64_t)f.in_h * f.in_sy + 3 * f.in_sc, out_span = (int64_t)f.H * f.out_sy + 3 * f.out_sc;
-        // (interleaved frames always take the general-layout path)
-        const bool aligned = !p.il && f.C == 3 && f.in_c0 == 0 && f.out_c0 == 0 && f.in_c >= 3 && aw(f.W * eb) && aw(f.out_x0 * eb) &&
-                             aw(f.in_x0 * eb) && aw((int64_t)(uintptr_t)f.in) && aw((int64_t)(uintptr_t)f.out) &&
-                             aw(f.in_sy * eb) && aw(f.in_sc * eb) && aw(f.out_sy * eb) && aw(f.out_sc * eb) &&
-                             aw(p.fs.in * eb) && aw(p.fs.out * eb) && f.in_sy > 0 && f.in_sc > 0 && f.out_sy > 0 &&
-                             f.out_sc > 0 && in_span < (1ll << 31) && out_span < (1ll << 31) && !(g_force_naive & 16);
-        // Interleaved RGB / RGBA frames of channels [0, 3) (RGB -> RGB, RGBA -> RGB, RGBA -> RGBA's channels [0, 3)) take
-        // the kernel's aligned form with fixed pitches: the frame tile by TMA (an RGBA input must describe its fourth
-        // channel: the tile reads whole pixels), a pixel pair's output samples stored together as wb-byte words (so the
-        // output's base, row and frame strides in bytes are multiples of wb, and both its columns and the input's start
-        // even).  Everything else interleaved takes the general-layout path.
-        const int pin = p.fs.px_in, pout = p.fs.px_out;
-        const bool il_fast = p.il && f.C == 3 && f.in_c0 == 0 && f.out_c0 == 0 && f.in_c == pin &&
-                             ((pin == 3 && pout == 3) || (pin == 4 && (pout == 3 || pout == 4))) && f.W % 2 == 0 &&
-                             f.out_x0 % 2 == 0 && f.in_x0 % 2 == 0 && aw((int64_t)(uintptr_t)f.out) && aw(f.out_sy * eb) &&
-                             aw(p.fs.out * eb) && f.out_sy > 0 && !(g_force_naive & 16) && !(g_force_naive & 64);
-        const bool beta1 = f.beta == 1.0f;
+    const LLFrameT<T> &f = p.f;
+    if (!fast_final(p)) {
         for_frame_groups(p, [&](int n0, int nf) {
-            const LLFrameT<T> fg = at_frame(f, p.fs, n0);
-            // frame tile by TMA when the buffer meets TMA's rules (16-byte aligned base and strides); the map describes
-            // the input buffer itself (x, y, c), and the group's frames as a fourth dimension when there are several, so a
-            // tile reaching past it reads zeros for pixels that are never stored
-            CUtensorMap in_map = {};
-            bool use_tma = false;
-            if (aligned && !(g_force_naive & 64)) {
-                const int rank = nf > 1 ? 4 : 3;
-                const int64_t strides[3] = {f.in_sy * eb, f.in_sc * eb, p.fs.in * eb};
-                // (every tile's first column must also start on a 16-byte boundary: crops at other even offsets take the
-                // load path; so do frame strides that are no 16-byte multiple)
-                if (tma::strides_ok(fg.in, strides, rank - 1) && (((f.out_x0 & ~1) - f.in_x0) * eb) % 16 == 0) {
-                    const uint64_t dims[4] = {(uint64_t)f.in_w, (uint64_t)f.in_h, (uint64_t)f.in_c, (uint64_t)nf};
-                    const uint32_t box[4] = {(uint32_t)up_in_w<T>(), kUpTH, 3, 1};
-                    use_tma = tma::encode(&in_map, sizeof(T) == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16, rank,
-                                          (void *)fg.in, dims, strides, box);
-                }
-            }
-            if (il_fast) {
-                const int rank = nf > 1 ? 3 : 2;
-                const int64_t strides[2] = {f.in_sy * eb, p.fs.in * eb};
-                if (tma::strides_ok(fg.in, strides, rank - 1) && (((f.out_x0 & ~1) - f.in_x0) * eb) % 16 == 0) {
-                    // RGB: x runs over samples (a box of 3 * up_in_w samples); RGBA: over pixels, one 4-sample element each
-                    const uint64_t dims[3] = {(uint64_t)(pin == 3 ? 3 * f.in_w : f.in_w), (uint64_t)f.in_h, (uint64_t)nf};
-                    const uint32_t box[3] = {(uint32_t)(pin == 3 ? 3 * up_in_w<T>() : up_in_w<T>()), kUpTH, 1};
-                    const CUtensorMapDataType dt = pin == 3 ? (sizeof(T) == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16)
-                                                            : (sizeof(T) == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_UINT64);
-                    use_tma = tma::encode(&in_map, dt, rank, (void *)fg.in, dims, strides, box);
-                }
-            }
-            auto launch = [&](auto kern, bool tma_on, int samples = 3) {
-                const int smem = up2_smem_bytes(true, tma_on, (int)sizeof(T), samples);
-                const dim3 g = up_grid(f.out_x0, f.out_x0 + f.W - 1, f.out_y0, f.out_y0 + f.H - 1, nf);
-                hb::allow_smem(kern, smem);
-                HB_LAUNCH("ll_final2", kern, g, 256, smem, s, fg, at_frame(lb[1], 1, p.fs, n0), at_frame(lb[2], 2, p.fs, n0), in_map, 1,
-                          p.fs);
-            };
-            auto pick = [&](auto frames) {
-                constexpr bool F = decltype(frames)::value;
-                if (p.il && use_tma) {
-                    if (pin == 3 && beta1) launch(ll_up2_kernel<true, true, true, true, F, T, 3, 3>, true, 3);
-                    else if (pin == 3) launch(ll_up2_kernel<true, true, false, true, F, T, 3, 3>, true, 3);
-                    else if (pout == 3 && beta1) launch(ll_up2_kernel<true, true, true, true, F, T, 4, 3>, true, 4);
-                    else if (pout == 3) launch(ll_up2_kernel<true, true, false, true, F, T, 4, 3>, true, 4);
-                    else if (beta1) launch(ll_up2_kernel<true, true, true, true, F, T, 4, 4>, true, 4);
-                    else launch(ll_up2_kernel<true, true, false, true, F, T, 4, 4>, true, 4);
-                } else if (use_tma && beta1) launch(ll_up2_kernel<true, true, true, true, F, T>, true);
-                else if (use_tma) launch(ll_up2_kernel<true, true, false, true, F, T>, true);
-                else if (aligned && beta1) launch(ll_up2_kernel<true, true, true, false, F, T>, false);
-                else if (aligned) launch(ll_up2_kernel<true, true, false, false, F, T>, false);
-                else if (p.il && beta1) launch(ll_up2_kernel<true, false, true, false, F, T, 0, 0>, false);
-                else if (p.il) launch(ll_up2_kernel<true, false, false, false, F, T, 0, 0>, false);
-                else if (beta1) launch(ll_up2_kernel<true, false, true, false, F, T>, false);
-                else launch(ll_up2_kernel<true, false, false, false, F, T>, false);
-            };
-            if (nf > 1) pick(std::true_type{});
-            else pick(std::false_type{});
+            HB_LAUNCH("ll_final", ll_final_naive_kernel<T>, grid_for(f.W, f.H, nf), kBlk, 0, s, at_frame(f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0),
+                      1, p.fs);
         });
-    } else {
-        for_frame_groups(p, [&](int n0, int nf) {
-            dim3 g = grid_for(p.f.W, p.f.H);
-            g.z = nf;
-            HB_LAUNCH("ll_final", ll_final_naive_kernel<T>, g, kBlk, 0, s, at_frame(p.f, p.fs, n0), at_frame(lb[1], 1, p.fs, n0), 1, p.fs);
-        });
+        return;
     }
+    const Form form = final_form(p);
+    for_frame_groups(p, [&](int n0, int nf) {
+        const LLFrameT<T> fg = at_frame(f, p.fs, n0);
+        CUtensorMap in_map = {};
+        Form g = form;
+        if (form >= Form::AlignedTma && !frame_tile_map(p, fg.in, nf, &in_map)) g = form == Form::AlignedTma ? Form::Aligned : Form::GeneralIL;
+        // (the kernels of one element type take the same parameters)
+        const auto kern = with_flags([&](auto beta1, auto frames) {
+            switch (g) {
+            case Form::General: return ll_up2_kernel<true, false, beta1, false, frames, T>;
+            case Form::GeneralIL: return ll_up2_kernel<true, false, beta1, false, frames, T, 0, 0>;
+            case Form::Aligned: return ll_up2_kernel<true, true, beta1, false, frames, T>;
+            case Form::AlignedTma: return ll_up2_kernel<true, true, beta1, true, frames, T>;
+            case Form::Rgb: return ll_up2_kernel<true, true, beta1, true, frames, T, 3, 3>;
+            case Form::RgbaToRgb: return ll_up2_kernel<true, true, beta1, true, frames, T, 4, 3>;
+            default: return ll_up2_kernel<true, true, beta1, true, frames, T, 4, 4>;  // Form::Rgba
+            }
+        }, f.beta == 1.0f, nf > 1);
+        const int smem = up2_smem_bytes(true, g >= Form::AlignedTma, (int)sizeof(T), g >= Form::RgbaToRgb ? 4 : 3);
+        hb::allow_smem(kern, smem);
+        HB_LAUNCH("ll_final2", kern, up_grid(f.out_x0, f.out_x0 + f.W - 1, f.out_y0, f.out_y0 + f.H - 1, nf), 256, smem, s, fg,
+                  at_frame(lb[1], 1, p.fs, n0), at_frame(lb[2], 2, p.fs, n0), in_map, 1, p.fs);
+    });
 }
 
 // Coarse tail in one cooperative launch: levels j0+1 .. J-1 down and up (see ll_coarse_fused_kernel).
@@ -524,9 +517,10 @@ bool launch_coarse_fused(P &p, int j0, cudaStream_t s) {
     LevelSet ls8;
     memcpy(ls8.lv, p.ls.lv, sizeof ls8.lv);
     const bool deep = p.J > ll::kMaxJ, frames = p.N > 1;
-    const void *kern = deep ? (frames ? (const void *)ll_coarse_fused_kernel<true, LevelSetDeep, LevelStridesDeep>
-                                      : (const void *)ll_coarse_fused_kernel<false, LevelSetDeep>)
-                            : (frames ? (const void *)ll_coarse_fused_kernel<true> : (const void *)ll_coarse_fused_kernel<false>);
+    const void *kern = with_flags([](auto D, auto F) {
+        return (const void *)ll_coarse_fused_kernel<F, std::conditional_t<D, LevelSetDeep, LevelSet>,
+                                                    std::conditional_t<D && F, LevelStridesDeep, FrameStrides>>;
+    }, deep, frames);
     const int max_blocks = std::min(hb::resident_blocks(kern, 256, 0), 2 * hb::sm_count());
     int J = p.J, K = p.f.levels, levels = p.f.levels, jd = fast_down(p) && j0 < 2 ? 2 : j0, nf = p.N;
     float flm1 = p.f.flm1;
@@ -580,23 +574,27 @@ void run_coarse_sweep(P &p, int from_level, cudaStream_t s) {
 // [0, 3), the unit's run of 8 * pitch samples (16-byte words, 8-byte ones for uint8 RGB), and for an RGBA output the word
 // of a pixel's R and G (an RGBA input must describe its fourth channel: the run covers whole pixels).
 template<typename T>
+Form tone_form(const PlanT<T> &p) {
+    const bool general = g_force_naive & 16;
+    const LLFrameT<T> &f = p.f;
+    const int pin = p.fs.px_in, pout = p.fs.px_out;
+    const int64_t eb = sizeof(T);
+    const T *in0 = f.in + (int64_t)(f.out_y0 - f.in_y0) * f.in_sy + (int64_t)(f.out_x0 - f.in_x0) * pin;
+    if (p.il) {
+        auto run_word = [&](int pitch) -> int64_t { return multiples_of(16, kTonePx * pitch * eb) ? 16 : 8; };
+        const int64_t ai = run_word(pin), ao = pout == 3 ? run_word(3) : 2 * eb;
+        const bool words = multiples_of(ai, in0, f.in_sy * eb, p.fs.in * eb) && multiples_of(ao, f.out, f.out_sy * eb, p.fs.out * eb);
+        return words && !general ? il_form(p) : Form::GeneralIL;
+    }
+    const bool vec = multiples_of(kTonePx * eb, in0, f.in_sy * eb, f.in_sc * eb, p.fs.in * eb, f.out, f.out_sy * eb, f.out_sc * eb, p.fs.out * eb);
+    return vec && !general ? Form::Aligned : Form::General;
+}
+
+template<typename T>
 void launch_tone(PlanT<T> &p, cudaStream_t s) {
     const LLFrameT<T> &f = p.f;
     const int upr = (f.W + kTonePx - 1) / kTonePx;
     const long long units = (long long)upr * f.H;
-    const int pin = p.fs.px_in, pout = p.fs.px_out;
-    const int64_t eb = sizeof(T);
-    auto al = [](int64_t bytes, int64_t a) { return bytes % a == 0; };
-    const T *in0 = f.in + (int64_t)(f.out_y0 - f.in_y0) * f.in_sy + (int64_t)(f.out_x0 - f.in_x0) * pin;
-    const int64_t in_b = (int64_t)(uintptr_t)in0, out_b = (int64_t)(uintptr_t)f.out;
-    const int64_t a = kTonePx * eb;
-    const bool vec = !p.il && al(in_b, a) && al(f.in_sy * eb, a) && al(f.in_sc * eb, a) && al(p.fs.in * eb, a) && al(out_b, a) &&
-                     al(f.out_sy * eb, a) && al(f.out_sc * eb, a) && al(p.fs.out * eb, a) && !(g_force_naive & 16);
-    auto run_word = [&](int pitch) -> int64_t { return kTonePx * pitch * eb % 16 == 0 ? 16 : 8; };
-    const int64_t ai = run_word(pin), ao = pout == 3 ? run_word(3) : 2 * eb;
-    const bool il_vec = p.il && f.C == 3 && f.in_c0 == 0 && f.out_c0 == 0 && f.in_c == pin &&
-                        ((pin == 3 && pout == 3) || (pin == 4 && (pout == 3 || pout == 4))) && al(in_b, ai) && al(f.in_sy * eb, ai) &&
-                        al(p.fs.in * eb, ai) && al(out_b, ao) && al(f.out_sy * eb, ao) && al(p.fs.out * eb, ao) && !(g_force_naive & 16);
     const size_t smem = (size_t)(2 * f.lut_half + 1) * sizeof(float);
     // the planar uint16 single-frame form: units counted in 64 bits, one launch
     auto launch1 = [&](auto kern) {
@@ -621,19 +619,19 @@ void launch_tone(PlanT<T> &p, cudaStream_t s) {
             }
         });
     };
+    const Form form = tone_form(p);
     if constexpr (std::is_same<T, uint16_t>::value) {
-        if (!p.il && p.N == 1) {
-            if (vec) launch1(ll_tone_kernel<true>);
-            else launch1(ll_tone_kernel<false>);
-            return;
-        }
+        if (!p.il && p.N == 1) return with_flags([&](auto vec) { launch1(ll_tone_kernel<vec>); }, form == Form::Aligned);
     }
-    if (il_vec && pin == 3) launch(ll_tone_kernel<true, T, 3, 3, true>);
-    else if (il_vec && pout == 3) launch(ll_tone_kernel<true, T, 4, 3, true>);
-    else if (il_vec) launch(ll_tone_kernel<true, T, 4, 4, true>);
-    else if (p.il) launch(ll_tone_kernel<false, T, 0, 0, true>);
-    else if (vec) launch(ll_tone_kernel<true, T, 1, 1, true>);
-    else launch(ll_tone_kernel<false, T, 1, 1, true>);
+    switch (form) {
+    case Form::General: return launch(ll_tone_kernel<false, T, 1, 1, true>);
+    case Form::Aligned: return launch(ll_tone_kernel<true, T, 1, 1, true>);
+    case Form::GeneralIL: return launch(ll_tone_kernel<false, T, 0, 0, true>);
+    case Form::Rgb: return launch(ll_tone_kernel<true, T, 3, 3, true>);
+    case Form::RgbaToRgb: return launch(ll_tone_kernel<true, T, 4, 3, true>);
+    case Form::Rgba: return launch(ll_tone_kernel<true, T, 4, 4, true>);
+    case Form::AlignedTma: break;  // (final kernel only)
+    }
 }
 
 // One GPU, args = {input, output} of 3 dimensions (one frame) or 4 (a batch of frames along dimension 3), elements T;
