@@ -15,9 +15,7 @@
 //     strips sized to fill the resident warps a whole number of times.
 //   * blur3x3_u16_kernel — any alignment: a lane owns 8 pixels, aligned 16-byte loads realigned by funnel shifts, the
 //     2-pixel horizontal apron from the neighbouring lane by shuffle.  Bound by the integer pipe.
-// halide_b200_blur_batch runs the same two kernels on every frame of a clip, in one launch (FR instances).
-#include <type_traits>
-
+// Both kernels walk the frames of a clip (halide_b200_blur_batch) in one launch; a one-frame call is a clip of one frame.
 #include "hb_common.h"
 
 namespace {
@@ -28,6 +26,8 @@ constexpr int kWarpsPerBlock = 4;
 int g_force_general = 0;  // test hook (halide_b200_blur_force_general): 1 = route aligned frames through the general kernel too,
                           // >= 8 = aligned kernel with this strip height (small test frames then reach its unclamped main loop)
 
+// The frames of a clip: frame 0's parameters, then the strides from one frame to the next and the number of frames.
+// in_lo and in_hi span the whole 3-D input allocation, relative to frame 0's `in`.
 struct BlurArgs {
     const uint16_t *in;   // element (in_x0, in_y0) of the input == the one feeding output (0,0)
     uint16_t *out;        // element at output mins
@@ -36,35 +36,17 @@ struct BlurArgs {
     int rows_per_warp;
     // valid element range of the input allocation relative to `in`, for guarding vector loads
     int64_t in_lo, in_hi;
-};
-// The parameters of the FR instances, which filter the frames of a clip: BlurArgs at the clip's first frame (in_lo and
-// in_hi span the whole 3-D input allocation, relative to frame 0's `in`), the strides from one frame to the next and the
-// number of frames.  (A separate type, so that the one-frame kernels keep their parameter block byte for byte: any field
-// appended to it changes their code.)
-struct BlurBatchArgs : BlurArgs {
     int64_t in_sn, out_sn;  // frame strides in elements (negative or, the input, zero too)
     int n;                  // frames
 };
-template<bool FR>
-using BlurArgsOf = std::conditional_t<FR, BlurBatchArgs, BlurArgs>;
 
 // Frame n's input offset, relative to `in` (every input offset the kernels form stays relative to frame 0's `in`, so the
-// allocation span guards frame n unchanged), its output, and the number of frames.  They read the parameter block and
-// never write it; in a one-frame instance they give its own pointers and 1 frame.
-template<bool FR>
-__device__ __forceinline__ int64_t frame_in_off(const BlurArgsOf<FR> &a, int n) {
-    if constexpr (FR) return (int64_t)n * a.in_sn;
-    else return 0;
+// allocation span guards frame n unchanged), and its output.  They read the parameter block and never write it.
+__device__ __forceinline__ int64_t frame_in_off(const BlurArgs &a, int n) {
+    return (int64_t)n * a.in_sn;
 }
-template<bool FR>
-__device__ __forceinline__ int frame_count(const BlurArgsOf<FR> &a) {
-    if constexpr (FR) return a.n;
-    else return 1;
-}
-template<bool FR>
-__device__ __forceinline__ uint16_t *frame_out(const BlurArgsOf<FR> &a, int n) {
-    if constexpr (FR) return a.out + (int64_t)n * a.out_sn;
-    else return a.out;
+__device__ __forceinline__ uint16_t *frame_out(const BlurArgs &a, int n) {
+    return a.out + (int64_t)n * a.out_sn;
 }
 
 __device__ __forceinline__ uint4 load_chunk(const uint16_t *p, int64_t off, int64_t lo, int64_t hi) {
@@ -145,11 +127,8 @@ __device__ __forceinline__ void blur_x_row(const RawRow &raw, int lane, uint32_t
     }
 }
 
-// FR: a clip, frames blockIdx.z, blockIdx.z + gridDim.z, ... (gridDim.z <= kMaxGridZ); the one-frame instance runs the
-// body once, for its frame.  (Written as one body rather than a frame loop around a device function: either of those
-// changed the one-frame instance's code.)
-template<bool FR = false>
-__global__ void __launch_bounds__(32 * kWarpsPerBlock) blur3x3_u16_kernel(BlurArgsOf<FR> a) {
+// Frames blockIdx.z, blockIdx.z + gridDim.z, ... (gridDim.z <= kMaxGridZ).
+__global__ void __launch_bounds__(32 * kWarpsPerBlock) blur3x3_u16_kernel(BlurArgs a) {
     int lane = threadIdx.x & 31;
     int warp = threadIdx.x >> 5;
     int x0 = blockIdx.x * kStripW;
@@ -157,9 +136,9 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) blur3x3_u16_kernel(BlurAr
     if (y0 >= a.h) return;
     int y1 = min(y0 + a.rows_per_warp, a.h);
 
-    int n = FR ? blockIdx.z : 0;
+    int n = blockIdx.z;
     do {
-        const int64_t fo = frame_in_off<FR>(a, n);
+        const int64_t fo = frame_in_off(a, n);
         uint32_t r0[8], r1[8], r2[8];
         blur_x_row(load_raw_row(a, fo + (int64_t)y0 * a.in_stride_y, x0, lane), lane, r0);
         blur_x_row(load_raw_row(a, fo + (int64_t)(y0 + 1) * a.in_stride_y, x0, lane), lane, r1);
@@ -172,7 +151,7 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) blur3x3_u16_kernel(BlurAr
             uint32_t o[8];
 #pragma unroll
             for (int i = 0; i < 8; i++) o[i] = ((r0[i] + r1[i] + r2[i]) & 0xffffu) / 3u;
-            uint16_t *dst = frame_out<FR>(a, n) + (int64_t)y * a.out_stride_y + xl;
+            uint16_t *dst = frame_out(a, n) + (int64_t)y * a.out_stride_y + xl;
             if (xl + 8 <= a.w && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
                 uint4 pk = make_uint4(o[0] | (o[1] << 16), o[2] | (o[3] << 16), o[4] | (o[5] << 16), o[6] | (o[7] << 16));
                 *reinterpret_cast<uint4 *>(dst) = pk;
@@ -185,8 +164,8 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) blur3x3_u16_kernel(BlurAr
 #pragma unroll
             for (int i = 0; i < 8; i++) { r0[i] = r1[i]; r1[i] = r2[i]; }
         }
-        if constexpr (FR) n += gridDim.z;
-    } while (FR && n < frame_count<FR>(a));
+        n += gridDim.z;
+    } while (n < a.n);
 }
 
 // ---- fast path: frames whose rows keep pixel pairs 4-byte aligned (even strides, aligned bases) ----------------------
@@ -313,21 +292,16 @@ struct QuadStrip {
 };
 
 // a.rows_per_warp = strip height; strips are numbered x-fastest so the warps of a block read adjacent spans of a row.
-// FR: a clip's strips, frame by frame: strip t is strip t mod `strips` of frame t / `strips`.
-template<int AHEAD, bool FR = false>
-__global__ void __launch_bounds__(32 * kQuadWarps) blur3x3_u16_quad_kernel(BlurArgsOf<FR> a, int strips_x, int strips) {
+// A clip's strips, frame by frame: strip t is strip t mod `strips` of frame t / `strips`.
+template<int AHEAD>
+__global__ void __launch_bounds__(32 * kQuadWarps) blur3x3_u16_quad_kernel(BlurArgs a, int strips_x, int strips) {
     const int lane = threadIdx.x & 31;
     int t = blockIdx.x * kQuadWarps + (threadIdx.x >> 5);
-    int n = 0;
-    if constexpr (FR) {
-        if (t >= strips * a.n) return;
-        n = t / strips;
-        t -= n * strips;
-    } else {
-        if (t >= strips) return;
-    }
-    const uint16_t *in = a.in + frame_in_off<FR>(a, n);
-    uint16_t *out = frame_out<FR>(a, n);
+    if (t >= strips * a.n) return;
+    const int n = t / strips;
+    t -= n * strips;
+    const uint16_t *in = a.in + frame_in_off(a, n);
+    uint16_t *out = frame_out(a, n);
     const int sx = t % strips_x, sy = t / strips_x;
     const int xw = sx * kQuadW, y0 = sy * a.rows_per_warp;
     const int y1 = min(y0 + a.rows_per_warp, a.h);
@@ -350,14 +324,13 @@ const halide_filter_argument_t kArgs[2] = {
 // The batch entry point: the same buffers with a third dimension, the frame index n.
 const halide_filter_argument_t kBatchArgs[2] = {hb::variant(kArgs[0], 1), hb::variant(kArgs[1], 1)};
 
-// The one launch of a frame (FR false) or of a clip (FR): the pair kernel when `pair_ok`, the general one otherwise.
-template<bool FR>
-void launch(BlurArgsOf<FR> &a, bool pair_ok, int frames, cudaStream_t s) {
-    const int w = a.w, h = a.h;
+// The one launch of a call: the pair kernel when `pair_ok`, the general one otherwise.
+void launch(BlurArgs &a, bool pair_ok, cudaStream_t s) {
+    const int w = a.w, h = a.h, frames = a.n;
     if (pair_ok) {
         // strips of 128 columns; height such that the strips of all frames fill the resident warps a whole number of times
         const int sxq = (w + kQuadW - 1) / kQuadW;
-        auto kernel = blur3x3_u16_quad_kernel<6, FR>;
+        auto kernel = blur3x3_u16_quad_kernel<6>;
         const int64_t slots = (int64_t)hb::resident_blocks(kernel, 32 * kQuadWarps, 0) * kQuadWarps;
         int qrows = 8;
         for (int m = 1; m <= 64; m++) {
@@ -383,7 +356,7 @@ void launch(BlurArgsOf<FR> &a, bool pair_ok, int frames, cudaStream_t s) {
         a.rows_per_warp = rows;
         int warps_y = (h + rows - 1) / rows;
         dim3 grid(strips_x, (warps_y + kWarpsPerBlock - 1) / kWarpsPerBlock, frames < hb::kMaxGridZ ? frames : hb::kMaxGridZ);
-        HB_LAUNCH("blur3x3_u16", blur3x3_u16_kernel<FR>, grid, 32 * kWarpsPerBlock, 0, s, a);
+        HB_LAUNCH("blur3x3_u16", blur3x3_u16_kernel, grid, 32 * kWarpsPerBlock, 0, s, a);
     }
 }
 
@@ -404,7 +377,7 @@ int run_blur(halide_buffer_t *input, halide_buffer_t *blur_y, const halide_filte
     if (w <= 0 || h <= 0 || N <= 0) return 0;
     if ((r = hb::acquire(args, 2))) return r;
 
-    BlurBatchArgs a;
+    BlurArgs a;
     const int64_t isy = input->dim[1].stride;
     const int64_t origin = (int64_t)(ox - input->dim[0].min) + (int64_t)(oy - input->dim[1].min) * isy + c.in_off;
     a.in = (const uint16_t *)args[0].dev + origin;
@@ -430,8 +403,7 @@ int run_blur(halide_buffer_t *input, halide_buffer_t *blur_y, const halide_filte
     cudaStream_t s = hb::stream();
     {
         hb::CallTimer timer(s);
-        if (c.clip) launch<true>(a, pair_ok, N, s);
-        else launch<false>(a, pair_ok, 1, s);
+        launch(a, pair_ok, s);
     }
     return hb::finish(args, 2, what);
 }

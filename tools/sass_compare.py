@@ -22,7 +22,9 @@ with no new one of its name is also matched by name and template arguments alone
 template argument `0` dropped on both sides (a plain function: by name alone): the template arguments fix the parameter
 types however they are spelled (nl_means's and bilateral_grid's kernels take theirs through an alias, which demangles as
 `std::conditional<...>::type`), and a std::enable_if choice between overloads adds that `0` (nl_means_window_kernel
-before it was one template).  Instruction addresses and padding are
+before it was one template).  An old frame-walking instance, `f<..., true>(` or `f<true>(`, is also matched by name and
+template arguments alone against the kernel without its `bool FR` parameter (blur3x3_u16_kernel and
+blur3x3_u16_quad_kernel<6>, which serve one frame and clips alike).  Instruction addresses and padding are
 dropped before comparing; opcodes, operands and encodings must match.  Prints each old kernel that is missing or differs, then a count; exits 1 if any.
 """
 import re
@@ -39,6 +41,9 @@ HEADS = [(re.compile(r"^void (.*)<float>\("), r"\1("), (re.compile(r"<float, "),
 # list (the first parenthesis that follows a name character: "(anonymous namespace)" precedes none)
 BARE = re.compile(r"(, 0)?>\(.*\)$")
 PLAIN = re.compile(r"(?<=\w)\(.*\)$")
+# an old frame-walking instance's last template argument, `bool FR = true` (a plain function without it also loses its
+# return type, as in HEADS)
+FR_TAILS = [(re.compile(r", true>\("), ">("), (re.compile(r"^void (.*)<true>\("), r"\1(")]
 
 
 def bare(name):
@@ -84,7 +89,10 @@ def main():
         by_bare.setdefault(bare(k), []).extend(vs)
     bad = 0
     for k, v in old.items():
-        cands = by_name.get(k) or by_bare.get(bare(k), [])
+        without_fr = k
+        for pat, repl in FR_TAILS:
+            without_fr = pat.sub(repl, without_fr, count=1)
+        cands = by_name.get(k) or by_bare.get(bare(k)) or by_bare.get(bare(without_fr), [])
         if not any(c == v for c in cands):
             print(("DIFFERS " if cands else "MISSING ") + k)
             bad += 1
